@@ -1,17 +1,18 @@
 #!/usr/bin/env python
-"""bench.py — decode tokens/sec (+ p50 TTFT) of the TGIS hot path on B200, per the driver contract.
+"""bench.py — decode tokens/sec (+ p50 TTFT) of the TGIS hot path on H100.
 
 A "step" = one pass of the hot path over one batch of synthetic input = one whole batched generation job:
 B concurrent requests x (512-token prompt -> 128 generated tokens), greedy, on synthetic seeded weights of the named
-architecture (BASELINE.json configs[1]: Llama-3-8B bf16, 1xB200, batch 32, 512-in/128-out).
+architecture (BASELINE.json configs[1]: Llama-3-8B bf16, 1xH100, batch 32, 512-in/128-out).
 
   value  : decode tokens/s with inputs resident in HBM — tokens sampled in pure-decode engine steps divided by the
            CUDA-event time of those steps (events on the engine's launching stream), max over ranks.
   e2e    : the same metric through the public C-ABI call with HOST buffers (tgis_engine_add_request /
            run_until_idle / poll): wall clock of the decode phase, i.e. including the per-step H2D metadata copy, the
            D2H result copy and the host scheduler.  Also reports whole-job output tokens/s and p50 TTFT.
-  roofline: dominant kernel = the tcgen05 GEMM; achieved = algorithmic bytes / CUDA-event time per launch, measured in
-           a separate short profiled pass (events around every GEMM launch), against MEASURED_PEAKS.json hbm_gbs;
+  roofline: dominant kernel = the wgmma GEMM; achieved = algorithmic bytes / CUDA-event time per launch, measured in
+           a separate short profiled pass (events around every GEMM launch), against the H100 SXM data-sheet HBM3
+           bandwidth (3.35 TB/s);
            decode_step_frac_of_hbm_roofline = algorithmic bytes of one decode step / measured step time / peak.
   cpu_baseline / --impl reference: the CPU oracle (oracle/llama_oracle.py — the port of the reference's vLLM-CPU path,
            which cannot be built offline; BASELINE.md §4) timed on the host cores on a bounded sample.
@@ -21,7 +22,12 @@ row-parallel o / down with the fused push all-reduce + residual + RMSNorm exchan
 the SAME workload as N = 1 -> "scaling": "strong"; `tp_parity` compares its greedy tokens with a single-GPU engine in
 the same run.  Secondary fields: `dp` (independent replicas, weak scaling: the faster way to use N GPUs for a model that
 fits one), `named_configs` (N = 4: BASELINE configs[3]; N = 8: configs[4], Llama-3-70B TP = 8, 256 requests),
-`vllm_gpu_baseline` (GPU vLLM 0.22.0 on the same pool, from profiles/).  --parallel dp restores the replicas-only run.
+--parallel dp restores the replicas-only run.
+
+--dump-outputs DIR: after the timed steps, the token ids the last timed step generated ([batch, gen_len] float64, rows in
+request order; rank 0's requests when N > 1) are written to DIR/tokens.npy.  They are the timed path's whole output: its
+requests ask for no logprobs (num_logprobs = 0), so the engine computes none.  Weights, prompts and
+sampling are seeded, so two builds given the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -67,6 +73,8 @@ def parse_args():
     ap.add_argument("--cpu-layers", type=int, default=8, help="layers timed by the CPU baseline (extrapolated)")
     ap.add_argument("--cpu-steps", type=int, default=20, help="decode steps of the ours-arm cpu_baseline leg")
     ap.add_argument("--cpu-budget-s", type=float, default=60.0, help="wall-clock bound of the CPU baseline sample")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's generated token ids to DIR/tokens.npy (rank 0)")
     return ap.parse_args()
 
 
@@ -78,14 +86,11 @@ def log(msg: str) -> None:
 
 
 def peaks() -> tuple[float, str]:
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "NVIDIA H100 SXM data sheet (HBM3, 700 W part); not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -285,34 +290,6 @@ def cpu_reference_opt(args, steps: int, warmup: int, budget_s: float | None = No
             "ttft_p50_est_ms": 1e3 * statistics.median(ttfts), "step_times_s": [round(t, 4) for t in times[:64]]}
 
 
-def ncu_traffic_per_launch(n_layers: int):
-    """DRAM bytes (read + write) per launch of the dominant kernel from the committed `ncu --set full` capture
-    (profiles/, produced by scripts/gpu_check.sh prof_gemm: the qkv, o, gate_up, down and lm_head launches of one decode
-    step at batch 32), weighted like the timed mix: n_layers x the four layer GEMMs + one lm_head."""
-    import csv
-    import glob
-    files = sorted(glob.glob(str(Path(__file__).resolve().parent / "profiles" / "r*_ncu_full_gemm_tcgen05.csv")))
-    if not files:
-        return None, None
-    try:
-        with open(files[-1]) as f:
-            rows = list(csv.DictReader(f))
-        def col(row, name):
-            for k, v in row.items():
-                if k.startswith(name):
-                    unit = k[k.index("[") + 1:k.index("]")] if "[" in k else "byte"
-                    mult = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[unit]
-                    return float(v) * mult
-            raise KeyError(name)
-        per = [col(r, "dram__bytes_read.sum") + col(r, "dram__bytes_write.sum") for r in rows]
-        if len(per) != 5:
-            return None, None
-        total = n_layers * sum(per[:4]) + per[4]
-        return total / (4 * n_layers + 1), f"{Path(files[-1]).name} (ncu --set full, cold-cache replay)"
-    except Exception:  # noqa: BLE001
-        return None, None
-
-
 def reduce_over_ranks(max_vals: list[float], sum_vals: list[float], device: str) -> tuple[list[float], list[float]]:
     """Whole-job aggregation for the N>1 (data-parallel replicas) path: times -> MAX over ranks, counts -> SUM.
     Works on any initialised torch.distributed backend (NCCL on the GPU box, gloo in tests/test_multirank_cpu.py)."""
@@ -328,7 +305,7 @@ def reduce_over_ranks(max_vals: list[float], sum_vals: list[float], device: str)
 
 
 # ----------------------------------------------------------------------------------------------------------- ours
-METRIC = "decode tokens/sec + p50 TTFT, 512-in/128-out batch, 1/2/4/8xB200 vs CPU ref"
+METRIC = "decode tokens/sec + p50 TTFT, 512-in/128-out batch, 1/2/4/8xH100 vs CPU ref"
 
 
 def _load_synthetic(eng, cfg, seed: int) -> None:
@@ -529,26 +506,13 @@ def _step_bytes(cfg, B: int, mean_ctx: float, tp: int) -> float:
     return (n_params * 2 + B * mean_ctx * kv_tok) / tp + B * cfg.vocab * 2
 
 
-def _vllm_baseline(model: str, batch: int):
-    """GPU vLLM 0.22.0 on the same pool (scripts/vllm_crosscheck.py bench; builder-run, committed under profiles/)."""
-    import glob
+def _dump_outputs(out_dir: str, leg: dict) -> None:
+    """What a caller of the timed path received in its last step: every request's generated token ids."""
+    import numpy as np
 
-    files = sorted(glob.glob(str(ROOT / "profiles" / "r*_vllm_baseline.json")))
-    if not files:
-        return None
-    try:
-        d = json.loads(Path(files[-1]).read_text())
-        if d["meta"]["model"] != model:
-            return None
-        for r in d["runs"]:
-            if r["batch"] == batch and r["prompt_len"] == 512 and r["gen_len"] == 128:
-                return {"decode_tokens_per_s": r["decode_tokens_per_s"], "decode_ms_per_step": r["decode_ms_per_step"],
-                        "job_output_tokens_per_s": r["job_output_tokens_per_s"],
-                        "prefill_burst_s": r["t_prefill_burst_s"], "vllm": d["meta"]["vllm"], "gpu": d["meta"]["gpu"],
-                        "source": f"profiles/{Path(files[-1]).name} (builder-run on this pool; not timed in this run)"}
-    except Exception:  # noqa: BLE001
-        return None
-    return None
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "tokens.npy", np.array(leg["tokens"], dtype=np.float64))
 
 
 def run_ours(args) -> dict | None:
@@ -603,6 +567,8 @@ def run_ours(args) -> dict | None:
         primary = _timed_jobs(eng, prompts, sp, args.warmup, args.steps, barrier_dp if tp == 1 else barrier_local, local,
                               "primary")
         log(f"timed region done: {args.steps} jobs in {primary['wall']:.3f}s")
+        if args.dump_outputs and rank == 0:
+            _dump_outputs(args.dump_outputs, primary)
         prof = _profiled_pass(eng, prompts)
         log(f"profiled pass done: {prof['gemm_calls']} GEMM launches, {prof['gemm_ms']:.2f} ms")
         if named_b:   # BASELINE configs[3]: 8B TP=4, 128 concurrent requests, mixed prompt lengths, continuous batching
@@ -661,8 +627,7 @@ def run_ours(args) -> dict | None:
                               "generated is scored by a single-GPU engine given the same prefix (prompt-logprob pass): it "
                               "must be that engine's argmax or lose to it by a few bf16 ulps of the logits (0.031 at |x| in "
                               "[4, 8)).  free_running: the two greedy continuations part ways at the first such near-tie -- "
-                              "on this synthetic checkpoint a quarter of all steps are <= 1-ulp races (vLLM diverges from "
-                              "itself the same way, profiles/r02_vllm_crosscheck.json)"}
+                              "on this synthetic checkpoint many steps are <= 1-ulp races"}
         # (b) BASELINE configs[4]: Llama-3-70B TP=8, 256 concurrent requests
         if do_cfg4:
             B70 = 256
@@ -712,7 +677,6 @@ def run_ours(args) -> dict | None:
     step_ms = primary["dec_ms"] / max(primary["dec_steps"], 1)
     gemm_ms, gemm_bytes, gemm_calls = prof["gemm_ms"], prof["gemm_bytes"], prof["gemm_calls"]
     achieved = gemm_bytes / (gemm_ms * 1e-3) / 1e9 if gemm_ms > 0 else None
-    traffic, traffic_src = ncu_traffic_per_launch(cfg.n_layers) if args.model == "llama3-8b" and tp == 1 else (None, None)
     ttft_p50 = 1e3 * statistics.median(primary["ttfts"])
     out = {
         "metric": METRIC,
@@ -746,14 +710,12 @@ def run_ours(args) -> dict | None:
         "graph_launches": int(primary["graph_launches"]),
         "clocks": primary["clocks"],
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": (achieved / peak) if achieved else None, "traffic": traffic, "traffic_source": traffic_src,
-                     "peak_source": peak_src,
-                     "kernel": "gemm_bf16_tcgen05_kernel", "launches_timed": int(gemm_calls),
+                     "frac": (achieved / peak) if achieved else None, "peak_source": peak_src,
+                     "kernel": "gemm_bf16_wgmma_kernel", "launches_timed": int(gemm_calls),
                      "algorithmic_bytes_per_launch": gemm_bytes / max(gemm_calls, 1),
                      "avg_launch_us": 1e3 * gemm_ms / max(gemm_calls, 1),
                      "decode_step_ms": step_ms, "decode_step_algorithmic_bytes": bytes_step,
                      "decode_step_frac_of_hbm_roofline": bytes_step / (step_ms * 1e-3) / 1e9 / peak if step_ms else None},
-        "vllm_gpu_baseline": _vllm_baseline(args.model, B),
     }
     if tp > 1:
         out["roofline"]["exchange_ms_per_step"] = prof["exchange_ms"] / max(prof["decode_steps"], 1)
@@ -767,6 +729,10 @@ def run_ours(args) -> dict | None:
 
 def main():
     args = parse_args()
+    if args.dump_outputs and args.steps < 1:
+        raise SystemExit("--dump-outputs needs at least one timed step")
+    if args.dump_outputs and args.impl == "reference":
+        raise SystemExit("--dump-outputs writes the GPU engine's outputs; --impl reference has none")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.impl == "reference":
@@ -792,11 +758,6 @@ def main():
     out = run_ours(args)
     if out is None:
         return
-    try:  # keep the GPU numbers even if the CPU baseline leg is cut short by a timeout
-        (ROOT / "gpurun_out").mkdir(exist_ok=True)
-        (ROOT / "gpurun_out" / "bench_ours_partial.json").write_text(json.dumps(out))
-    except OSError:
-        pass
     if not args.no_cpu_baseline:   # rank 0, every N
         ref = cpu_reference(args, steps=args.cpu_steps, warmup=3, budget_s=args.cpu_budget_s)
         out["cpu_baseline"] = {k: ref[k] for k in ("value", "unit", "cores", "kind", "sample", "ttft_p50_est_ms")}

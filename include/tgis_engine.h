@@ -1,5 +1,5 @@
 /*
- * tgis_engine.h — C ABI of libtgis_engine.so, the B200-native continuous-batching engine that replaces the
+ * tgis_engine.h — C ABI of libtgis_engine.so, the H100-native continuous-batching engine that replaces the
  * vLLM AsyncLLMEngine behind the TGIS gRPC adapter's generation path.
  *
  * Drop-in boundary (SURVEY.md §8b).  The reference has no FFI; its seam is the `EngineClient` object that
@@ -27,7 +27,7 @@
  * tgis_last_error() returns a thread-local message valid until the next call on the same thread.  The caller owns
  * input buffers until the call returns (the engine copies).  One dedicated engine thread per process runs the step
  * loop (scheduler + kernel launches); all entry points are thread-safe enqueue/dequeue operations.
- * There is NO CPU fallback: tgis_engine_create fails if no sm_100 device is present.
+ * There is NO CPU fallback: tgis_engine_create fails if no sm_90 (H100) device is present.
  */
 #ifndef TGIS_ENGINE_H_
 #define TGIS_ENGINE_H_
@@ -180,7 +180,7 @@ typedef struct tgis_status {
   int64_t decode_tokens;     /* tokens sampled in pure-decode steps */
   int64_t h2d_bytes;         /* per-step metadata shipped host->device, cumulative */
   int64_t d2h_bytes;         /* per-step result records read back, cumulative */
-  double gemm_ms;            /* with profiling on: summed CUDA-event time of every tcgen05 GEMM launch */
+  double gemm_ms;            /* with profiling on: summed CUDA-event time of every wgmma GEMM launch */
   double gemm_bytes;         /* ... and their algorithmic bytes (weights + activations in + result out) */
   int64_t gemm_calls;
   int64_t graph_launches;    /* decode steps replayed from a captured CUDA graph */

@@ -1,5 +1,5 @@
 /*
- * tgis_kernels.h — C ABI test hooks of libtgis_engine.so: each sm_100a kernel of the hot path callable on raw device
+ * tgis_kernels.h — C ABI test hooks of libtgis_engine.so: each sm_90a kernel of the hot path callable on raw device
  * pointers, so the parity tests (tests/ -m gpu) can compare every kernel with the CPU oracle through the same shared
  * library the server loads.  All pointers marked "dev" are device memory; metadata arrays are HOST memory and are
  * staged internally.  Every call synchronises before returning; 0 = ok, <0 = error (tgis_last_error()).
@@ -21,7 +21,7 @@ extern "C" {
 #endif
 
 /* y[T,N] = x[T,K] . w[N,K]^T ; y is bf16 (out_f32 = 0) or fp32 (out_f32 = 1, the lm_head logits path);
- * impl 0 = tcgen05 kernel, 1 = SIMT cross-check kernel.  x must have >= 256 rows
+ * impl 0 = wgmma kernel, 1 = SIMT cross-check kernel.  x must have >= 256 rows
  * allocated (TMA box height) or T rows when impl == 1. */
 int tgis_k_gemm(const void* x_dev, const void* w_dev, void* y_dev, int32_t T, int32_t N, int32_t K, int32_t x_rows_alloc,
                 int32_t impl, int32_t iters, float* ms_out, int32_t out_f32);

@@ -26,7 +26,7 @@ def one(src: str) -> Path:
 
 with concurrent.futures.ThreadPoolExecutor(8) as ex:
     objs = list(ex.map(one, b.SOURCES))
-r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(lib), *map(str, objs),
+r = subprocess.run([nvcc, "-shared", *b.ARCH, "-o", str(lib), *map(str, objs),
                     "-Xcompiler", "-pthread", "-cudart", "static", "-lrt", "-ldl"], capture_output=True, text=True)
 if r.returncode != 0:
     raise SystemExit(r.stderr)

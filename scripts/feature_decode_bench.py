@@ -1,5 +1,5 @@
 """Engine-level cost of the two late round-2 features on the BASELINE configs[1] shape (Llama-3-8B dims, 32 requests,
-512-in / 64-out, greedy, one B200): device-timed decode ms per step (tgis_status.gpu_decode_ms / decode_steps) for
+512-in / 64-out, greedy, one H100): device-timed decode ms per step (tgis_status.gpu_decode_ms / decode_steps) for
   base    : no adapter, no grammar (the fused production path, CUDA-graph decode steps)
   lora    : every request on ONE rank-16 adapter over all seven projections (unfused projections + lora.cu, graphs)
   lora4   : the requests spread over FOUR adapters (mixed-adapter token tiles)

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM through the C ABI on Llama-3-8B decode / prefill shapes.
+"""Micro-benchmark of the wgmma GEMM through the C ABI on Llama-3-8B decode / prefill shapes.
 Weights are rotated over several distinct buffers so every launch streams from HBM, not L2."""
 import ctypes as C
 import json

@@ -22,7 +22,6 @@ for st in $STAGES; do
     bench_gpu) timeout 600 python bench.py --no-cpu-baseline > gpurun_out/bench_gpu.log 2> gpurun_out/bench_gpu.err; echo "bench_gpu rc=$?" ;;
     bench_ref) timeout 400 python bench.py --impl reference --steps 1 --warmup 1 > gpurun_out/bench_ref.log 2> gpurun_out/bench_ref.err; echo "bench_ref rc=$?" ;;
     prof_list) timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv python scripts/profile_decode.py 4 32 512 6 0 > gpurun_out/prof_list.log 2>&1; echo "prof_list rc=$?" ;;
-    prof_gemm) timeout 900 ncu --set full --clock-control none --import-source on -k regex:gemm_bf16_tcgen05 -s 13 -c 5 -f -o gpurun_out/prof_gemm python scripts/profile_decode.py 2 32 512 4 0 > gpurun_out/prof_gemm.log 2>&1; echo "prof_gemm rc=$?" ;;
     prof_attn) timeout 900 ncu --set full --clock-control none --import-source on -k regex:attn_decode -s 2 -c 2 -f -o gpurun_out/prof_attn python scripts/profile_decode.py 2 32 512 4 0 > gpurun_out/prof_attn.log 2>&1; echo "prof_attn rc=$?" ;;
     decode_quick) for pdl in 0 1; do for gr in 0 1; do TGIS_PDL=$pdl timeout 300 python scripts/profile_decode.py 8 32 512 24 $gr > gpurun_out/decode_pdl${pdl}_graph${gr}.log 2>&1; done; done; echo "decode_quick rc=$?" ;;
     tp2) timeout 600 python -m torch.distributed.run --nnodes=1 --nproc-per-node=2 --master-addr 127.0.0.1 --master-port 29511 scripts/tp_check.py tiny > gpurun_out/tp2.log 2>&1; echo "tp2 rc=$?"; timeout 600 python -m torch.distributed.run --nnodes=1 --nproc-per-node=2 --master-addr 127.0.0.1 --master-port 29512 scripts/tp_check.py tiny > gpurun_out/tp2_b.log 2>&1; echo "tp2 small rc=$?" ;;

@@ -12,7 +12,7 @@ run() {  # name, kernel regex, skip, count, command...
   rm -f gpurun_out/ncu/$name.ncu-rep
 }
 # decode step of a 2-layer 8B-shaped model, batch 32, context 512 (graphs off: ncu profiles plain launches)
-run gemm_decode  "tcgen05_kernel<32>"   9 9  python scripts/profile_decode.py 2 32 512 4 0
+run gemm_decode  "wgmma_kernel<32>"     9 9  python scripts/profile_decode.py 2 32 512 4 0
 run attn_decode  "attn_decode"          2 2  python scripts/profile_decode.py 2 32 512 4 0
 run norm         "rmsnorm_kernel"       10 2 python scripts/profile_decode.py 2 32 512 4 0
 run sampler_greedy "tgis_sampler"       1 1  python scripts/profile_decode.py 2 32 512 4 0

@@ -70,7 +70,6 @@ def launch_list(src: Path, out_agg: Path, out_raw: Path) -> None:
 
 
 launch_list(SRC / "launches.csv", DST / f"{tag}_launches_decode_step_summary.csv", DST / f"{tag}_launches_decode_step.csv")
-ncu_raw(SRC / "prof_gemm.ncu-rep", DST / f"{tag}_ncu_full_gemm_tcgen05.csv")
 ncu_raw(SRC / "prof_attn.ncu-rep", DST / f"{tag}_ncu_full_attn_decode.csv")
 ncu_raw(SRC / "prof_gemm_prefill.ncu-rep", DST / f"{tag}_ncu_full_gemm_prefill.csv")
 for name in ("bench.log", "bench_ref.log", "parity_stats.json", "gemm_bench.json", "gemm_cta_sweep.json", "gemm_timeline.log",

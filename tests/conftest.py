@@ -11,7 +11,7 @@ for _p in (str(ROOT), str(ROOT / "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a; run with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

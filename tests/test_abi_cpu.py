@@ -94,28 +94,29 @@ def test_decode_work_items_host_logic():
 
 
 def test_gemm_launch_plan_host_logic():
-    """Pure host arithmetic of the GEMM launcher (gemm_tcgen05.cu): for the decode shapes of the 8B and 70B/TP8 layer
+    """Pure host arithmetic of the GEMM launcher (gemm_wgmma.cu): for the decode shapes of the 8B and 70B/TP8 layer
     stacks the plan must (a) never use more CTAs than SMs (the stream-K fix-up and the chain kernel rely on co-residency),
     (b) in even-split mode give every CTA a k-range inside ONE tile (the cluster epilogue reduces exactly one unit per
-    CTA), and (c) cover the (tile, k-block) space exactly once."""
+    CTA), and (c) cover the (tile, k-block) space exactly once.  132 SMs = H100 SXM; 148 keeps a second SM count in play
+    (the split factors of qkv / o / down differ between the two)."""
     lib = _lib.load_library()
-    sms = 148
     shapes = [(6144, 4096), (4096, 4096), (28672, 4096), (4096, 14336), (128256, 4096),      # Llama-3-8B
               (1280, 8192), (8192, 1024), (7168, 8192), (8192, 3584)]                        # 70B / TP8 shards
-    for T in (1, 16, 32, 64, 128, 256):
-        for N, K in shapes:
-            bt, grid, split = C.c_int32(), C.c_int32(), C.c_int32()
-            assert lib.tgis_k_gemm_plan(T, N, K, sms, C.byref(bt), C.byref(grid), C.byref(split)) == 0
-            bt, grid, split = bt.value, grid.value, split.value
-            assert bt >= T and bt in (16, 32, 64, 128, 256)
-            assert 1 <= grid <= sms
-            unit = lib.tgis_k_gemm_unit_rows(T)       # 128; 256 with the TGIS_GEMM_NW=2 experiment
-            assert unit in (128, 256)
-            n_tiles, kb = (N + unit - 1) // unit, (K + 63) // 64
-            total = n_tiles * kb
-            bounds = [total * c // grid for c in range(grid + 1)]
-            assert bounds[0] == 0 and bounds[-1] == total and all(b1 > b0 for b0, b1 in zip(bounds, bounds[1:]))
-            if split:
-                assert 2 <= split and grid == n_tiles * split
-                for c in range(grid):
-                    assert bounds[c] // kb == (bounds[c + 1] - 1) // kb == c // split     # one unit, in tile c // split
+    for sms in (132, 148):
+        for T in (1, 16, 32, 64, 128, 256):
+            for N, K in shapes:
+                bt, grid, split = C.c_int32(), C.c_int32(), C.c_int32()
+                assert lib.tgis_k_gemm_plan(T, N, K, sms, C.byref(bt), C.byref(grid), C.byref(split)) == 0
+                bt, grid, split = bt.value, grid.value, split.value
+                assert bt >= T and bt in (16, 32, 64, 128, 256)
+                assert 1 <= grid <= sms
+                unit = lib.tgis_k_gemm_unit_rows(T)       # 128; 256 with the TGIS_GEMM_NW=2 experiment
+                assert unit in (128, 256)
+                n_tiles, kb = (N + unit - 1) // unit, (K + 63) // 64
+                total = n_tiles * kb
+                bounds = [total * c // grid for c in range(grid + 1)]
+                assert bounds[0] == 0 and bounds[-1] == total and all(b1 > b0 for b0, b1 in zip(bounds, bounds[1:]))
+                if split:
+                    assert 2 <= split and grid == n_tiles * split
+                    for c in range(grid):
+                        assert bounds[c] // kb == (bounds[c + 1] - 1) // kb == c // split     # one unit, in tile c // split

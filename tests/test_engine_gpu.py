@@ -13,7 +13,7 @@ pytestmark = pytest.mark.gpu
 
 
 def _record_stats(name, stats):
-    """Parity statistics are kept as evidence (copied into profiles/ by hand after a GPU run)."""
+    """Parity statistics are kept as evidence of a GPU run."""
     import json
     import os
 
@@ -206,7 +206,7 @@ def test_prompt_logprobs_match_oracle(chunk):
 @pytest.mark.parametrize("model", ["tiny", "small"])
 def test_fused_rope_epilogue_is_bit_identical(model, monkeypatch):
     """Decode-shaped steps apply RoPE and scatter K/V into the paged cache inside the qkv GEMM's cluster epilogue
-    (gemm_tcgen05.cu) instead of running rope_kvwrite_kernel; same arithmetic and rounding points, so tokens AND logprobs
+    (gemm_wgmma.cu) instead of running rope_kvwrite_kernel; same arithmetic and rounding points, so tokens AND logprobs
     of a mixed prefill/decode run (incl. preemption-free chunked prefill below 256 tokens per step) must be bit-identical
     with TGIS_FUSE_ROPE=0 and =1."""
     from vllm_tgis_adapter_b200.engine.core import make_sampling_params

@@ -60,6 +60,42 @@ def test_gemm_fp32_output_for_logits(g):
     assert float((y - ref).abs().max()) < 2e-5 * float(ref.abs().max()) + 1e-5
 
 
+_NW2_CHILD = """
+import sys
+sys.path[:0] = [sys.argv[1], sys.argv[1] + "/tests"]
+import torch
+import tgis_gpu_utils as g
+assert g.lib().tgis_k_gemm_unit_rows(32) == 256 and g.lib().tgis_k_gemm_unit_rows(200) == 128
+for T, N, K in [(7, 256, 512), (16, 384, 4096), (32, 6144, 4096), (33, 1000, 520), (64, 4096, 14336), (128, 1024, 4096)]:
+    gen = torch.Generator(device="cuda").manual_seed(T * 7 + N + K)
+    x = (torch.randn(T, K, generator=gen, device="cuda") * 0.5).bfloat16()
+    w = (torch.randn(N, K, generator=gen, device="cuda") * 0.05).bfloat16()
+    y, _ = g.gemm(x, w)
+    ref = x.float() @ w.float().t()
+    ulp = g.bf16_ulp_diff(y, ref.bfloat16())
+    bad = (ulp > 1.01) & ((y.float() - ref).abs() > 1e-3 * ref.abs().mean())
+    assert int(bad.sum()) == 0, (T, N, K, float(ulp.max()))
+    assert float((ulp == 0).float().mean()) > 0.97, (T, N, K)
+    assert torch.equal(y, g.gemm(x, w)[0])
+print("NW2_OK")
+"""
+
+
+def test_gemm_two_weight_tiles_per_unit_experiment():
+    """TGIS_GEMM_NW=2 (off by default; read once per process, hence a child process): launches of at most 128 tokens
+    share one activation tile between two weight tiles (two accumulators per consumer thread).  Same tolerance as
+    test_gemm_tcgen05_matches_fp32_reference, bit-deterministic; larger token tiles keep one weight tile per unit."""
+    import os
+    import subprocess
+    import sys
+    from pathlib import Path
+
+    root = str(Path(__file__).resolve().parent.parent)
+    r = subprocess.run([sys.executable, "-c", _NW2_CHILD, root], env=dict(os.environ, TGIS_GEMM_NW="2"),
+                       capture_output=True, text=True, timeout=600)
+    assert "NW2_OK" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
+
+
 @pytest.mark.parametrize("T,F,K", [(32, 1536, 512), (7, 14336, 4096), (300, 1024, 256)])
 def test_gemm_fused_swiglu_epilogue(g, T, F, K):
     """gate_up GEMM with SwiGLU fused in the epilogue (rows interleaved gate_j, up_j) == GEMM -> bf16 -> silu*mul."""
@@ -181,11 +217,11 @@ def test_rope_and_kv_scatter_bit_exact(g):
 @pytest.mark.parametrize("heads", [(24, 4), (32, 8)])
 @pytest.mark.parametrize("T", [32, 200])
 def test_qkv_gemm_with_fused_rope_epilogue_is_bit_identical(g, T, heads):
-    """The qkv projection's split-tile reduction (gemm_tcgen05.cu) followed in the same kernel by RoPE + scatter into the
+    """The qkv projection's split-tile reduction (gemm_wgmma.cu) followed in the same kernel by RoPE + scatter into the
     paged K / V layouts, against the unfused pair (GEMM -> bf16 qkv, then rope_kvwrite_kernel): qkv rows and both caches
-    must be bit-identical.  32 heads = 32 weight tiles split 4 ways = clusters of 4 (reduction through distributed
-    shared memory); 48 heads (the Llama-3-8B shape) = 48 tiles split 3 ways, whose 48 clusters do not fit a 148-SM part
-    at once, so that shape takes the global-memory fix-up path."""
+    must be bit-identical.  32 heads = 32 weight tiles, 48 heads (the Llama-3-8B shape) = 48 tiles, each split over a
+    cluster (reduction through distributed shared memory) or, where the clusters do not all fit the GPU at once, through
+    the global-memory fix-up.  T = 200 (one 256-token tile over 16 k-blocks) is not split: the test skips there."""
     import ctypes as C
 
     (n_q, n_kv), K = heads, 1024

@@ -122,7 +122,7 @@ def _vllm_request_sets(vocab):
 
 @pytest.mark.parametrize("name,top_logit", [("opt-tiny", 1.0), ("opt-125m", 2.0)])
 def test_opt_oracle_matches_vllm_fixture(name, top_logit):
-    """The OPT oracle against the reference's REAL engine path: vLLM 0.22.0 (its own OPTForCausalLM, FlashInfer) on a B200
+    """The OPT oracle against the reference's REAL engine path: vLLM 0.22.0 (its own OPTForCausalLM, FlashInfer) on a GPU
     over the same seeded checkpoint and requests (tests/golden/vllm_<name>.json, scripts/vllm_crosscheck.py check --configs
     opt-tiny opt-125m).  Teacher-forced on vLLM's tokens, in bf16 ulps of the logits, like the Llama fixtures."""
     import math

@@ -150,11 +150,11 @@ def test_check_stop_order():
 
 @pytest.mark.parametrize("name,top_logit", [("tiny", 1.0), ("small", 2.0)])
 def test_llama_oracle_matches_vllm_fixture(name, top_logit):
-    """The oracle against what the reference's REAL engine path produced: vLLM 0.22.0 on a B200 running the same seeded
+    """The oracle against what the reference's REAL engine path produced: vLLM 0.22.0 on a GPU running the same seeded
     checkpoint and requests (tests/golden/vllm_<name>.json, written by scripts/vllm_crosscheck.py on the GPU box).
     Teacher-forced on vLLM's tokens: logprobs within 2 bf16 ulps of the logits (mean < 0.6 ulp), greedy argmax equal
     wherever vLLM's own top-2 margin exceeds 2 ulps, prompt-token ranks within the tie band.  (vLLM against itself --
-    one batch vs one request at a time -- differs by up to 1 ulp on the 8B-dim stack: profiles/r02_vllm_crosscheck.json.)"""
+    one batch vs one request at a time -- differs by up to 1 ulp on the 8B-dim stack.)"""
     import math
 
     fx = json.loads((GOLD / f"vllm_{name}.json").read_text())

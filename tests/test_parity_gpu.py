@@ -5,14 +5,14 @@
     (repetition penalty + ExpDecay length penalty + typical-p sampling, seeded -> compared through the Philox restatement);
   * mixed prompt lengths 64..512 with a KV cache too small for them (forced preemption + recompute) -- configs[3] shape;
   * a real `tgis_engine_abort` mid-generation on the threaded engine (reference call sites grpc_server.py:292,388);
-  * engine vs tests/golden/vllm_<cfg>.json: token ids / logprobs / ranks that vLLM itself produced on this pool's B200
+  * engine vs tests/golden/vllm_<cfg>.json: token ids / logprobs / ranks that vLLM itself produced on a GPU
     for the same synthetic checkpoints and request sets (scripts/vllm_crosscheck.py).
 
 The oracle is evaluated with torch ops on the CUDA device here (same code as on the CPU; oracle/llama_oracle.py
 `device=`): the 8B-dim shapes are minutes of CPU time.  Tolerances are stated in bf16 ulps of the logits: the logits ARE
 bf16 numbers (vLLM's lm_head rounds to the model dtype), so a logit that lands on the other side of a rounding boundary
 moves a logprob by one ulp (0.0156 at |x| in [2,4), 0.031 in [4,8)) -- the reference's own batch-composition noise has
-exactly this size (DESIGN.md section 5, profiles/r02_vllm_crosscheck.json).
+exactly this size (DESIGN.md section 5).
 """
 import dataclasses
 import json
@@ -234,7 +234,7 @@ def test_8b_dims_mixed_lengths_with_forced_preemption():
     # measured: 11 of 16 requests identical, 83 % matching prefix with ONE preemption -- on this synthetic checkpoint a
     # quarter of the greedy steps have a top-2 margin of <= 1 bf16 ulp of the logits (N(0, 1.3) logits over a 128k
     # vocabulary), so any change of summation order flips a token within a few steps (vLLM against itself, batched vs
-    # one request at a time, diverges the same way: profiles/r02_vllm_crosscheck.json)
+    # one request at a time, diverges the same way)
     assert prefix >= 0.6 * n_new * len(prompts), prefix
 
 
@@ -306,7 +306,7 @@ _TOP_LOGIT = {"tiny": 1.0, "small": 2.0, "8b2l": 4.0}
 
 @pytest.mark.parametrize("name", ["tiny", "small", "8b2l"])
 def test_engine_matches_vllm_fixture(name):
-    """Engine vs what vLLM 0.22.0 produced on a B200 for the same checkpoint and requests (tests/golden/vllm_<name>.json,
+    """Engine vs what vLLM 0.22.0 produced on a GPU for the same checkpoint and requests (tests/golden/vllm_<name>.json,
     scripts/vllm_crosscheck.py).  Greedy token ids must agree up to the first step where vLLM's own top-2 logprob
     margin is within 2 bf16 ulps; logprobs within 3 ulps of the logits, ranks equal off ties."""
     from vllm_tgis_adapter_b200.engine.core import make_sampling_params

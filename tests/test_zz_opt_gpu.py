@@ -92,7 +92,7 @@ def test_opt_embed_kernel_is_exact():
 
 # ---------------------------------------------------------------------------------------------------- engine
 def _record(name, stats):
-    """Parity statistics kept as evidence (copied into profiles/ after a GPU run)."""
+    """Parity statistics kept as evidence of a GPU run."""
     import json
     import os
 
@@ -259,7 +259,7 @@ def test_opt_engine_refuses_what_it_does_not_implement():
 
 @pytest.mark.parametrize("name,top_logit", [("opt-tiny", 1.0), ("opt-125m", 2.0)])
 def test_opt_engine_matches_vllm_fixture(name, top_logit):
-    """Engine (C ABI) vs what vLLM 0.22.0's own OPT implementation produced on a B200 for the same seeded checkpoint and
+    """Engine (C ABI) vs what vLLM 0.22.0's own OPT implementation produced on a GPU for the same seeded checkpoint and
     requests (tests/golden/vllm_<name>.json from scripts/vllm_crosscheck.py check --configs opt-tiny opt-125m): vLLM's
     greedy continuations scored by the engine's prompt-logprob pass (every step compared, teacher-forced), vLLM's prompt
     logprobs, and the free-running greedy prefix.  In bf16 ulps of the logits, like the Llama fixtures."""

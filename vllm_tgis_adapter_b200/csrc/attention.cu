@@ -513,10 +513,9 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
   const long long max_flat = (long long)max_entries * n_kv;
   const int grid = (int)std::min<long long>((long long)TGIS_DEC_MINB * num_sms, (max_flat + DEC_WARPS - 1) / DEC_WARPS);
   // split merge: the PDL-chained attn_merge_kernel (default), or inside the streaming kernel by the last-arriving warp
-  // (TGIS_ATTN_INKERNEL_MERGE=1, bit-identical).  Measured (profiles/r02_step_timeline_*): folding the merge saves its
-  // launch (-100 us per step at batch 32) but the o-proj GEMM that follows then loses the window in which it prefetched
-  // its weights next to the small merge kernel (attention CTAs fill the SM's shared memory): +140 us on the GEMM, net
-  // -1 % at batch 64.  So the separate kernel stays the default.
+  // (TGIS_ATTN_INKERNEL_MERGE=1, bit-identical).  Folding the merge saves its launch, but the o-proj GEMM that follows
+  // then loses the window in which it prefetched its weights next to the small merge kernel (attention CTAs fill the
+  // SM's shared memory).  The separate kernel is the default.
   const char* env_merge = getenv("TGIS_ATTN_INKERNEL_MERGE");  // read per launch: the A/B test flips it in-process
   const int inkernel = (env_merge && env_merge[0] == '1') ? 1 : 0;
   const char* env_pre = getenv("TGIS_ATTN_PREFETCH");  // 0: no cache reads before the grid-dependency wait

@@ -1,6 +1,6 @@
-"""Build libtgis_engine.so in-tree with nvcc for sm_100a (no torch extension machinery, no JIT cache).
+"""Build libtgis_engine.so in-tree with nvcc for sm_90a (H100) (no torch extension machinery, no JIT cache).
 
-The .so lands in vllm_tgis_adapter_b200/lib/ so it travels to the GPU box with the repo snapshot.
+The .so lands in vllm_tgis_adapter_b200/lib/, next to the package, so the package imports from the source tree.
 """
 from __future__ import annotations
 
@@ -16,13 +16,14 @@ PKG = CSRC.parent
 LIB_DIR = PKG / "lib"
 OBJ_DIR = CSRC / "build"
 LIB_PATH = LIB_DIR / "libtgis_engine.so"
-SOURCES = ["gemm_tcgen05.cu", "gemm_ref.cu", "elementwise.cu", "attention.cu", "sampler.cu", "lora.cu", "opt.cu", "engine.cu", "test_api.cu"]
+SOURCES = ["gemm_wgmma.cu", "gemm_ref.cu", "elementwise.cu", "attention.cu", "sampler.cu", "lora.cu", "opt.cu", "engine.cu", "test_api.cu"]
 HEADERS = ["ptx.cuh", "launch.cuh", "kernels.h", "../../include/tgis_engine.h", "../../include/tgis_kernels.h"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-pthread",
-    # bounded mbarrier spins: a pipeline-protocol bug traps (sticky CUDA error) instead of hanging the GPU box
+    # bounded mbarrier spins: a pipeline-protocol bug traps (sticky CUDA error) instead of hanging the GPU
     "-DTGIS_MBAR_TIMEOUT=1",
 ]
 
@@ -77,7 +78,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
 
     with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB_PATH), *map(str, objs),
+    link = [nvcc, "-shared", *ARCH, "-o", str(LIB_PATH), *map(str, objs),
             "-Xcompiler", "-pthread", "-cudart", "static", "-lrt", "-ldl"]
     r = subprocess.run(link, capture_output=True, text=True)
     if r.returncode != 0:

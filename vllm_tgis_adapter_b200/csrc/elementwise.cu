@@ -529,7 +529,7 @@ cudaError_t logits_push_launch(const void* shard, void* dst_peer0, int R, int Vl
   if (R <= 0) return cudaSuccess;
   if (Vl_bytes % 16 || V_bytes % 16 || col_bytes % 16) return cudaErrorInvalidValue;
   const size_t total = (size_t)R * (Vl_bytes / 16);
-  const int grid = (int)std::min<size_t>(148 * 2, (total + 255) / 256);
+  const int grid = (int)std::min<size_t>(132 * 2, (total + 255) / 256);
   return launch_k(logits_push_kernel, dim3(grid), dim3(256), 0, stream, (const uint4*)shard, (uint4*)dst_peer0, R,
                   Vl_bytes / 16, V_bytes / 16, col_bytes / 16, remote_flag, local_counter, epoch_base, epoch_idx);
 }
@@ -567,7 +567,7 @@ cudaError_t silu_mul_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, in
   if (ffn % 8 != 0) return cudaErrorInvalidValue;
   const long long total = (long long)T * (ffn / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   return launch_k(silu_mul_kernel, dim3((int)blocks), dim3(256), 0, stream, gate_up, act, T, ffn);
 }
 

@@ -1,12 +1,12 @@
 // libtgis_engine.so — continuous-batching engine + C ABI (include/tgis_engine.h).
 //
-// This is the B200-native replacement for what sits behind `self.engine.generate(...)`
+// This is the H100-native replacement for what sits behind `self.engine.generate(...)`
 // (/root/reference/src/vllm_tgis_adapter/grpc/grpc_server.py:222): vLLM's EngineCore busy loop, scheduler,
 // KV block manager, GPUModelRunner and Sampler (SURVEY.md §2.2 K1-K15, §3.2 "THE HOT LOOP").
 //
 //   host side (this file, C++): request queues, paged-KV block allocator, continuous-batching scheduler with chunked
 //       prefill + recompute preemption, stop checks (vllm v1/core/sched/utils.py:94-130), output ring.
-//   device side: one flat token batch per step -> Llama layer stack built from the sm_100a kernels in this directory.
+//   device side: one flat token batch per step -> Llama layer stack built from the sm_90a kernels in this directory.
 //       All per-step metadata is packed into ONE pinned staging buffer and shipped with ONE H2D copy; results come
 //       back with ONE D2H copy of SampleOut records.
 #include <algorithm>
@@ -204,7 +204,7 @@ int bt_index(int T) {
 
 struct tgis_engine {
   tgis_config cfg{};
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int q_dim = 0, qkv_dim = 0, bt_stride = 0, max_splits_cap = 0, bitmap_words = 0;
@@ -313,7 +313,7 @@ struct tgis_engine {
   int rope_fuse_max_t = 32;
   int rope_fuse_cluster_max_t = 256;
   // residual add + RMSNorm folded into the o / down projections' cluster reduction and the gate_up / qkv projections'
-  // operand staging (GemmNorm, gemm_tcgen05.cu): tp == 1, steps of at most GEMM_NORM_MAX_T tokens.  TGIS_FUSE_NORM=0: off
+  // operand staging (GemmNorm, gemm_wgmma.cu): tp == 1, steps of at most GEMM_NORM_MAX_T tokens.  TGIS_FUSE_NORM=0: off
   bool fuse_norm = false;
   // tensor parallelism, decode-shaped steps: one-shot all-reduce + residual + RMSNorm over NVLink peer memory
   // (ar_add_rmsnorm_kernel) instead of ncclAllReduce + rmsnorm kernel.  TGIS_TP_FUSED_AR=0: NCCL baseline.
@@ -412,8 +412,9 @@ struct tgis_engine {
     CK(cudaSetDevice(c.device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, c.device));
-    if (prop.major != 10) throw CudaError("tgis_engine requires an sm_100 (B200) device; found sm_" +
-                                          std::to_string(prop.major) + std::to_string(prop.minor));
+    if (prop.major != 9 || prop.minor != 0)
+      throw CudaError("tgis_engine requires an sm_90 (H100) device; found sm_" + std::to_string(prop.major) +
+                      std::to_string(prop.minor));
     num_sms = prop.multiProcessorCount;
     CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     CK(cudaEventCreate(&ev0));
@@ -1063,7 +1064,7 @@ struct tgis_engine {
 
   // ------------------------------------------------------------------------------------------------ device step
   // next_wm / nT,nN,nK describe the GEMM that follows this one in the layer stack: its first weight boxes are
-  // prefetched into L2 by this launch's producer warp (gemm_tcgen05.cu)
+  // prefetched into L2 by this launch's producer warp (gemm_wgmma.cu)
   void gemm(const CUtensorMap* xmaps, const CUtensorMap& wm, const bf16* X, const bf16* W, void* Y, int T, int N, int K,
             int out_f32 = 0, const CUtensorMap* next_wm = nullptr, int nT = 0, int nN = 0, int nK = 0, int ldy = 0,
             const GemmRope* rope = nullptr, const GemmNorm* norm = nullptr) {
@@ -1139,8 +1140,8 @@ struct tgis_engine {
     const bool ar_fused = exchange_mode(T) != 0;
     // RoPE + KV-cache scatter fused into the qkv GEMM's split-tile reduction (decode-shaped steps where every weight
     // tile is split over several CTAs; TGIS_FUSE_ROPE=0: off)
-    // (measured: -2 % per step at 32 tokens, but +2...5 % at 64...256 -- the last-arriving CTA's serial tail grows with
-    // T while the stand-alone kernel spreads over all SMs -- hence the token limit)
+    // (the last-arriving CTA's serial tail grows with T while the stand-alone kernel spreads over all SMs -- hence the
+    // token limit)
     // ... unless the qkv launch reduces its split tiles on chip (cluster mode): then the epilogue is spread over the
     // cluster's CTAs by token and the fusion pays up to 256 tokens (TGIS_FUSE_ROPE_CLUSTER_MAX_T)
     const int qkv_cluster = cfg.debug_gemm_ref ? 0 : gemm_cluster_split(T, qkv_dim, H, num_sms);
@@ -1286,7 +1287,7 @@ struct tgis_engine {
     CK(stl_marker_launch(22, stream));  // timeline builds: step end (after the result copy)
   }
 
-  // OPT layer stack (vllm model_executor/models/opt.py:170-197, do_layer_norm_before): the tcgen05 GEMMs write their fp32
+  // OPT layer stack (vllm model_executor/models/opt.py:170-197, do_layer_norm_before): the wgmma GEMMs write their fp32
   // accumulators (out mode 1) and the kernels of opt.cu add the bias before the single rounding to bf16; the paged
   // attention kernels run unchanged on zero-padded 128-dim heads with the model's softmax scale.  Per layer:
   //   LN1 [+ previous fc2 bias/residual] -> qkv GEMM -> bias + KV scatter -> attention -> out_proj GEMM ->
@@ -1367,7 +1368,7 @@ struct tgis_engine {
       gemm(xm_last, m_lm, last_hidden.p, lm_head, logits_shard.p, rows, Vl, H, lm_mode);
       NK(nccl().AllGather(logits_shard.p, logits_gather.p, (size_t)rows * Vl * lsz, ncclInt8, comm, stream));
       if (rank == 0) {
-        CK(launch_k(gather_relayout_kernel, dim3(148 * 4), dim3(256), 0, stream, (const uint4*)logits_gather.p,
+        CK(launch_k(gather_relayout_kernel, dim3(num_sms * 4), dim3(256), 0, stream, (const uint4*)logits_gather.p,
                     (uint4*)logits.p, rows, (int)(Vl * lsz / 16), tp));
         ++n_launches;
       }

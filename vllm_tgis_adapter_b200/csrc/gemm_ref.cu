@@ -1,4 +1,4 @@
-// Debug-only SIMT GEMM used by tests to cross-check the tcgen05 kernel on the device (never on the product path).
+// Debug-only SIMT GEMM used by tests to cross-check the wgmma kernel on the device (never on the product path).
 #include "kernels.h"
 
 namespace tgis {

@@ -1,4 +1,4 @@
-// Internal launcher declarations for the sm_100a kernels of the TGIS decode/prefill hot path.
+// Internal launcher declarations for the sm_90a kernels of the TGIS decode/prefill hot path.
 // (Internal C++ header; the drop-in C ABI is include/tgis_engine.h.)
 #pragma once
 #include <cuda.h>
@@ -9,7 +9,7 @@
 
 namespace tgis {
 
-// ---- gemm_tcgen05.cu --------------------------------------------------------------------------------------------
+// ---- gemm_wgmma.cu ---------------------------------------------------------------------------------------------
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                       uint32_t box_rows, uint32_t box_cols);
 int gemm_pick_bt(int T);
@@ -265,7 +265,7 @@ constexpr int SAMPLE_FORCED = 32;  // token = seed_lo is given (prompt logprobs)
 // top-k / top-p / race) -> 8 CTAs per row; otherwise the cluster size shrinks with the row count (sampler_cluster_size).
 cudaError_t sampler_launch(const void* logits, int logits_bf16, int ld, int vocab, const SampleRow* rows, int n_rows,
                            const uint32_t* seen_bitmap, int bitmap_words, float* scratch, SampleOut* out,
-                           cudaStream_t stream, int any_complex = 1, int num_sms = 148,
+                           cudaStream_t stream, int any_complex = 1, int num_sms = 132,
                            const uint32_t* allow_bitmap = nullptr /* [slots][bitmap_words], rows flagged SAMPLE_MASKED */);
 int sampler_cluster_size(int n_rows, int any_complex, int num_sms);
 // seen-token bitmap maintenance

@@ -31,7 +31,7 @@ namespace tgis {
 namespace {
 
 // 8 consecutive bf16 values as fp32 through ONE 16-byte load (an aggregate of eight __nv_bfloat16 read element-wise compiles
-// to eight 2-byte loads: the first version of these kernels ran 10x slower for exactly that reason, profiles/r02_ncu_lora.csv)
+// to eight 2-byte loads)
 struct F8 {
   float v[8];
 };
@@ -279,7 +279,7 @@ lora_expand_kernel(const float* __restrict__ v, const int32_t* __restrict__ tok_
 }
 
 // gate_up [T, 2F] with interleaved columns (2j = gate_j, 2j+1 = up_j) -> act [T, F]; the rounding points of the GEMM's
-// fused SwiGLU epilogue (gemm_tcgen05.cu swiglu_bf16) and of silu_mul_kernel
+// fused SwiGLU epilogue (gemm_wgmma.cu swiglu_bf16) and of silu_mul_kernel
 __global__ void silu_mul_interleaved_kernel(const __nv_bfloat16* __restrict__ gate_up, __nv_bfloat16* __restrict__ act,
                                             int T, int ffn) {
   griddep_launch();
@@ -343,7 +343,7 @@ cudaError_t silu_mul_interleaved_launch(const __nv_bfloat16* gate_up, __nv_bfloa
   if (ffn % 4 != 0) return cudaErrorInvalidValue;
   const long long total = (long long)T * (ffn / 4);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   return launch_k(silu_mul_interleaved_kernel, dim3((int)blocks), dim3(256), 0, stream, gate_up, act, T, ffn);
 }
 

@@ -2,13 +2,13 @@
 // facebook/opt-125m, /root/reference/tests/conftest.py:79-91 (no --model: vLLM's default, facebook/opt-125m) and tests/test_hub.py:17).  The GEMMs, the paged attention kernels, the lm_head and
 // the sampler are the Llama path's; what OPT adds is
 //   * learned position embeddings with offset 2                    vllm model_executor/models/opt.py:61-70, :268-290
-//   * biased projections: the tcgen05 GEMM hands over its fp32 accumulators and the bias is added BEFORE the single
+//   * biased projections: the wgmma GEMM hands over its fp32 accumulators and the bias is added BEFORE the single
 //     rounding to bf16 (F.linear(x, W, b) in the model dtype; cuBLASLt's bias epilogue)        opt.py:92-101, :150-165
 //   * ReLU (exact on bf16)                                                                      opt.py:156
 //   * LayerNorm with affine weight + bias (torch.nn.LayerNorm: fp32 mean, biased variance, one rounding)  opt.py:148,166
 // Rounding points are those of oracle/opt_oracle.py, which is pinned to transformers' OPTForCausalLM.
 // HBM-bound, every byte touched once: 16-byte vector accesses, a row per CTA for the reductions, grid-stride over
-// 148 x 8 CTAs for the plain elementwise pass.  All launched with PDL (launch.cuh).
+// num_sms x 8 CTAs for the plain elementwise pass.  All launched with PDL (launch.cuh).
 #include <algorithm>
 
 #include "kernels.h"
@@ -31,9 +31,8 @@ __device__ __forceinline__ float wsum(float v) {
 
 // Row geometry by hidden size: THREADS threads x NVEC 16-byte vectors each.  The per-thread state (row values in fp32, the
 // affine parameters, the projection bias) lives in registers, so NVEC is as small as the row allows: the 8192-wide
-// instantiation needs 117 registers (2 CTAs of 256 threads per SM), the <= 2048-wide ones 40.  Measured on the first version
-// (one 256 x 4 instantiation for every width, profiles/r02_ncu_opt_v1.csv): a 2048-row prefill chunk of opt-125m
-// (hidden 768: 96 of 256 threads busy, seven waves of CTAs) took 17.3 us for 15.7 MB.
+// instantiation needs 117 registers (2 CTAs of 256 threads per SM), the <= 2048-wide ones 40.  One 256 x 4 instantiation
+// for every width would leave 160 of 256 threads idle at hidden 768 (opt-125m) and need seven waves of CTAs.
 template <int THREADS>
 __device__ __forceinline__ float bsum(float v, float* red) {
   v = wsum(v);

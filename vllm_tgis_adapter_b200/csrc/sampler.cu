@@ -13,7 +13,7 @@
 // 50-100 instructions per element, which is ISSUE bound on one SM (1 ms per row).  So a row is owned by a thread-block
 // CLUSTER of 8 CTAs x 1024 threads on 8 SMs: each CTA scans one eighth of the vocabulary, block results are exchanged
 // through distributed shared memory and combined in rank order (deterministic).  The fp32 row (512 KiB) is read from
-// HBM once and stays in the 126 MB L2 for the selection passes (radix-select thresholds instead of the reference's
+// HBM once and stays in the 50 MB L2 for the selection passes (radix-select thresholds instead of the reference's
 // full sorts).  Loads are 16-byte vectorised and coalesced.
 #include <cooperative_groups.h>
 
@@ -762,9 +762,8 @@ int sampler_cluster_size(int n_rows, int any_complex, int num_sms) {
     const int v = atoi(e);
     if (v == 1 || v == 2 || v == 4 || v == 8) return v;
   }
-  // one wave of clusters over the GPU: the largest power of two with n_rows * ncl <= #SMs.  Measured for sampling rows too
-  // (profiles/r02_sampler_bench.json: 64 configs[2] rows 403 us with 8 CTAs per row = 4 waves of resident clusters, 256 us
-  // with 2; 32 rows 241 vs 137 us with 4), so the rule does not depend on the row type any more.
+  // one wave of clusters over the GPU: the largest power of two with n_rows * ncl <= #SMs, for sampling rows too (more
+  // CTAs per row than that means several waves of resident clusters).
   (void)any_complex;
   int ncl = 8;
   while (ncl > 1 && n_rows * ncl > num_sms) ncl >>= 1;

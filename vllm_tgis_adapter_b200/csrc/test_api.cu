@@ -27,7 +27,7 @@ int kfail(const std::string& m) {
   } while (0)
 
 int test_num_sms() {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;
@@ -92,7 +92,7 @@ int tgis_k_gemm(const void* x_dev, const void* w_dev, void* y_dev, int32_t T, in
       KCK(gemm_bf16_ref_launch((const bf16*)x_dev, K, (const bf16*)w_dev, y_dev, out_f32 == 2 ? N / 2 : N, T, N, K, st, out_f32));
     KCK(cudaEventRecord(e1, st));
   } else {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     KCK(cudaGetDevice(&dev));
     KCK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     CUtensorMap wm, xm;
@@ -139,7 +139,7 @@ int tgis_k_opt_layernorm(const void* acc_dev, const void* acc_bias_dev, void* re
 }
 
 int tgis_k_opt_bias_act(const void* acc_dev, const void* bias_dev, void* out_dev, int32_t T, int32_t N, int32_t relu) {
-  KCK(opt_bias_act_launch((const float*)acc_dev, N, (const bf16*)bias_dev, (bf16*)out_dev, N, T, N, relu, 148, 0));
+  KCK(opt_bias_act_launch((const float*)acc_dev, N, (const bf16*)bias_dev, (bf16*)out_dev, N, T, N, relu, test_num_sms(), 0));
   KCK(cudaDeviceSynchronize());
   return 0;
 }
@@ -426,11 +426,11 @@ int tgis_k_sampler_masked(const void* logits_dev, int32_t logits_bf16, int32_t l
   KCK(cudaEventCreate(&e0));
   KCK(cudaEventCreate(&e1));
   if (iters > 1)  // warm-up launch outside the timed region
-    KCK(sampler_launch(logits_dev, logits_bf16, ld, vocab, rows.p, n_rows, bm, words, scratch.p, outs.p, 0, any_complex, 148,
+    KCK(sampler_launch(logits_dev, logits_bf16, ld, vocab, rows.p, n_rows, bm, words, scratch.p, outs.p, 0, any_complex, test_num_sms(),
                        (const uint32_t*)allow_bitmap_dev));
   KCK(cudaEventRecord(e0, 0));
   for (int it = 0; it < iters; ++it)
-    KCK(sampler_launch(logits_dev, logits_bf16, ld, vocab, rows.p, n_rows, bm, words, scratch.p, outs.p, 0, any_complex, 148,
+    KCK(sampler_launch(logits_dev, logits_bf16, ld, vocab, rows.p, n_rows, bm, words, scratch.p, outs.p, 0, any_complex, test_num_sms(),
                        (const uint32_t*)allow_bitmap_dev));
   KCK(cudaEventRecord(e1, 0));
   KCK(cudaMemcpy(out_host, outs.p, sizeof(SampleOut) * n_rows, cudaMemcpyDeviceToHost));

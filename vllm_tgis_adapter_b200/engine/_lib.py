@@ -103,7 +103,7 @@ def load_library() -> C.CDLL:
         if have_nvcc() or not path.exists():
             build(force=bool(os.environ.get("TGIS_FORCE_BUILD")))
     if not path.exists():
-        raise RuntimeError(f"{path} is missing and could not be built: the TGIS B200 engine has no fallback path")
+        raise RuntimeError(f"{path} is missing and could not be built: the TGIS engine has no fallback path")
     lib = C.CDLL(str(path))
     vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
     lib.tgis_last_error.restype = C.c_char_p

@@ -1,4 +1,4 @@
-"""`fmaas.GenerationService` servicer on top of the B200-native engine.
+"""`fmaas.GenerationService` servicer on top of the H100-native engine.
 
 Behavioural mirror of /root/reference/src/vllm_tgis_adapter/grpc/grpc_server.py (same RPC surface, same parameter
 mapping, same stop-reason / token-info conversion, same error strings and status codes) with the engine call

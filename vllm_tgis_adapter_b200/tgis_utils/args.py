@@ -142,7 +142,7 @@ def postprocess_tgis_args(args: argparse.Namespace) -> argparse.Namespace:
             raise ValueError("Inconsistent dtype and dtype_str arg values")
         args.dtype = args.dtype_str
     if args.quantize:
-        raise ValueError("quantized checkpoints are not supported by the B200 bf16 engine")
+        raise ValueError("quantized checkpoints are not supported by the bf16 engine")
     if args.num_gpus is not None or args.num_shard is not None:
         if args.num_gpus is not None and args.num_shard is not None and args.num_gpus != args.num_shard:
             raise ValueError("Inconsistent num_gpus and num_shard arg values")
