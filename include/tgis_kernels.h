@@ -21,7 +21,8 @@ extern "C" {
 #endif
 
 /* y[T,N] = x[T,K] . w[N,K]^T ; y is bf16 (out_f32 = 0) or fp32 (out_f32 = 1, the lm_head logits path);
- * impl 0 = wgmma kernel, 1 = SIMT cross-check kernel.  x must have >= 256 rows
+ * impl 0 = wgmma kernel, 1 = SIMT cross-check kernel, 2 = wgmma kernel without the lean decode instantiation (always
+ * one CTA per SM; same results bit for bit).  x must have >= 256 rows
  * allocated (TMA box height) or T rows when impl == 1. */
 int tgis_k_gemm(const void* x_dev, const void* w_dev, void* y_dev, int32_t T, int32_t N, int32_t K, int32_t x_rows_alloc,
                 int32_t impl, int32_t iters, float* ms_out, int32_t out_f32);
@@ -62,6 +63,8 @@ int tgis_k_gemm_plan(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* 
                      int32_t* even_split_out);
 /* weight rows per GEMM unit for a T-token launch (128 x weight tiles per shared activation tile) */
 int tgis_k_gemm_unit_rows(int32_t T);
+/* CTAs per SM of the GEMM instantiation a T-token launch runs (lean = 0: the one-CTA-per-SM instantiation) */
+int tgis_k_gemm_blocks_per_sm(int32_t T, int32_t lean, int32_t* out);
 /* host-only: the decode work-item list of a step (csrc/kernels.h DecItem: q_row, kv_len, seq | split << 16, 0,
  * blocks[4]); record 0 holds the entry count; entries are listed longest first */
 int tgis_k_decode_items(const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_stride,

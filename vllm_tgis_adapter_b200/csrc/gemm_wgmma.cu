@@ -43,8 +43,18 @@ constexpr int GEMM_THREADS_NORM = GEMM_THREADS + 64;  // + 2 activation-transfor
 // NW = weight tiles (of GEMM_BN = 128 rows) per unit that share ONE activation tile: every unit re-reads its [BT x 64]
 // activation tile per k-block, and with NW = 2 that tile feeds two MMAs (two accumulators), halving the activation bytes
 // per weight byte.  An experiment (TGIS_GEMM_NW=2, see gemm_nw()): NW = 1 is what runs.
-template <int BT, int NW>
+//
+// LEAN = the decode instantiation (token tiles of at most GEMM_LEAN_MAX_T rows, NW = 1, no fused-norm warps, no push
+// variant of the cluster reduction): a GEMM_LEAN_STAGES-deep ring and at most 96 registers per thread (ptxas' cap for two
+// 288-thread CTAs), so TWO CTAs fit one SM (2 x (104 KB + 1 KB reserved) <= 228 KB of shared memory).  The grid still
+// holds at most one CTA per SM; the second slot is for the NEXT GEMM of the chain, whose CTAs become resident as soon as
+// this one triggers its dependents and fill their rings while this one drains (with one CTA per SM nothing of the next
+// launch could be resident until this one's CTA on that SM had exited).
+constexpr int GEMM_LEAN_MAX_T = 32;
+constexpr int GEMM_LEAN_STAGES = 5;
+template <int BT, int NW, bool LEAN = false>
 struct GemmCfg {
+  static_assert(!LEAN || (BT <= GEMM_LEAN_MAX_T && NW == 1), "lean instantiation: decode token tiles, one weight tile");
   static constexpr int W_TILE_BYTES = GEMM_BN * GEMM_BK * 2;
   static constexpr int W_BYTES = NW * W_TILE_BYTES;
   static constexpr int X_BYTES = BT * GEMM_BK * 2;
@@ -56,13 +66,18 @@ struct GemmCfg {
 #ifndef TGIS_GEMM_DECODE_STAGES
 #define TGIS_GEMM_DECODE_STAGES 8
 #endif
-  static constexpr int STAGES_CAP = BT <= 64 ? TGIS_GEMM_DECODE_STAGES : 12;
+  static constexpr int STAGES_CAP = LEAN ? GEMM_LEAN_STAGES : BT <= 64 ? TGIS_GEMM_DECODE_STAGES : 12;
   static constexpr int STAGES = STAGES_RAW > STAGES_CAP ? STAGES_CAP : STAGES_RAW;
   static constexpr int PART_FLOATS = NW * BT * GEMM_BN;                  // fp32 partial of one unit
   static constexpr int BAR_BYTES = 512;   // mbarriers (full, empty, ready, xfull), flag
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + BAR_BYTES + 256 /*rstd*/;
   // fused-norm consumers append the norm weights (+ K * 2 bytes, K <= 8192)
-  static constexpr int SMEM_MAX = (SMEM_BYTES + 16384) < 227 * 1024 ? (SMEM_BYTES + 16384) : 227 * 1024;
+  static constexpr int SMEM_MAX =
+      LEAN ? SMEM_BYTES : (SMEM_BYTES + 16384) < 227 * 1024 ? (SMEM_BYTES + 16384) : 227 * 1024;
+  static constexpr int THREADS = !LEAN && BT <= GEMM_NORM_MAX_T ? GEMM_THREADS_NORM : GEMM_THREADS;  // launch bound
+  static constexpr int MIN_BLOCKS = LEAN ? 2 : 1;
+  static_assert(!LEAN || 2 * (SMEM_BYTES + 1024) <= 228 * 1024, "two lean CTAs must fit one SM's shared memory");
+  static_assert(!LEAN || PART_FLOATS * 4 <= STAGES * STAGE_BYTES, "the cluster reduction parks a partial in the ring");
 };
 
 // Prefill-shaped launches (more than one token tile): "data-parallel waves + stream-K tail".  Linear tile index i
@@ -220,9 +235,10 @@ __device__ __forceinline__ void qkv_rope_store(const GemmRope& rope, int head, i
   }
 }
 
-// (the fused-norm warps only exist for token tiles of at most GEMM_NORM_MAX_T rows: larger tiles get their registers)
-template <int BT, int NW>
-__global__ void __launch_bounds__(BT <= GEMM_NORM_MAX_T ? GEMM_THREADS_NORM : GEMM_THREADS, 1)
+// (the fused-norm warps only exist for token tiles of at most GEMM_NORM_MAX_T rows and not in the lean instantiation:
+// larger tiles get their registers, the lean one its second CTA per SM)
+template <int BT, int NW, bool LEAN>
+__global__ void __launch_bounds__(GemmCfg<BT, NW, LEAN>::THREADS, GemmCfg<BT, NW, LEAN>::MIN_BLOCKS)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap xmap,
                          void* __restrict__ Yv, int ldy, int T, int N, int K, float* __restrict__ ws,
                          int* __restrict__ counters, int stream_weights, int out_f32,
@@ -231,7 +247,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
   // output: bf16 (rounded once from the fp32 accumulator, = F.linear in model dtype) or raw fp32 (lm_head logits)
   __nv_bfloat16* __restrict__ Y = reinterpret_cast<__nv_bfloat16*>(Yv);
   float* __restrict__ Yf = reinterpret_cast<float*>(Yv);
-  using Cfg = GemmCfg<BT, NW>;
+  using Cfg = GemmCfg<BT, NW, LEAN>;
+  constexpr bool NORM_ROLES = !LEAN && BT <= GEMM_NORM_MAX_T;  // fused RMSNorm consumer (warps 9..10) compiled in
   constexpr int STAGES = Cfg::STAGES;
   constexpr int BNW = GEMM_BN * NW;            // weight rows per unit
   extern __shared__ uint8_t smem_raw[];
@@ -246,7 +263,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
   uint64_t* xfull_bar = bars + 52;  // [STAGES <= 12] fused-norm consumer: raw token tile landed (weights: full_bar)
   float* rstd_smem = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES);  // [64]
   uint8_t* wn_smem = smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES + 256;                      // [K] bf16 norm weights
-  const bool norm_in = norm.h != nullptr;  // the token operand is RMSNorm(h): warps 9..10 rewrite each landed stage in place
+  // the token operand is RMSNorm(h): warps 9..10 rewrite each landed stage in place
+  const bool norm_in = NORM_ROLES && norm.h != nullptr;
 
   const int warp = threadIdx.x >> 5;
   STL_ENTER(2 | (N << 8));
@@ -261,7 +279,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
   // cluster mode, push variant: every CTA sends its partial rows straight into the OWNER's receive buffer (tokens
   // t = r (mod s) belong to rank r), ONE cluster barrier, then each owner sums its own shared memory in rank order -- no
   // remote read latency and no exit barrier (pull variant: park locally, barrier, read peers, barrier)
-  const bool cl_push = (stream_weights & 4) != 0;
+  const bool cl_push = !LEAN && (stream_weights & 4) != 0;
   stream_weights &= 1;
   const long long total = sched.sk_total;  // stream-K region (== everything for decode-shaped launches)
 
@@ -291,7 +309,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
   // signals ready_bar, which the consumer warps wait for.  Warps 9 / 10 take the even / odd k-blocks; when the dependency
   // resolves a whole ring of tiles lands at once, so the (then idle) first consumer warpgroup takes k-blocks 2..5 of that
   // burst before it issues its first MMA.
-  constexpr int NJ = BT <= GEMM_NORM_MAX_T ? BT / 4 : 1;
+  constexpr int NJ = NORM_ROLES ? BT / 4 : 1;
   const int norm_n_kb = (int)((total * (cta + 1)) / ncta - (total * cta) / ncta);  // decode-shaped: no whole-tile waves
   const int norm_kb0 = (int)(((total * cta) / ncta) % KB);
   const bool norm_helpers = norm_in && STAGES >= 6 && norm_n_kb >= 6;
@@ -418,7 +436,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
       TL(2);           // weight prefetch issued
       griddep_wait();  // activations (and everything the epilogue will touch) are now final
       TL(3);           // dependency wait returned
-      if (threadIdx.x == 0) STL_WAITED();
+      STL_WAITED_REC(*stl_slot_smem);  // (the producer warp does not hold thread 0's record index)
       int stage = 0;
       uint32_t phase = 0;
       for (int i = 0; i < n_kb; ++i) {
@@ -441,7 +459,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
         }
       }
       TL(4);  // last TMA issued
-      STL_EXTRA(STL_MINE(), 1);
+      STL_EXTRA(*stl_slot_smem, 1);
       // Cross-kernel weight prefetch: HBM goes idle while this kernel drains its pipeline, reduces split tiles and
       // exits, and the next GEMM of the layer stack needs ~10 us before its own loads are in flight.  So the boxes
       // that the next GEMM's CTAs will read FIRST are pulled into the 50 MB L2 now (TMA prefetch, no smem, no
@@ -468,7 +486,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
     // 8 j + frag_col + e
     const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     const int frag_col = 2 * (lane & 3);
-    if constexpr (BT <= GEMM_NORM_MAX_T) {
+    if constexpr (NORM_ROLES) {
       if (norm_helpers && warp < 4) {  // start-up burst of the fused-norm consumer: k-blocks 2..5
         asm volatile("bar.sync 2, 192;\n" ::: "memory");  // rstd is in shared memory
         float rs[NJ];
@@ -595,7 +613,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
           // Ordered (CTA-rank) reduction, one L2 round trip for the common case: thread -> 4 consecutive rows
           // (one 16-B load per contributor and token), tokens t == ep_tid/32 (mod 8); all FIX_T x FIX_C loads of a
           // batch are issued before the first add.  Sum order per element is contributor rank order -> deterministic.
-          constexpr int FIX_C = 3, FIX_T = 8;
+          // (lean: smaller load batches keep it within 96 registers without spills; the sum order per element is the
+          // contributor order either way)
+          constexpr int FIX_C = LEAN ? 2 : 3, FIX_T = LEAN ? 2 : 8;
           const int r4 = (ep_tid & 31) * 4;   // first of this thread's 4 rows
           const int tq = ep_tid >> 5;         // token phase 0..EP_WARPS-1
 #pragma unroll 1
@@ -673,7 +693,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
     // k-blocks alternate between the two warps; consumer warps 0..3 take k-blocks 2..5 of the start-up burst (see
     // norm_stage above).  rstd first: lane p fetches partial sum p of every row of this warp's half of the token tile
     // (all loads independent: one L2 round trip), a fixed shuffle tree adds them (deterministic).
-    if constexpr (BT <= GEMM_NORM_MAX_T) {
+    if constexpr (NORM_ROLES) {
       const int tw = warp - NORM_WARP0;            // 0 / 1
       const int tid = threadIdx.x - GEMM_THREADS;  // 0..63
       const int lane = lane_id();
@@ -727,7 +747,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
       const int r4 = (ep_tid & 31) * 4;   // this thread's 4 consecutive weight rows
       const int tq = ep_tid >> 5;         // token phase 0..EP_WARPS-1
       const uint32_t stg = smem_u32(smem);
-      constexpr int FIX_T = 4;
+      constexpr int FIX_T = LEAN ? 2 : 4;  // (lean: a CTA owns at most 16 tokens of its 32-token tile at split >= 2)
 #pragma unroll 1
       for (int h = 0; h < NW; ++h) {
       const int nt = cl_tile * NW + h;    // weight tile (= head of the qkv projection)
@@ -739,7 +759,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
 #pragma unroll
         for (int j = 0; j < FIX_T; ++j) acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
         uint2 resv[FIX_T];  // fused residual add: this thread's residual values, in flight during the DSMEM reads
-        if (norm.sumsq_out != nullptr) {
+        if (!LEAN && norm.sumsq_out != nullptr) {
 #pragma unroll
           for (int j = 0; j < FIX_T; ++j) {
             const int t = crank + cluster_split * (i0 + EP_WARPS * j);
@@ -771,7 +791,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
           if (t < cl_tvalid) {
             const size_t o = (size_t)t * ldy + n4;
             const float av[4] = {acc[j].x, acc[j].y, acc[j].z, acc[j].w};
-            if (norm.sumsq_out != nullptr) {
+            if (!LEAN && norm.sumsq_out != nullptr) {
               // h = bf16(bf16(y) + residual) (fused_add_rms_norm's add), back into the residual stream, + this tile's
               // share of sum(h^2) for the consumer's rstd; t and the tile are warp-uniform
               const float rr[4] = {__uint_as_float(resv[j].x << 16), __uint_as_float(resv[j].x & 0xffff0000u),
@@ -895,14 +915,31 @@ static bool gemm_cluster_enabled() {  // TGIS_GEMM_CLUSTER=0: always reduce spli
   return v == 1;
 }
 
-template <int BT, int NW>
+template <int BT, int NW, bool LEAN>
 __global__ void gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap, const __grid_constant__ CUtensorMap, void*, int,
                                          int, int, int, float*, int*, int, int, const __grid_constant__ CUtensorMap,
                                          GemmNext, int, GemmRope, GemmNorm);
 
+// Per-instantiation function attributes, set once (retried until they succeed): the dynamic shared memory limit, and for
+// the lean instantiation the full 228 KB shared-memory carveout its two CTAs per SM need.
+template <int BT, int NW, bool LEAN>
+static cudaError_t gemm_set_attrs() {
+  static bool done = false;
+  if (done) return cudaSuccess;
+  cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BT, NW, LEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       GemmCfg<BT, NW, LEAN>::SMEM_MAX);
+  if (e == cudaSuccess && LEAN)
+    e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BT, NW, LEAN>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                             (int)cudaSharedmemCarveoutMaxShared);
+  done = e == cudaSuccess;
+  return e;
+}
+
 // How many clusters of `s` GEMM CTAs (one CTA per SM) the device can hold at once: a GPC hosts floor(its SMs / s) of them,
 // so fewer than num_sms / s.  Queried once per size; without a device (host-only plan tests) the
-// optimistic num_sms / s.
+// optimistic num_sms / s.  The query (and cluster_split_bt's) deliberately uses the one-CTA-per-SM instantiation, also
+// for launches that run lean: a lean launch becomes resident next to the previous GEMM's CTA, i.e. with one free slot
+// per SM, and the split factor (hence the split points and the numerics) must not depend on which instantiation runs.
 static int gemm_max_clusters(int s, int num_sms) {
   static int cache[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   if (s < 2 || s > 8) return num_sms / (s > 0 ? s : 1);
@@ -920,9 +957,8 @@ static int gemm_max_clusters(int s, int num_sms) {
     qc.attrs = qa;
     qc.numAttrs = 1;
     int n = 0;
-    if (cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<32, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_MAX) ==
-            cudaSuccess &&
-        cudaOccupancyMaxActiveClusters(&n, gemm_bf16_wgmma_kernel<32, 1>, &qc) == cudaSuccess && n > 0) {
+    if (gemm_set_attrs<32, 1, false>() == cudaSuccess &&
+        cudaOccupancyMaxActiveClusters(&n, gemm_bf16_wgmma_kernel<32, 1, false>, &qc) == cudaSuccess && n > 0) {
       cache[s] = n;
     } else {
       cudaGetLastError();
@@ -1016,11 +1052,7 @@ static int cluster_split_bt(int T, int N, int K, int num_sms) {
   const int nc = grid / split;
   if (nc >= 160) return 0;
   if (cluster_ok[split][nc] == 0) {
-    static bool attr_set = false;
-    if (!attr_set) {
-      cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BT, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_MAX);
-      attr_set = true;
-    }
+    gemm_set_attrs<BT, NW, false>();
     cudaLaunchConfig_t qc{};
     qc.gridDim = dim3(split * (num_sms / split));
     qc.blockDim = dim3(GEMM_THREADS);
@@ -1033,7 +1065,7 @@ static int cluster_split_bt(int T, int N, int K, int num_sms) {
     qc.attrs = qa;
     qc.numAttrs = 1;
     int n_clusters = 0;
-    const cudaError_t qe = cudaOccupancyMaxActiveClusters(&n_clusters, gemm_bf16_wgmma_kernel<BT, NW>, &qc);
+    const cudaError_t qe = cudaOccupancyMaxActiveClusters(&n_clusters, gemm_bf16_wgmma_kernel<BT, NW, false>, &qc);
     // All clusters of the launch must be co-resident: a GPC only hosts floor(SMs / split) of them, and one cluster left
     // over for a second wave doubles the launch time.
     cluster_ok[split][nc] = (qe == cudaSuccess && n_clusters >= nc) ? 1 : -1;
@@ -1065,15 +1097,9 @@ int gemm_cluster_split(int T, int N, int K, int num_sms) {
 template <int BT, int NW>
 static cudaError_t launch_bt(const CUtensorMap& wmap, const CUtensorMap& xmap, void* Y, int ldy, int T, int N, int K,
                              float* ws, int* counters, int num_sms, int out_f32, cudaStream_t stream,
-                             const CUtensorMap& next_wmap, const GemmNext& nxt, const GemmRope& rope, const GemmNorm& norm) {
+                             const CUtensorMap& next_wmap, const GemmNext& nxt, const GemmRope& rope, const GemmNorm& norm,
+                             bool lean) {
   using Cfg = GemmCfg<BT, NW>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BT, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_MAX);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
   const int t_tiles = (T + BT - 1) / BT;
   const int grid = gemm_grid_size(T, N, K, num_sms);
   // bit 0: weights are read once (evict-first); bit 1: stream-K share before the whole tiles (GemmSched::sk_first;
@@ -1111,18 +1137,31 @@ static cudaError_t launch_bt(const CUtensorMap& wmap, const CUtensorMap& xmap, v
                             smem_bytes > (size_t)Cfg::SMEM_MAX))
     return cudaErrorInvalidValue;
   const int threads = norm.h != nullptr ? GEMM_THREADS_NORM : GEMM_THREADS;
+  // decode token tiles without the fused-norm roles or the push receive buffer run lean (GemmCfg): same tiles, split
+  // points and reduction order, a shorter ring and room for the next launch's CTA on every SM
+  auto kernel = gemm_bf16_wgmma_kernel<BT, NW, false>;
+  size_t smem = smem_bytes;
+  cudaError_t e = gemm_set_attrs<BT, NW, false>();
+  if constexpr (BT <= GEMM_LEAN_MAX_T && NW == 1) {
+    if (lean && norm.h == nullptr && norm.sumsq_out == nullptr && !push) {
+      kernel = gemm_bf16_wgmma_kernel<BT, NW, true>;
+      smem = GemmCfg<BT, NW, true>::SMEM_BYTES;
+      e = gemm_set_attrs<BT, NW, true>();
+    }
+  }
+  if (e != cudaSuccess) return e;
   if (split > 0)
-    return launch_k_cluster(gemm_bf16_wgmma_kernel<BT, NW>, dim3(grid), dim3(threads), smem_bytes, stream, split,
-                            wmap, xmap, Y, ldy, T, N, K, ws, counters, stream_weights, out_f32, next_wmap, nxt, split, rope,
-                            norm);
-  return launch_k(gemm_bf16_wgmma_kernel<BT, NW>, dim3(grid), dim3(threads), smem_bytes, stream, wmap, xmap, Y,
-                  ldy, T, N, K, ws, counters, stream_weights, out_f32, next_wmap, nxt, 0, rope, norm);
+    return launch_k_cluster(kernel, dim3(grid), dim3(threads), smem, stream, split, wmap, xmap, Y, ldy, T, N, K, ws,
+                            counters, stream_weights, out_f32, next_wmap, nxt, split, rope, norm);
+  return launch_k(kernel, dim3(grid), dim3(threads), smem, stream, wmap, xmap, Y, ldy, T, N, K, ws, counters,
+                  stream_weights, out_f32, next_wmap, nxt, 0, rope, norm);
 }
 
 // xmap must have been built with box_rows == gemm_pick_bt(T)
 cudaError_t gemm_bf16_launch(const CUtensorMap& wmap, const CUtensorMap& xmap, void* Y, int ldy, int T, int N, int K,
                              float* ws, int* counters, int num_sms, cudaStream_t stream, int out_f32,
-                             const CUtensorMap* next_wmap, const GemmNext* next, const GemmRope* rope, const GemmNorm* norm) {
+                             const CUtensorMap* next_wmap, const GemmNext* next, const GemmRope* rope, const GemmNorm* norm,
+                             bool lean) {
   GemmRope rp{};
   if (rope) rp = *rope;
   GemmNorm nr{};
@@ -1132,8 +1171,8 @@ cudaError_t gemm_bf16_launch(const CUtensorMap& wmap, const CUtensorMap& xmap, v
   const CUtensorMap& nm = (next && next_wmap) ? *next_wmap : wmap;
   const int nw = gemm_nw(T);
 #define TGIS_GEMM_CASE(B)                                                                                              \
-  return nw == 2 ? launch_bt<B, 2>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, nm, nx, rp, nr) \
-                 : launch_bt<B, 1>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, nm, nx, rp, nr)
+  return nw == 2 ? launch_bt<B, 2>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, nm, nx, rp, nr, lean) \
+                 : launch_bt<B, 1>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, nm, nx, rp, nr, lean)
   switch (gemm_pick_bt(T)) {
     case 16: TGIS_GEMM_CASE(16);
     case 32: TGIS_GEMM_CASE(32);
@@ -1142,6 +1181,26 @@ cudaError_t gemm_bf16_launch(const CUtensorMap& wmap, const CUtensorMap& xmap, v
     default: TGIS_GEMM_CASE(256);
   }
 #undef TGIS_GEMM_CASE
+}
+
+template <int BT, bool LEAN>
+static int blocks_per_sm_bt() {
+  if (gemm_set_attrs<BT, 1, LEAN>() != cudaSuccess) return -1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, gemm_bf16_wgmma_kernel<BT, 1, LEAN>, GEMM_THREADS,
+                                                    GemmCfg<BT, 1, LEAN>::SMEM_BYTES) != cudaSuccess)
+    return -1;
+  return n;
+}
+
+int gemm_blocks_per_sm(int T, bool lean) {
+  switch (gemm_pick_bt(T)) {
+    case 16: return lean ? blocks_per_sm_bt<16, true>() : blocks_per_sm_bt<16, false>();
+    case 32: return lean ? blocks_per_sm_bt<32, true>() : blocks_per_sm_bt<32, false>();
+    case 64: return blocks_per_sm_bt<64, false>();
+    case 128: return blocks_per_sm_bt<128, false>();
+    default: return blocks_per_sm_bt<256, false>();
+  }
 }
 
 }  // namespace tgis

@@ -65,7 +65,10 @@ int gemm_cluster_split(int T, int N, int K, int num_sms);
 cudaError_t gemm_bf16_launch(const CUtensorMap& wmap, const CUtensorMap& xmap, void* Y, int ldy, int T, int N, int K,
                              float* ws, int* counters, int num_sms, cudaStream_t stream, int out_f32 = 0,
                              const CUtensorMap* next_wmap = nullptr, const GemmNext* next = nullptr,
-                             const GemmRope* rope = nullptr, const GemmNorm* norm = nullptr);
+                             const GemmRope* rope = nullptr, const GemmNorm* norm = nullptr, bool lean = true);
+// CTAs per SM of the instantiation a T-token launch runs (the lean decode one when `lean` and T <= 32; gemm_wgmma.cu),
+// or -1 when the occupancy query fails
+int gemm_blocks_per_sm(int T, bool lean);
 
 // ---- gemm_ref.cu (debug cross-check only; never on the product path) ---------------------------------------------
 cudaError_t gemm_bf16_ref_launch(const __nv_bfloat16* X, int ldx, const __nv_bfloat16* W, void* Y, int ldy, int T,

@@ -315,11 +315,13 @@ __device__ __forceinline__ unsigned long long stl_timer() {
 // header word [1] = latest exit stamp of ANY warp of any instrumented kernel; the next kernel's CTA 0 stores
 // (its wait-return time - that stamp) in bits 32..51 of its record's word 0, so the "gap" after a kernel splits into
 // the kernel's own tail (last warp exit - CTA 0 exit) and the dependency-resolution latency.
-#define STL_WAITED() do { if (_stl >= 0) {                                                            \
+// STL_WAITED_REC: the same from another thread of CTA 0 that learnt the record index through STL_SHARE.
+#define STL_WAITED_REC(rec) do { const int _rw = (rec); if (g_stl != nullptr && _rw >= 0) {            \
     const unsigned long long _t = stl_timer();                                                        \
-    g_stl[8 + _stl * 4 + 2] = _t;                                                                     \
+    g_stl[8 + _rw * 4 + 2] = _t;                                                                      \
     const unsigned long long _last = *((volatile unsigned long long*)(g_stl + 1));                    \
-    g_stl[8 + _stl * 4 + 0] |= ((_t > _last ? _t - _last : 0ull) & 0xfffffull) << 32; } } while (0)
+    g_stl[8 + _rw * 4 + 0] |= ((_t > _last ? _t - _last : 0ull) & 0xfffffull) << 32; } } while (0)
+#define STL_WAITED() STL_WAITED_REC(_stl)
 #define STL_EXIT() do {                                                                               \
     if (g_stl != nullptr && (threadIdx.x & 31) == 0) atomicMax(g_stl + 1, stl_timer());               \
     if (_stl >= 0) g_stl[8 + _stl * 4 + 3] = stl_timer(); } while (0)
@@ -334,6 +336,7 @@ __device__ __forceinline__ unsigned long long stl_timer() {
   int prefix##_set_step_timeline(unsigned long long*) { return -2; }
 #define STL_ENTER(kid) do {} while (0)
 #define STL_WAITED() do {} while (0)
+#define STL_WAITED_REC(rec) do {} while (0)
 #define STL_EXIT() do {} while (0)
 #define STL_SHARE(smem_int_ptr) do {} while (0)
 #define STL_EXTRA(rec, k) do {} while (0)

@@ -107,7 +107,8 @@ int tgis_k_gemm(const void* x_dev, const void* w_dev, void* y_dev, int32_t T, in
     KCK(cudaMemset(ctr.p, 0, sizeof(int) << 16));
     KCK(cudaEventRecord(e0, st));
     for (int i = 0; i < iters; ++i)
-      KCK(gemm_bf16_launch(wm, xm, y_dev, out_f32 == 2 ? N / 2 : N, T, N, K, ws.p, ctr.p, sms, st, out_f32));
+      KCK(gemm_bf16_launch(wm, xm, y_dev, out_f32 == 2 ? N / 2 : N, T, N, K, ws.p, ctr.p, sms, st, out_f32, nullptr,
+                           nullptr, nullptr, nullptr, /*lean=*/impl != 2));
     KCK(cudaEventRecord(e1, st));
     KCK(cudaStreamSynchronize(st));
   }
@@ -373,6 +374,13 @@ int tgis_k_gemm_plan(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* 
   *grid_out = gemm_grid_size(T, N, K, num_sms);
   *even_split_out = gemm_even_split(T, N, K, num_sms);
   return 0;
+}
+
+// CTAs per SM the GEMM instantiation of a T-token launch can hold (lean != 0: the lean decode instantiation where T <= 32)
+int tgis_k_gemm_blocks_per_sm(int32_t T, int32_t lean, int32_t* out) {
+  if (T <= 0) return kfail("bad shape");
+  *out = gemm_blocks_per_sm(T, lean != 0);
+  return *out > 0 ? 0 : kfail("occupancy query failed");
 }
 
 // weight rows per GEMM unit (128 x the number of weight tiles that share one activation tile) for a T-token launch
