@@ -58,6 +58,16 @@ int tgis_k_gemm_norm_chain(const void* a_dev, int32_t a_rows_alloc, const void* 
 int tgis_k_attention(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, const int32_t* seqs_host,
                      int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride, void* out_dev,
                      int32_t n_q, int32_t n_kv, float scale);
+/* this step's K / V rows written into the cache, then tgis_k_attention's launches, on one stream with no synchronisation
+ * in between (the engine's layer step: the decode kernel streams cache blocks of earlier steps while the writer drains).
+ * writer 0: RoPE + KV scatter (tgis_k_rope_kv) on qkv_dev in place, x_dev / w_dev / K unused; writer 1: qkv_dev = x . w^T
+ * with RoPE and the scatter fused into the GEMM (tgis_k_gemm_rope; returns 1, nothing computed, when the launch plan does
+ * not split every weight tile).  positions / slot mapping: one per query row, T = the sum of q_len over seqs_host. */
+int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, int32_t K, int32_t x_rows_alloc,
+                          void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
+                          const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, const int32_t* seqs_host,
+                          int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride,
+                          void* out_dev, int32_t n_q, int32_t n_kv, float scale);
 /* host-only: GEMM launch plan for a shape: token tile (16..256), grid, even-split factor (0: stream-K + global fix-up) */
 int tgis_k_gemm_plan(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* bt_out, int32_t* grid_out,
                      int32_t* even_split_out);

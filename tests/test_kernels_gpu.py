@@ -2,8 +2,10 @@
 
 Tolerances (written here, per the task contract):
   * integer / index results (greedy token ids, ranks, top-n ids, KV-cache placement, RoPE bits): bit-exact
-  * bf16 tensor results whose fp32 accumulation ORDER differs from the oracle's (GEMM, RMSNorm, attention): <= 1 bf16 ulp
-    per element (2 ulp for attention, whose prefill path rounds probabilities to bf16 like every flash kernel)
+  * bf16 tensor results whose fp32 accumulation ORDER differs from the oracle's (GEMM, RMSNorm): <= 1 bf16 ulp per element
+  * attention (both kernels feed P to the tensor cores as bf16 hi + lo): against a float64 softmax from the same bf16
+    inputs, <= 1 bf16 ulp per element or <= 2^-16 of the row's largest output, and >= 99 % bit-exact
+    (tgis_gpu_utils.attention_bar; tests/test_attention_precision_gpu.py runs the same bar at serving shapes)
   * logprobs: 1e-3 absolute (BASELINE.json north_star)
 """
 import ctypes as C
@@ -296,12 +298,7 @@ def test_fused_residual_rmsnorm_in_gemms_matches_three_launch_path(g, T, K1, H, 
 
 
 def _attention_case(g, n_q, n_kv, seq_specs, seed):
-    """seq_specs: list of (context_len_before, q_len).  Returns (out_gpu, out_oracle)."""
-    from oracle.llama_oracle import LlamaConfig, LlamaOracle
-
-    cfg = LlamaConfig(n_layers=1, hidden=128, n_q_heads=n_q, n_kv_heads=n_kv, ffn=128, vocab=8, max_model_len=4096)
-    ora = LlamaOracle.__new__(LlamaOracle)
-    ora.cfg, ora.dtype = cfg, torch.bfloat16
+    """seq_specs: list of (context_len_before, q_len).  Returns (out_gpu, float64 reference) on the CPU."""
     gen = torch.Generator().manual_seed(seed)
     T = sum(q for _, q in seq_specs)
     q_all = torch.randn(T, n_q, 128, generator=gen).bfloat16()
@@ -314,7 +311,7 @@ def _attention_case(g, n_q, n_kv, seq_specs, seed):
     v_dense = torch.zeros(n_blocks * 32, n_kv, 128, dtype=torch.bfloat16)
     bt = np.zeros((len(seq_specs), bt_stride), dtype=np.int32)
     seqs = np.zeros((len(seq_specs), 4), dtype=np.int32)
-    ref = torch.zeros(T, n_q, 128, dtype=torch.bfloat16)
+    ref = torch.zeros(T, n_q, 128, dtype=torch.float64)
     blk_cursor, q_start = 0, 0
     for s, (ctx, ql) in enumerate(seq_specs):
         kv_len = ctx + ql
@@ -328,7 +325,8 @@ def _attention_case(g, n_q, n_kv, seq_specs, seed):
             slot = int(blocks[j // 32]) * 32 + j % 32
             k_dense[slot], v_dense[slot] = k[j], v[j]
         seqs[s] = (q_start, ql, kv_len, s)
-        ref[q_start: q_start + ql] = ora._attend(q_all[q_start: q_start + ql], k, v, ctx)
+        ref[q_start: q_start + ql] = g.attention_reference_f64(q_all[q_start: q_start + ql], k, v, ctx,
+                                                               1.0 / math.sqrt(128))
         q_start += ql
     kc = g.k_cache_from_dense(k_dense.cuda(), n_blocks)
     vc = g.v_cache_from_dense(v_dense.cuda(), n_blocks)
@@ -345,9 +343,9 @@ def _attention_case(g, n_q, n_kv, seq_specs, seed):
 def test_attention_decode_split_kv(g, n_q, n_kv):
     specs = [(c, 1) for c in (0, 1, 30, 31, 32, 127, 128, 129, 255, 300, 575, 1000)]
     out, ref = _attention_case(g, n_q, n_kv, specs, seed=n_q * 10 + n_kv)
-    ulp = g.bf16_ulp_diff(out, ref)
-    big = (ulp > 2.0) & ((out.float() - ref.float()).abs() > 2e-3)
-    assert int(big.sum()) == 0, float(ulp.max())
+    n_bad, exact, worst = g.attention_bar(out, ref)
+    assert n_bad == 0, worst
+    assert exact >= 0.99, exact
 
 
 @pytest.mark.parametrize("n_q,n_kv", [(8, 2), (8, 1), (2, 2)])
@@ -368,9 +366,9 @@ def test_attention_inkernel_split_merge_is_bit_identical(g, n_q, n_kv, monkeypat
 def test_attention_prefill_and_mixed(g, n_q, n_kv):
     specs = [(0, 5), (0, 16), (0, 17), (0, 50), (40, 33), (0, 1), (100, 1), (31, 70), (0, 129), (200, 2)]
     out, ref = _attention_case(g, n_q, n_kv, specs, seed=n_q * 100 + n_kv)
-    diff = (out.float() - ref.float()).abs()
-    assert float(diff.max()) < 2e-2, float(diff.max())   # bf16 P in the tensor-core path
-    assert float(diff.mean()) < 1.5e-3, float(diff.mean())
+    n_bad, exact, worst = g.attention_bar(out, ref)
+    assert n_bad == 0, worst
+    assert exact >= 0.99, exact
 
 
 # ----------------------------------------------------------------------------------------------------- sampler

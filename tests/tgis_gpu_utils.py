@@ -64,6 +64,64 @@ def bf16_ulp_diff(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return (a32 - b32).abs() / ulp
 
 
+def attention_reference_f64(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, first_pos: int, scale: float
+                            ) -> torch.Tensor:
+    """float64 softmax(q k^T * scale) v of one sequence, causal by absolute position (query i sits at first_pos + i).
+    q [q_len, n_q, 128], k / v [kv_len, n_kv, 128] (bf16, any device) -> float64 [q_len, n_q, 128] on q's device."""
+    q_len, n_q, _ = q.shape
+    kv_len, n_kv, _ = k.shape
+    G = n_q // n_kv
+    k, v = k.to(q.device), v.to(q.device)
+    future = torch.arange(kv_len, device=q.device)[None, :] > (first_pos + torch.arange(q_len, device=q.device))[:, None]
+    out = torch.empty(q_len, n_q, HEAD_DIM, dtype=torch.float64, device=q.device)
+    for h in range(n_kv):  # one kv head at a time bounds the [G, q_len, kv_len] score tensor
+        s = q[:, h * G:(h + 1) * G].double().transpose(0, 1) @ k[:, h].double().t() * scale
+        p = torch.softmax(s.masked_fill_(future, float("-inf")), dim=-1)
+        out[:, h * G:(h + 1) * G] = (p @ v[:, h].double()).transpose(0, 1)
+    return out
+
+
+def attention_floor_scale(first_pos: int, q_len: int) -> torch.Tensor:
+    """Per query row of one sequence, the factor on attention_bar's 2^-16 floor: keys accumulated in one pass / 2048,
+    at least 1.  The tensor-core MMA does not round its fp32 accumulation like an FADD, so the error of O grows with
+    the number of MMAs chained into one accumulator.  A prefill row chains its whole context (2 MMAs per 16 keys,
+    hi and lo); decode restarts every 128-token split and merges the splits in ordinary fp32 arithmetic (q_len 1: 1).
+    Measured on H100: a chunk at context 7680 .. 8191 misses the plain 2^-16 floor by up to ~2x on a few elements."""
+    if q_len == 1:
+        return torch.ones(1, 1, 1, dtype=torch.float64)
+    keys = first_pos + 1 + torch.arange(q_len, dtype=torch.float64)
+    return (keys / 2048).clamp_min(1.0)[:, None, None]
+
+
+def attention_bar(out: torch.Tensor, ref: torch.Tensor, floor_scale: torch.Tensor | None = None
+                  ) -> tuple[int, float, str]:
+    """The accuracy bar of the attention kernels (P reaches the tensor cores as bf16 hi + lo, ~16 mantissa bits):
+    every element within one bf16 ulp of the float64 reference, or within 2^-16 * floor_scale of its row's largest
+    |ref| (the floor for near-cancelling outputs; floor_scale broadcasts against ref[..., :1], attention_floor_scale).
+    out bf16 [..., 128], ref float64, same shape.
+    Returns (elements over the bar, fraction bit-exact to bf16(ref), description of the worst element, which also
+    gives the largest error / floor ratio)."""
+    o = out.to(ref.device).double()
+    err = (o - ref).abs()
+    ulp = torch.exp2(torch.floor(torch.log2(ref.abs().clamp_min(1e-30))) - 7)
+    floor = 2.0 ** -16 * ref.abs().amax(dim=-1, keepdim=True)
+    if floor_scale is not None:
+        floor = floor * floor_scale.to(ref.device)
+    bad = (err > ulp) & (err > floor)
+    exact = float((out.to(ref.device) == ref.to(torch.bfloat16)).double().mean())
+    over_ulp = err > ulp
+    ratio = float(torch.where(over_ulp, err / floor.clamp_min(1e-300), torch.zeros_like(err)).max()) if bool(
+        over_ulp.any()) else 0.0
+    worst = f"max error / floor where over 1 ulp: {ratio:.2f}"
+    n_bad = int(bad.sum())
+    if n_bad:
+        i = int(torch.argmax(torch.where(bad, err / ulp, torch.zeros_like(err))))
+        idx = np.unravel_index(i, tuple(ref.shape))
+        worst += (f"; worst at {tuple(int(j) for j in idx)}: out {float(o.flatten()[i])!r} "
+                  f"ref {float(ref.flatten()[i])!r} ({float((err / ulp).flatten()[i]):.1f} ulp)")
+    return n_bad, exact, worst
+
+
 def k_cache_from_dense(k: torch.Tensor, n_blocks: int) -> torch.Tensor:
     """k: [tokens, n_kv, 128] (already placed: token t lives in slot t) -> engine K layout
     [blocks][n_kv][16 chunks][32 tok][8]."""

@@ -261,53 +261,133 @@ int tgis_k_gemm_norm_chain(const void* a_dev, int32_t a_rows_alloc, const void* 
   return 0;
 }
 
+namespace {
+// The device-side metadata of one attention call (sequences, decode items, prefill tiles, split partials), uploaded
+// before anything is launched, so that the launches can follow a cache-writing kernel on the same stream with no
+// synchronisation in between, as in the engine's step.
+struct AttnCall {
+  int n_q = 0, n_kv = 0, n_dec = 0, n_tiles = 0, max_splits = 1, bt_stride = 0;
+  Tmp<AttnSeq> seqs;
+  Tmp<int32_t> dec, tseq, tq0, bt;
+  Tmp<float> po, pml;
+  Tmp<DecItem> items;
+  Tmp<int> arrive;  // arrival counters of the in-kernel split merge (the launcher ignores them when that path is off)
+
+  int prepare(const int32_t* seqs_host, int n_seqs, const int32_t* block_table_host, int bt_rows, int stride, int nq,
+              int nkv) {
+    if (nkv <= 0 || nq % nkv) return kfail("bad head counts");
+    n_q = nq;
+    n_kv = nkv;
+    bt_stride = stride;
+    const int G = n_q / n_kv;
+    std::vector<AttnSeq> h_seqs(n_seqs);
+    std::vector<int32_t> h_dec, h_tseq, h_tq0;
+    int max_kv = 1;
+    for (int s = 0; s < n_seqs; ++s) {
+      h_seqs[s] = AttnSeq{seqs_host[4 * s], seqs_host[4 * s + 1], seqs_host[4 * s + 2], seqs_host[4 * s + 3]};
+      if (h_seqs[s].q_len == 1) {
+        h_dec.push_back(s);
+        max_kv = std::max(max_kv, h_seqs[s].kv_len);
+      } else {
+        for (int q0 = 0; q0 < h_seqs[s].q_len; q0 += 16) {
+          h_tseq.push_back(s);
+          h_tq0.push_back(q0);
+        }
+      }
+    }
+    n_dec = (int)h_dec.size();
+    n_tiles = (int)h_tseq.size();
+    KCK(seqs.upload(h_seqs.data(), n_seqs));
+    KCK(dec.upload(h_dec.data(), h_dec.size()));
+    KCK(tseq.upload(h_tseq.data(), h_tseq.size()));
+    KCK(tq0.upload(h_tq0.data(), h_tq0.size()));
+    KCK(bt.upload(block_table_host, (size_t)bt_rows * bt_stride));
+    max_splits = (max_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
+    const size_t nd = n_dec ? n_dec : 1;
+    KCK(po.alloc(nd * n_kv * max_splits * G * HEAD_DIM));
+    KCK(pml.alloc(nd * n_kv * max_splits * G * 2));
+    std::vector<DecItem> h_items(1 + nd * max_splits);
+    decode_items_build(h_items.data(), h_seqs.data(), h_dec.data(), n_dec, block_table_host, bt_stride);
+    KCK(items.upload(h_items.data(), h_items.size()));
+    KCK(arrive.alloc(nd * n_kv));
+    KCK(cudaMemset(arrive.p, 0, sizeof(int) * nd * n_kv));
+    return 0;
+  }
+  // decode (+ split merge), then prefill: the engine's order
+  int launch(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, void* out_dev, float scale,
+             cudaStream_t st) {
+    const int qkv_ld = (n_q + 2 * n_kv) * HEAD_DIM, out_ld = n_q * HEAD_DIM;
+    KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, items.p,
+                           n_dec * max_splits, seqs.p, dec.p, n_dec, max_splits, po.p, pml.p, (bf16*)out_dev, out_ld,
+                           n_q, n_kv, scale, test_num_sms(), st, arrive.p));
+    KCK(attn_prefill_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, seqs.p,
+                            tseq.p, tq0.p, n_tiles, bt.p, bt_stride, (bf16*)out_dev, out_ld, n_q, n_kv, scale, st));
+    return 0;
+  }
+};
+}  // namespace
+
 int tgis_k_attention(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, const int32_t* seqs_host,
                      int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride, void* out_dev,
                      int32_t n_q, int32_t n_kv, float scale) {
-  if (n_kv <= 0 || n_q % n_kv) return kfail("bad head counts");
-  const int G = n_q / n_kv;
-  const int qkv_ld = (n_q + 2 * n_kv) * HEAD_DIM, out_ld = n_q * HEAD_DIM;
-  std::vector<AttnSeq> seqs(n_seqs);
-  std::vector<int32_t> dec, tseq, tq0;
-  int max_kv = 1;
-  for (int s = 0; s < n_seqs; ++s) {
-    seqs[s] = AttnSeq{seqs_host[4 * s], seqs_host[4 * s + 1], seqs_host[4 * s + 2], seqs_host[4 * s + 3]};
-    if (seqs[s].q_len == 1) {
-      dec.push_back(s);
-      max_kv = std::max(max_kv, seqs[s].kv_len);
-    } else {
-      for (int q0 = 0; q0 < seqs[s].q_len; q0 += 16) {
-        tseq.push_back(s);
-        tq0.push_back(q0);
-      }
-    }
-  }
-  Tmp<AttnSeq> d_seqs;
-  Tmp<int32_t> d_dec, d_tseq, d_tq0, d_bt;
-  Tmp<float> po, pml;
-  KCK(d_seqs.upload(seqs.data(), n_seqs));
-  KCK(d_dec.upload(dec.data(), dec.size()));
-  KCK(d_tseq.upload(tseq.data(), tseq.size()));
-  KCK(d_tq0.upload(tq0.data(), tq0.size()));
-  KCK(d_bt.upload(block_table_host, (size_t)bt_rows * bt_stride));
-  const int max_splits = (max_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
-  const size_t nd = dec.size() ? dec.size() : 1;
-  KCK(po.alloc(nd * n_kv * max_splits * G * HEAD_DIM));
-  KCK(pml.alloc(nd * n_kv * max_splits * G * 2));
-  std::vector<DecItem> items(1 + nd * max_splits);
-  decode_items_build(items.data(), seqs.data(), dec.data(), (int)dec.size(), block_table_host, bt_stride);
-  Tmp<DecItem> d_items;
-  KCK(d_items.upload(items.data(), items.size()));
-  Tmp<int> arrive;  // arrival counters of the in-kernel split merge (the launcher ignores them when that path is off)
-  KCK(arrive.alloc(nd * n_kv));
-  KCK(cudaMemset(arrive.p, 0, sizeof(int) * nd * n_kv));
-  KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, d_items.p,
-                         (int)dec.size() * max_splits, d_seqs.p, d_dec.p, (int)dec.size(), max_splits, po.p, pml.p,
-                         (bf16*)out_dev, out_ld, n_q, n_kv, scale, test_num_sms(), 0, arrive.p));
-  KCK(attn_prefill_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, d_seqs.p,
-                          d_tseq.p, d_tq0.p, (int)tseq.size(), d_bt.p, bt_stride, (bf16*)out_dev, out_ld, n_q, n_kv,
-                          scale, 0));
+  AttnCall call;
+  if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv) != 0) return -1;
+  if (call.launch(qkv_dev, k_cache_dev, v_cache_dev, out_dev, scale, 0) != 0) return -1;
   KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
+// This step's K / V rows written into the cache, then attention over it, on one stream with no synchronisation in
+// between (the engine's layer step): the decode kernel's cache reads before its grid-dependency wait then overlap the
+// writer's tail.  writer 0: rope_kvwrite_launch on qkv_dev in place (x_dev, w_dev, K unused); writer 1: qkv_dev =
+// x . w^T by the GEMM with the fused RoPE + KV-scatter epilogue (returns 1, nothing computed, when the launch plan does
+// not split every weight tile).  T = the sum of the sequences' q_len.
+int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, int32_t K, int32_t x_rows_alloc,
+                          void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
+                          const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, const int32_t* seqs_host,
+                          int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride,
+                          void* out_dev, int32_t n_q, int32_t n_kv, float scale) {
+  if (writer != 0 && writer != 1) return kfail("writer must be 0 (rope_kvwrite) or 1 (GEMM with fused RoPE)");
+  int T = 0;
+  for (int s = 0; s < n_seqs; ++s) T += seqs_host[4 * s + 1];
+  const int N = (n_q + 2 * n_kv) * HEAD_DIM;
+  const int sms = test_num_sms();
+  if (writer == 1 && gemm_even_split(T, N, K, sms) < 2) return 1;
+  AttnCall call;
+  if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv) != 0) return -1;
+  Tmp<int32_t> pos, sm;
+  KCK(pos.upload(positions_host, T));
+  KCK(sm.upload(slot_mapping_host, T));
+  Tmp<float> ws;
+  Tmp<int> ctr;
+  CUtensorMap wm, xm;
+  if (writer == 1) {
+    const int bt = gemm_pick_bt(T);
+    if (x_rows_alloc < bt) return kfail("x must have at least one TMA box of rows allocated");
+    if (make_tmap_bf16_2d(&wm, w_dev, N, K, K, 128, 64) != 0) return kfail("weight tensor map failed");
+    if (make_tmap_bf16_2d(&xm, x_dev, x_rows_alloc, K, K, bt, 64) != 0) return kfail("activation tensor map failed");
+    KCK(ws.alloc(gemm_workspace_bytes(sms) / sizeof(float)));
+    KCK(ctr.alloc(1 << 16));
+    KCK(cudaMemset(ctr.p, 0, sizeof(int) << 16));
+  }
+  KCK(cudaDeviceSynchronize());  // every upload has landed: from here on only launches on `st`
+  cudaStream_t st;
+  KCK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  int rc = 0;
+  cudaError_t e;
+  if (writer == 1) {
+    const GemmRope rp{pos.p, sm.p, (const bf16*)cos_sin_dev, (bf16*)k_cache_dev, (bf16*)v_cache_dev, n_q, n_kv};
+    e = gemm_bf16_launch(wm, xm, qkv_dev, N, T, N, K, ws.p, ctr.p, sms, st, 0, nullptr, nullptr, &rp);
+  } else {
+    e = rope_kvwrite_launch((bf16*)qkv_dev, pos.p, sm.p, (const bf16*)cos_sin_dev, (bf16*)k_cache_dev,
+                            (bf16*)v_cache_dev, T, n_q, n_kv, st);
+  }
+  if (e != cudaSuccess) rc = kfail(std::string("cache writer: ") + cudaGetErrorString(e));
+  if (rc == 0) rc = call.launch(qkv_dev, k_cache_dev, v_cache_dev, out_dev, scale, st);
+  e = cudaStreamSynchronize(st);
+  cudaStreamDestroy(st);
+  if (rc != 0) return rc;
+  if (e != cudaSuccess) return kfail(std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e));
   return 0;
 }
 
