@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define TGIS_ABI_VERSION 7
+#define TGIS_ABI_VERSION 8
 #define TGIS_MAX_REQUEST_ID 96
 #define TGIS_MAX_TOPN 12 /* reference forces max_logprobs >= 11: tgis_utils/args.py:214-216 */
 #define TGIS_MAX_STOP_TOKEN_IDS 8
@@ -66,7 +66,7 @@ typedef struct tgis_config {
   int32_t n_kv_heads;
   int32_t head_dim; /* 128; OPT: 64 or 128 */
   int32_t ffn;
-  int32_t vocab;
+  int32_t vocab;              /* any size when tp_size == 1 (the lm_head is padded to a multiple of 8 internally) */
   float rope_theta;
   float rms_eps;              /* RMSNorm epsilon; OPT: the LayerNorm epsilon */
   int32_t max_model_len;      /* reference: --max-sequence-length / --max-model-len (tgis_utils/args.py:187-192) */
@@ -75,7 +75,7 @@ typedef struct tgis_config {
   int64_t kv_cache_bytes;     /* 0 = size from gpu_mem_fraction */
   float gpu_mem_fraction;     /* fraction of free HBM the KV cache may take when kv_cache_bytes == 0 */
   int32_t device;             /* CUDA device ordinal */
-  int32_t tp_size;            /* tensor-parallel world (1 = single GPU); heads, ffn and vocab must divide */
+  int32_t tp_size;            /* tensor-parallel world (1 = single GPU); heads, ffn/64 and vocab/8 must divide */
   int32_t tp_rank;
   int32_t use_cuda_graphs;    /* capture decode steps into CUDA graphs */
   int32_t debug_gemm_ref;     /* debug only: route GEMMs through the SIMT cross-check kernel */
@@ -200,6 +200,15 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out);
  * ...; a 1-D tensor is passed as rows = n, cols = 1).  ptr may be host or device memory (cudaMemcpyDefault);
  * dtype 0 = bf16.  rows/cols describe the full (unsharded) tensor. */
 int tgis_engine_load_weight(tgis_engine* e, const char* name, const void* ptr, int64_t rows, int64_t cols, int32_t dtype);
+/* Granite (GraniteForCausalLM: the Llama layer stack plus four scalars of its config.json; vllm
+ * model_executor/models/granite.py).  Valid only between tgis_engine_create and tgis_engine_start, TGIS_ARCH_LLAMA only.
+ *   embedding_multiplier  h = bf16(embed[token] * m) after the lookup
+ *   residual_multiplier   r = bf16(r + bf16(x * m)) after o_proj and after down_proj; tp_size must be 1 unless m == 1
+ *   attention_multiplier  the softmax scale (0: 1 / sqrt(head_dim))
+ *   logit_scale           1 / logits_scaling: the sampler sees bf16(logit * s)
+ * The defaults 1, 1, 0, 1 are the Llama stack, bit for bit. */
+int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, float residual_multiplier,
+                                  float attention_multiplier, float logit_scale);
 int tgis_engine_start(tgis_engine* e);
 int tgis_engine_add_request(tgis_engine* e, const char* request_id, const int32_t* prompt_ids, int32_t n_prompt,
                             const tgis_sampling_params* params);

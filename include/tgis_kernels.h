@@ -29,6 +29,13 @@ int tgis_k_gemm(const void* x_dev, const void* w_dev, void* y_dev, int32_t T, in
 /* residual_dev may be NULL (plain rmsnorm); otherwise residual is updated in place */
 int tgis_k_rmsnorm(const void* x_dev, void* residual_dev, const void* w_dev, void* out_dev, int32_t T, int32_t hidden,
                    float eps);
+/* Granite (vllm model_executor/models/granite.py): residual = bf16(residual + bf16(x * res_mult)), then the same norm as
+ * tgis_k_rmsnorm (res_mult = 1: bit-identical to it).  residual_dev must not be NULL. */
+int tgis_k_rmsnorm_mult(const void* x_dev, void* residual_dev, const void* w_dev, void* out_dev, int32_t T,
+                        int32_t hidden, float eps, float res_mult);
+/* embedding gather: out[t] = bf16(table[tok[t]] * mult) (mult = 1: a plain copy); tok is an int32 DEVICE array */
+int tgis_k_embed(const void* tok_dev, const void* table_dev, void* out_dev, int32_t T, int32_t hidden, int32_t vocab,
+                 float mult);
 int tgis_k_silu_mul(const void* gate_up_dev, void* act_dev, int32_t T, int32_t ffn);
 /* OPT (csrc/opt.cu; vllm model_executor/models/opt.py:61-70,148-197 = torch.nn.LayerNorm / F.linear(x, W, b) / ReLU):
  * tgis_k_opt_layernorm: acc_dev != NULL: residual = bf16(residual + bf16(acc + acc_bias)) first (acc fp32 [T, hidden], the
@@ -99,6 +106,12 @@ int tgis_k_sampler_ex(const void* logits_dev, int32_t logits_bf16, int32_t ld, i
 int tgis_k_sampler_masked(const void* logits_dev, int32_t logits_bf16, int32_t ld, int32_t vocab, const void* rows_host,
                           int32_t n_rows, void* seen_bitmap_dev, const void* allow_bitmap_dev, void* out_host,
                           int32_t iters, float* us_out);
+/* same as tgis_k_sampler_masked (one launch), with Granite's logit scale: the sampler sees bf16(logit * logit_scale) (fp32
+ * logits: the fp32 product) in every pass, as after vLLM's LogitsProcessor(scale).  logits_dev itself is not modified.
+ * vocab may be any size <= ld (ld % 8 == 0); columns [vocab, ld) are padding. */
+int tgis_k_sampler_scaled(const void* logits_dev, int32_t logits_bf16, int32_t ld, int32_t vocab, const void* rows_host,
+                          int32_t n_rows, void* seen_bitmap_dev, const void* allow_bitmap_dev, void* out_host,
+                          float logit_scale);
 /* LoRA (csrc/lora.cu; vllm lora/punica_wrapper/punica_gpu.py add_lora_linear): x [T, ldx] bf16, tok_slot [T] int32 (0 = no
  * adapter, s >= 1 = slot s), A [slots][Rm][K] bf16, B [slots][N][Rm] bf16 (scaling folded in); in place on y [T, ldy] bf16:
  * y[t, col0 + n] = bf16(y + bf16(B_s[n, :] . bf16(A_s x[t]))) */

@@ -58,8 +58,11 @@ cudaError_t stl_marker_launch(int kid, cudaStream_t stream) {
 }
 
 // ------------------------------------------------------------------------------------------------ embedding / gather
+// SCALE: out = bf16(row * mult) (Granite's embedding_multiplier, vllm models/granite.py: one bf16 multiply after the
+// lookup); otherwise a plain copy (last-token rows, and every Llama embedding)
+template <bool SCALE>
 __global__ void gather_rows_kernel(const int32_t* __restrict__ idx, const __nv_bfloat16* __restrict__ table,
-                                   __nv_bfloat16* __restrict__ out, int hidden, int n_table_rows) {
+                                   __nv_bfloat16* __restrict__ out, int hidden, int n_table_rows, float mult) {
   STL_ENTER(8);
   griddep_launch();
   griddep_wait();
@@ -69,20 +72,53 @@ __global__ void gather_rows_kernel(const int32_t* __restrict__ idx, const __nv_b
   if (row < 0 || row >= n_table_rows) row = 0;  // padding rows: any valid row (never consumed)
   const BF8* src = reinterpret_cast<const BF8*>(table + (size_t)row * hidden);
   BF8* dst = reinterpret_cast<BF8*>(out + (size_t)t * hidden);
-  for (int i = threadIdx.x; i < hidden / 8; i += blockDim.x) dst[i] = src[i];
+  for (int i = threadIdx.x; i < hidden / 8; i += blockDim.x) {
+    BF8 v = src[i];
+    if (SCALE) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v.v[e] = __float2bfloat16_rn(__bfloat162float(v.v[e]) * mult);
+    }
+    dst[i] = v;
+  }
   STL_EXIT();
 }
 
 cudaError_t embed_gather_launch(const int32_t* token_ids, const __nv_bfloat16* table, __nv_bfloat16* out, int T,
-                                int hidden, int vocab, cudaStream_t stream) {
+                                int hidden, int vocab, cudaStream_t stream, float mult) {
   if (T <= 0) return cudaSuccess;
-  return launch_k(gather_rows_kernel, dim3(T), dim3(128), 0, stream, token_ids, table, out, hidden, vocab);
+  if (mult != 1.f)
+    return launch_k(gather_rows_kernel<true>, dim3(T), dim3(128), 0, stream, token_ids, table, out, hidden, vocab, mult);
+  return launch_k(gather_rows_kernel<false>, dim3(T), dim3(128), 0, stream, token_ids, table, out, hidden, vocab, 1.f);
 }
 
 cudaError_t gather_rows_launch(const __nv_bfloat16* x, const int32_t* rows, __nv_bfloat16* out, int R, int hidden,
                                cudaStream_t stream) {
   if (R <= 0) return cudaSuccess;
-  return launch_k(gather_rows_kernel, dim3(R), dim3(128), 0, stream, rows, x, out, hidden, 1 << 30);
+  return launch_k(gather_rows_kernel<false>, dim3(R), dim3(128), 0, stream, rows, x, out, hidden, 1 << 30, 1.f);
+}
+
+// Granite's logits_scaling (vllm models/granite.py LogitsProcessor(scale = 1 / logits_scaling), logits_processor.py
+// `logits *= scale` on the model-dtype lm_head output): logits[r, :vocab] = bf16(logits * scale) in place, one row per CTA.
+// The sampler then sees exactly the values vLLM's sampler casts to fp32.
+template <class LT>
+__global__ void logits_scale_kernel(LT* __restrict__ logits, int ld, int vocab, float scale) {
+  griddep_launch();
+  griddep_wait();
+  LT* row = logits + (size_t)blockIdx.x * ld;
+  for (int i = threadIdx.x; i < vocab; i += blockDim.x) {
+    if constexpr (sizeof(LT) == 2) row[i] = __float2bfloat16_rn(__bfloat162float(row[i]) * scale);
+    else row[i] = row[i] * scale;
+  }
+}
+
+cudaError_t logits_scale_launch(void* logits, int logits_bf16, int ld, int vocab, int rows, float scale,
+                                cudaStream_t stream) {
+  if (rows <= 0) return cudaSuccess;
+  if (logits_bf16)
+    return launch_k(logits_scale_kernel<__nv_bfloat16>, dim3(rows), dim3(512), 0, stream,
+                    static_cast<__nv_bfloat16*>(logits), ld, vocab, scale);
+  return launch_k(logits_scale_kernel<float>, dim3(rows), dim3(512), 0, stream, static_cast<float*>(logits), ld, vocab,
+                  scale);
 }
 
 // ------------------------------------------------------------------------------------------------ RMSNorm
@@ -92,10 +128,13 @@ constexpr int NORM_MAX_VEC = 4;  // hidden <= 256 * 8 * 4 = 8192
 // NORM_MAX_VEC (vectors per thread) is a template parameter: the row lives in registers, and the 8192-wide instantiation's
 // 80 registers cap a prefill chunk at 3 CTAs per SM; hidden = 4096 needs two vectors per thread.  Same thread -> element
 // map and the same reduction tree for every instantiation: results do not depend on it.
-template <bool ADD, int NORM_MAX_VEC>
+// MULT (ADD only): Granite's residual multiplier; a separate instantiation, so that the Llama stack runs the code it ran
+// before the multiplier existed
+template <bool ADD, int NORM_MAX_VEC, bool MULT = false>
 __global__ void __launch_bounds__(NORM_THREADS)
 rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ residual,
-               const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ out, int hidden, float eps) {
+               const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ out, int hidden, float eps,
+               float res_mult) {
   __shared__ float red[NORM_THREADS / 32];
   STL_ENTER(1);
   griddep_launch();
@@ -120,6 +159,11 @@ rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ 
       BF8 a = reinterpret_cast<const BF8*>(x + base)[i];
       if (ADD) {
         BF8 r = reinterpret_cast<const BF8*>(residual + base)[i];
+        // Granite: residual + bf16(x * residual_multiplier), two roundings (vllm models/granite.py); Llama: m = 1
+        if (MULT) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) a.v[e] = __float2bfloat16_rn(__bfloat162float(a.v[e]) * res_mult);
+        }
 #pragma unroll
         for (int e = 0; e < 8; ++e) a.v[e] = __float2bfloat16_rn(__bfloat162float(a.v[e]) + __bfloat162float(r.v[e]));
         reinterpret_cast<BF8*>(residual + base)[i] = a;
@@ -156,21 +200,31 @@ cudaError_t rmsnorm_launch(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_
   if (hidden % 8 != 0 || hidden > NORM_THREADS * 8 * NORM_MAX_VEC) return cudaErrorInvalidValue;
   __nv_bfloat16* none = nullptr;
   if (hidden <= NORM_THREADS * 8)
-    return launch_k(rmsnorm_kernel<false, 1>, dim3(T), dim3(NORM_THREADS), 0, stream, x, none, w, out, hidden, eps);
+    return launch_k(rmsnorm_kernel<false, 1>, dim3(T), dim3(NORM_THREADS), 0, stream, x, none, w, out, hidden, eps, 1.f);
   if (hidden <= NORM_THREADS * 16)
-    return launch_k(rmsnorm_kernel<false, 2>, dim3(T), dim3(NORM_THREADS), 0, stream, x, none, w, out, hidden, eps);
-  return launch_k(rmsnorm_kernel<false, 4>, dim3(T), dim3(NORM_THREADS), 0, stream, x, none, w, out, hidden, eps);
+    return launch_k(rmsnorm_kernel<false, 2>, dim3(T), dim3(NORM_THREADS), 0, stream, x, none, w, out, hidden, eps, 1.f);
+  return launch_k(rmsnorm_kernel<false, 4>, dim3(T), dim3(NORM_THREADS), 0, stream, x, none, w, out, hidden, eps, 1.f);
 }
 
 cudaError_t add_rmsnorm_launch(const __nv_bfloat16* x, __nv_bfloat16* residual, const __nv_bfloat16* w,
-                               __nv_bfloat16* out, int T, int hidden, float eps, cudaStream_t stream) {
+                               __nv_bfloat16* out, int T, int hidden, float eps, cudaStream_t stream, float res_mult) {
   if (T <= 0) return cudaSuccess;
   if (hidden % 8 != 0 || hidden > NORM_THREADS * 8 * NORM_MAX_VEC) return cudaErrorInvalidValue;
+  if (res_mult != 1.f) {
+    if (hidden <= NORM_THREADS * 8)
+      return launch_k(rmsnorm_kernel<true, 1, true>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden,
+                      eps, res_mult);
+    if (hidden <= NORM_THREADS * 16)
+      return launch_k(rmsnorm_kernel<true, 2, true>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden,
+                      eps, res_mult);
+    return launch_k(rmsnorm_kernel<true, 4, true>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden,
+                    eps, res_mult);
+  }
   if (hidden <= NORM_THREADS * 8)
-    return launch_k(rmsnorm_kernel<true, 1>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden, eps);
+    return launch_k(rmsnorm_kernel<true, 1>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden, eps, res_mult);
   if (hidden <= NORM_THREADS * 16)
-    return launch_k(rmsnorm_kernel<true, 2>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden, eps);
-  return launch_k(rmsnorm_kernel<true, 4>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden, eps);
+    return launch_k(rmsnorm_kernel<true, 2>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden, eps, res_mult);
+  return launch_k(rmsnorm_kernel<true, 4>, dim3(T), dim3(NORM_THREADS), 0, stream, x, residual, w, out, hidden, eps, res_mult);
 }
 
 // ------------------------------------------------------------------------------------------------ TP: fused exchange

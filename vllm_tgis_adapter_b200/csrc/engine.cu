@@ -230,6 +230,12 @@ struct tgis_engine {
   bf16 *pos_embed = nullptr, *final_norm_b = nullptr;
   int pos_rows = 0, model_head_dim = HEAD_DIM;
   float attn_scale = 0.f;
+  // Granite's scalars (tgis_engine_set_model_scalars; 1 = the Llama stack): embedding and residual multipliers, and the
+  // scale of the bf16 logits the sampler sees (1 / logits_scaling)
+  float emb_mult = 1.f, res_mult = 1.f, logit_scale = 1.f;
+  // rows of embed / lm_head: the vocabulary rounded up to a multiple of 8 (the padded rows are zero), so that the lm_head
+  // GEMM's output rows stay 16-byte aligned for any vocabulary; the sampler is told ld = Vpad, vocab = V
+  int Vpad = 0;
   DevBuf<float> y32;
   std::set<std::string> opt_loaded;  // tensor names seen by load_weight_opt (completeness check at start)
   std::vector<LayerW> layers;
@@ -425,6 +431,7 @@ struct tgis_engine {
     nkv = c.n_kv_heads / tp;
     Fl = c.ffn / tp;
     Vl = c.vocab / tp;
+    Vpad = (c.vocab + 7) / 8 * 8;  // == vocab under tensor parallelism (tgis_engine_create)
     opt = c.arch == TGIS_ARCH_OPT;
     model_head_dim = opt ? c.head_dim : HEAD_DIM;
     attn_scale = 1.0f / std::sqrt((float)model_head_dim);  // zero-padded head dims add nothing to q . k
@@ -465,7 +472,8 @@ struct tgis_engine {
     const size_t H = c.hidden, F = Fl, V = c.vocab, L = c.n_layers;  // F: this rank's ffn shard
     const size_t per_layer = (size_t)qkv_dim * H + H * q_dim + 2 * F * H + H * F + 2 * H;
     const size_t opt_extra = opt ? (size_t)pos_rows * H + H + L * ((size_t)qkv_dim + 4 * H + F) + 64 * (6 * L + 4) : 0;
-    const size_t total = V * H /*embed*/ + V * H /*lm_head*/ + H /*norm*/ + (size_t)c.max_model_len * HEAD_DIM +
+    const size_t Vp = Vpad;
+    const size_t total = Vp * H /*embed*/ + Vp * H /*lm_head*/ + H /*norm*/ + (size_t)c.max_model_len * HEAD_DIM +
                          L * per_layer + 64 * (6 * L + 8) + opt_extra;
     w_arena.alloc(total);
     if (opt) w_arena.zero();  // the padded head dims of q/k/v rows, out_proj columns and their biases stay zero
@@ -475,8 +483,12 @@ struct tgis_engine {
       p += (n + 63) / 64 * 64;  // 128-B aligned slices (TMA needs 16 B)
       return r;
     };
-    embed = take(V * H);
-    lm_head = take(V * H);
+    embed = take(Vp * H);
+    lm_head = take(Vp * H);
+    if (Vp > V) {  // padded vocabulary rows: zero logits, never sampled
+      CK(cudaMemset(embed + V * H, 0, (Vp - V) * H * sizeof(bf16)));
+      CK(cudaMemset(lm_head + V * H, 0, (Vp - V) * H * sizeof(bf16)));
+    }
     final_norm = take(H);
     cos_sin = take((size_t)c.max_model_len * HEAD_DIM);
     layers.resize(L);
@@ -539,7 +551,7 @@ struct tgis_engine {
       gu_buf.alloc(T_alloc * (size_t)2 * F);
     }
     last_hidden.alloc(S_alloc * H);
-    logits.alloc((size_t)S_max * V * lsz);
+    logits.alloc((size_t)S_max * Vp * lsz);
     if (tp > 1) {
       logits_shard.alloc((size_t)S_max * Vl * lsz);
       logits_gather.alloc((size_t)tp * S_max * Vl * lsz);
@@ -604,7 +616,7 @@ struct tgis_engine {
       wmap(&l.m_gu, l.wgu, opt ? F : 2 * F, H);  // OPT: fc1
       wmap(&l.m_d, l.wd, H, F);
     }
-    wmap(&m_lm, lm_head, Vl, H);  // this rank's vocab shard (== V when tp == 1)
+    wmap(&m_lm, lm_head, tp == 1 ? Vpad : Vl, H);  // this rank's vocab shard (the padded vocabulary when tp == 1)
     for (int i = 0; i < N_BT; ++i) {
       const int bt = BT_VALUES[i];
       auto xmap = [&](CUtensorMap* m, const bf16* x, size_t rows, size_t cols) {
@@ -1057,8 +1069,8 @@ struct tgis_engine {
         throw CudaError("OPT checkpoint incomplete: " + std::to_string(opt_loaded.size()) + " of " + std::to_string(expected) +
                         " tensors loaded (embed_tokens, embed_positions, final_layer_norm.{weight,bias} and 16 per layer)");
     }
-    if (!lm_head_loaded)  // tie_word_embeddings
-      CK(cudaMemcpy(lm_head, embed + (size_t)rank * Vl * cfg.hidden, (size_t)Vl * cfg.hidden * sizeof(bf16),
+    if (!lm_head_loaded)  // tie_word_embeddings (tp == 1: with the zero padding rows)
+      CK(cudaMemcpy(lm_head, embed + (size_t)rank * Vl * cfg.hidden, (size_t)(tp == 1 ? Vpad : Vl) * cfg.hidden * sizeof(bf16),
                     cudaMemcpyDeviceToDevice));
   }
 
@@ -1134,7 +1146,7 @@ struct tgis_engine {
     if (opt) {
       opt_layers(T, n_dec, n_tiles, max_dec_kv, S, R);  // embeddings + layer stack + final LayerNorm -> xn
     } else {
-      CK(embed_gather_launch(d_tok, embed, resid.p, T, H, V, stream));
+      CK(embed_gather_launch(d_tok, embed, resid.p, T, H, V, stream, emb_mult));
       ++n_launches;
     }
     const bool ar_fused = exchange_mode(T) != 0;
@@ -1181,7 +1193,7 @@ struct tgis_engine {
         } else if (ar_fused) {
           fused_ar_norm(1, l.ln1, T);  // previous layer's down-proj partials
         } else {
-          CK(add_rmsnorm_launch(tmp.p, resid.p, l.ln1, xn.p, T, H, c.rms_eps, stream));
+          CK(add_rmsnorm_launch(tmp.p, resid.p, l.ln1, xn.p, T, H, c.rms_eps, stream, res_mult));
           ++n_launches;
         }
         const GemmRope rp{ds<int32_t>(off_pos), ds<int32_t>(off_slotmap), cos_sin,
@@ -1232,7 +1244,7 @@ struct tgis_engine {
         fused_ar_norm(0, l.ln2, T);
       } else {
         all_reduce_tmp(T);  // row-parallel partial sums (tp > 1)
-        CK(add_rmsnorm_launch(tmp.p, resid.p, l.ln2, xn.p, T, H, c.rms_eps, stream));
+        CK(add_rmsnorm_launch(tmp.p, resid.p, l.ln2, xn.p, T, H, c.rms_eps, stream, res_mult));
         ++n_launches;
       }
       // gate_up GEMM with SwiGLU fused into its epilogue: writes act[T, F] directly (no gate_up round trip)
@@ -1269,14 +1281,15 @@ struct tgis_engine {
     if (R > 0) {
       if (ar_fused || opt) {
       } else {
-        CK(add_rmsnorm_launch(tmp.p, resid.p, final_norm, xn.p, T, H, c.rms_eps, stream));
+        CK(add_rmsnorm_launch(tmp.p, resid.p, final_norm, xn.p, T, H, c.rms_eps, stream, res_mult));
         ++n_launches;
       }
       CK(gather_rows_launch(xn.p, ds<int32_t>(off_samplesrc), last_hidden.p, R, H, stream));
       ++n_launches;
       lm_head_logits(R, 1);
       if (rank == 0) {
-        CK(sampler_launch(logits_ptr(), logits_bf16 ? 1 : 0, V, V, ds<SampleRow>(off_rows), R, seen_bitmap.p, bitmap_words,
+        scale_logits(R);
+        CK(sampler_launch(logits_ptr(), logits_bf16 ? 1 : 0, Vpad, V, ds<SampleRow>(off_rows), R, seen_bitmap.p, bitmap_words,
                           samp_scratch.p, d_samp_out.p, stream, samp_complex & 1, num_sms,
                           (samp_complex & 2) ? allow_bitmap.p : nullptr));
         ++n_launches;
@@ -1350,7 +1363,7 @@ struct tgis_engine {
     const int H = c.hidden, V = c.vocab;
     const int lm_mode = logits_bf16 ? 0 : 1;
     if (tp == 1) {
-      gemm(xm_last, m_lm, last_hidden.p, lm_head, logits.p, rows, V, H, lm_mode);
+      gemm(xm_last, m_lm, last_hidden.p, lm_head, logits.p, rows, Vpad, H, lm_mode);
     } else if (tp_fused_ar) {
       uint32_t* flags0 = reinterpret_cast<uint32_t*>(ar_peer[0] + lg_off + lg_logits_bytes());  // in rank 0's memory
       if (rank == 0) {
@@ -1375,19 +1388,27 @@ struct tgis_engine {
     }
   }
 
+  // Granite's logits_scaling: bf16(logit * (1 / logits_scaling)) in place before the sampler reads the rows (rank 0)
+  void scale_logits(int rows) {
+    if (logit_scale == 1.f) return;
+    CK(logits_scale_launch(logits_ptr(), logits_bf16 ? 1 : 0, Vpad, cfg.vocab, rows, logit_scale, stream));
+    ++n_launches;
+  }
+
   void plp_pass(int m, int need_norm, int T, size_t copy_bytes, int lg_idx) {
     const tgis_config& c = cfg;
     const int H = c.hidden, V = c.vocab;
     CK(cudaMemcpyAsync(d_stage.p, h_stage, copy_bytes, cudaMemcpyHostToDevice, stream));
     if (need_norm && !opt) {  // no sampled row in the step -> its final norm has not run yet (OPT: always run)
-      CK(add_rmsnorm_launch(tmp.p, resid.p, final_norm, xn.p, T, H, c.rms_eps, stream));
+      CK(add_rmsnorm_launch(tmp.p, resid.p, final_norm, xn.p, T, H, c.rms_eps, stream, res_mult));
       ++n_launches;
     }
     CK(gather_rows_launch(xn.p, ds<int32_t>(off_samplesrc), last_hidden.p, m, H, stream));
     ++n_launches;
     lm_head_logits(m, lg_idx);
     if (rank == 0) {
-      CK(sampler_launch(logits_ptr(), logits_bf16 ? 1 : 0, V, V, ds<SampleRow>(off_rows), m, seen_bitmap.p, bitmap_words,
+      scale_logits(m);
+      CK(sampler_launch(logits_ptr(), logits_bf16 ? 1 : 0, Vpad, V, ds<SampleRow>(off_rows), m, seen_bitmap.p, bitmap_words,
                         samp_scratch.p, d_samp_out.p, stream, /*any_complex=*/0, num_sms));
       ++n_launches;
       CK(cudaMemcpyAsync(h_plp_out, d_samp_out.p, sizeof(SampleOut) * m, cudaMemcpyDeviceToHost, stream));
@@ -1968,11 +1989,13 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
   if (cfg->n_kv_heads <= 0 || cfg->n_q_heads % cfg->n_kv_heads != 0) return fail("n_q_heads must be a multiple of n_kv_heads");
   const int G = cfg->n_q_heads / cfg->n_kv_heads;
   if (!(G == 1 || G == 2 || G == 3 || G == 4 || G == 8)) return fail("GQA group size must be 1, 2, 3, 4 or 8");
-  if (cfg->hidden % 64 || cfg->ffn % 64 || cfg->vocab % 8) return fail("hidden/ffn must be multiples of 64, vocab of 8");
+  if (cfg->hidden % 64 || cfg->ffn % 64) return fail("hidden/ffn must be multiples of 64");
+  if (cfg->vocab < 1) return fail("vocab must be positive");
   if (cfg->hidden > 8192) return fail("hidden > 8192 unsupported");
   const int tpv = cfg->tp_size > 1 ? cfg->tp_size : 1;
   if (tpv > 16 || cfg->tp_rank < 0 || cfg->tp_rank >= tpv) return fail("bad tp_size / tp_rank");
-  if (cfg->n_kv_heads % tpv || cfg->ffn % (64 * tpv) || cfg->vocab % (8 * tpv))
+  // (a single GPU takes any vocabulary: its lm_head is padded to a multiple of 8 rows)
+  if (cfg->n_kv_heads % tpv || cfg->ffn % (64 * tpv) || (tpv > 1 && cfg->vocab % (8 * tpv)))
     return fail("n_kv_heads, ffn/64 and vocab/8 must be divisible by tp_size");
   if (cfg->max_batched_tokens < 16 || cfg->max_num_seqs < 1 || cfg->max_model_len < 2) return fail("bad limits");
   if (cfg->max_loras < 0 || cfg->max_loras > 64) return fail("max_loras must be in [0, 64]");
@@ -2002,6 +2025,30 @@ int tgis_engine_load_weight(tgis_engine* e, const char* name, const void* ptr, i
   if (dtype != 0) return fail("only bf16 (dtype 0) weights are supported");
   if (e->started) return fail("engine already started");
   return e->load_weight(name, ptr, rows, cols);
+}
+
+int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, float residual_multiplier,
+                                  float attention_multiplier, float logit_scale) {
+  if (!e) return fail("null engine");
+  if (e->started) return fail("model scalars must be set before tgis_engine_start");
+  auto ok = [](float v) { return std::isfinite(v) && v > 0.f; };
+  if (!ok(embedding_multiplier) || !ok(residual_multiplier) || !ok(logit_scale) ||
+      !(std::isfinite(attention_multiplier) && attention_multiplier >= 0.f))
+    return fail("model scalars must be finite and positive (attention_multiplier: 0 = 1/sqrt(head_dim))");
+  const bool llama = embedding_multiplier == 1.f && residual_multiplier == 1.f && attention_multiplier == 0.f &&
+                     logit_scale == 1.f;
+  if (e->opt && !llama) return fail("model scalars (Granite) apply to the Llama layer stack only, not OPT");
+  // the tensor-parallel exchange kernels (ar_add_rmsnorm / ar2_add_rmsnorm) and the NCCL path's norm do not implement
+  // the residual multiplier
+  if (e->tp > 1 && residual_multiplier != 1.f)
+    return fail("Granite (residual_multiplier != 1) is not supported with tensor parallelism (tp_size must be 1)");
+  e->emb_mult = embedding_multiplier;
+  e->res_mult = residual_multiplier;
+  e->logit_scale = logit_scale;
+  e->attn_scale = attention_multiplier > 0.f ? attention_multiplier : 1.0f / std::sqrt((float)e->model_head_dim);
+  // the TGIS_FUSE_NORM experiment folds the residual add into the GEMMs without the multiplier
+  if (residual_multiplier != 1.f) e->fuse_norm = false;
+  return 0;
 }
 
 int tgis_engine_start(tgis_engine* e) {

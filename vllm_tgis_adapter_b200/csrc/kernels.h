@@ -76,14 +76,17 @@ cudaError_t gemm_bf16_ref_launch(const __nv_bfloat16* X, int ldx, const __nv_bfl
 
 // ---- elementwise.cu ----------------------------------------------------------------------------------------------
 cudaError_t stl_marker_launch(int kid, cudaStream_t stream);  // -DTGIS_STEP_TIMELINE builds only (else a no-op)
+// out[t] = table[token_ids[t]], or bf16(table[token_ids[t]] * mult) when mult != 1 (Granite's embedding_multiplier)
 cudaError_t embed_gather_launch(const int32_t* token_ids, const __nv_bfloat16* table, __nv_bfloat16* out, int T,
-                                int hidden, int vocab, cudaStream_t stream);
+                                int hidden, int vocab, cudaStream_t stream, float mult = 1.f);
 // out = rmsnorm(x) * w                                   (first layer: residual := x is done by the caller)
 cudaError_t rmsnorm_launch(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* out, int T, int hidden,
                            float eps, cudaStream_t stream);
 // residual = bf16(x + residual); out = rmsnorm(residual) * w     (vllm: layernorm.py fused_add_rms_norm)
+// res_mult != 1 (Granite's residual_multiplier): residual = bf16(residual + bf16(x * res_mult)) instead
 cudaError_t add_rmsnorm_launch(const __nv_bfloat16* x, __nv_bfloat16* residual, const __nv_bfloat16* w,
-                               __nv_bfloat16* out, int T, int hidden, float eps, cudaStream_t stream);
+                               __nv_bfloat16* out, int T, int hidden, float eps, cudaStream_t stream,
+                               float res_mult = 1.f);
 // Tensor parallelism, decode-shaped steps: one-shot all-reduce of the row-parallel GEMM partials over NVLink peer memory
 // fused with the residual add + RMSNorm (elementwise.cu).  own: this rank's partial [T, hidden]; recv[q]: rank q's receive
 // area for this exchange parity, mapped into this process (recv[own rank] = local): [8 source ranks][AR_MAX_ROWS rows]
@@ -115,6 +118,9 @@ cudaError_t logits_push_launch(const void* shard, void* dst_peer0, int R, int Vl
                                cudaStream_t stream);
 cudaError_t logits_wait_launch(const uint32_t* flags, int tp, const uint32_t* epoch_base, uint32_t epoch_idx,
                                cudaStream_t stream);
+// logits[r, :vocab] = bf16(logits * scale) in place (bf16 logits; fp32 logits: fp32 product), rows of ld elements
+cudaError_t logits_scale_launch(void* logits, int logits_bf16, int ld, int vocab, int rows, float scale,
+                                cudaStream_t stream);
 // act[t, i] = bf16(silu(gate_up[t, i])) * gate_up[t, F + i]
 cudaError_t silu_mul_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, int T, int ffn, cudaStream_t stream);
 // ---- multi-adapter LoRA (lora.cu): y[t, col0 + n] += bf16(B_s[n, :] . bf16(A_s x[t])), s = tok_slot[t] (0 = no adapter)
@@ -263,6 +269,7 @@ struct SampleOut {            // per row result (pinned host readable)
 constexpr int SAMPLE_GREEDY = 1, SAMPLE_LOGPROBS = 2, SAMPLE_TYPICAL = 4, SAMPLE_LENPEN = 8, SAMPLE_SEEDED = 16;
 constexpr int SAMPLE_MASKED = 64;  // guided decoding: row seq_slot of the allow bitmap holds this step's allowed-token bits
 constexpr int SAMPLE_FORCED = 32;  // token = seed_lo is given (prompt logprobs): report its logprob / rank / top-n only
+// vocab may be any size <= ld (ld % 8 == 0): columns [vocab, ld) are padding and are never read as vocabulary entries.
 // logits: [rows, ld] bf16 (logits_bf16 = 1: the lm_head GEMM's model-dtype output, what vLLM's sampler sees after its
 // fp32 cast) or fp32 (kernel-level golden tests).  any_complex: some row needs selection passes (sampling rows: typical-p /
 // top-k / top-p / race) -> 8 CTAs per row; otherwise the cluster size shrinks with the row count (sampler_cluster_size).

@@ -40,7 +40,7 @@ struct RowCtx {
   const LT* x;             // raw logits
   const LT* xc;            // this CTA's slice staged in shared memory by pass 1 (xc[i - lo]), or nullptr
   int V;
-  int lo, hi;              // this CTA's slice of the vocabulary (multiples of 8)
+  int lo, hi;              // this CTA's slice of the vocabulary (lo a multiple of 8; hi too, or hi == V)
   const uint32_t* seen;    // bitmap of prompt U output tokens (may be null)
   const uint32_t* allow;   // guided decoding: bit i set = token i allowed this step (null: unconstrained).  A cleared bit
                            // turns the RAW logit into -inf before anything else looks at it, which is where vLLM applies
@@ -537,28 +537,42 @@ tgis_sampler_kernel(const LT* __restrict__ logits, int ld, int V, const SampleRo
       }
     }
   };
+  // one group of 8 logits: guided mask, staging copy, then the sweep's reductions
+  auto take8 = [&](float (&v)[8], int iu) {
+    if (MASKED && c.allow != nullptr) {  // iu % 8 == 0: the 8 bits of this group sit in one byte of the bitmap
+      const uint32_t bits = (c.allow[iu >> 5] >> (iu & 31)) & 0xffu;
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        if (!((bits >> e) & 1u)) v[e] = -INFINITY;
+    }
+    if (cache_x) store_x8(xs + (iu - lo), v);
+    consume8(v, iu);
+  };
   constexpr int P1_UNROLL = 4;  // 16-byte loads in flight per thread (64 KB per SM)
-  for (int i0 = lo + threadIdx.x * 8; i0 < hi; i0 += SAMP_THREADS * 8 * P1_UNROLL) {
+  const int hi8 = lo + (hi - lo) / 8 * 8;  // whole groups; == hi unless V % 8 != 0 and this is the last slice
+  for (int i0 = lo + threadIdx.x * 8; i0 < hi8; i0 += SAMP_THREADS * 8 * P1_UNROLL) {
     float xv[P1_UNROLL][8];
 #pragma unroll
     for (int u = 0; u < P1_UNROLL; ++u) {
       const int iu = i0 + u * SAMP_THREADS * 8;
-      if (iu < hi) load_x8(c.x, iu, xv[u]);
+      if (iu < hi8) load_x8(c.x, iu, xv[u]);
     }
 #pragma unroll
     for (int u = 0; u < P1_UNROLL; ++u) {
       const int iu = i0 + u * SAMP_THREADS * 8;
-      if (iu < hi) {
-        if (MASKED && c.allow != nullptr) {  // iu % 8 == 0: the 8 bits of this group sit in one byte of the bitmap
-          const uint32_t bits = (c.allow[iu >> 5] >> (iu & 31)) & 0xffu;
-#pragma unroll
-          for (int e = 0; e < 8; ++e)
-            if (!((bits >> e) & 1u)) xv[u][e] = -INFINITY;
-        }
-        if (cache_x) store_x8(xs + (iu - lo), xv[u]);
-        consume8(xv[u], iu);
-      }
+      if (iu < hi8) take8(xv[u], iu);
     }
+  }
+  // a vocabulary that is not a multiple of 8: the row's last group is partial, and its columns >= V are padding (the
+  // lm_head's zero rows, inside ld).  They become -inf, which neither the max / sum-exp nor the argmax counts, and every
+  // later pass stops at hi = V.  Thread 0 takes the group after its others: its indices stay ascending (argmax ties).
+  if (hi8 < hi && threadIdx.x == 0) {
+    float xv[8];
+    load_x8(c.x, hi8, xv);
+#pragma unroll
+    for (int e = 0; e < 8; ++e)
+      if (hi8 + e >= hi) xv[e] = -INFINITY;
+    take8(xv, hi8);
   }
   if (cache_x) c.xc = xs;  // visible to every thread after the barriers of the reductions below
   int token;
@@ -810,7 +824,7 @@ cudaError_t sampler_launch(const void* logits, int logits_bf16, int ld, int voca
                            const uint32_t* seen_bitmap, int bitmap_words, float* scratch, SampleOut* out,
                            cudaStream_t stream, int any_complex, int num_sms, const uint32_t* allow_bitmap) {
   if (n_rows <= 0) return cudaSuccess;
-  if (vocab % 8 != 0 || ld % 8 != 0) return cudaErrorInvalidValue;
+  if (ld % 8 != 0 || vocab > ld || vocab <= 0) return cudaErrorInvalidValue;
   const int ncl = sampler_cluster_size(n_rows, any_complex, num_sms);
   if (logits_bf16)
     return sampler_launch_t(static_cast<const __nv_bfloat16*>(logits), ld, vocab, rows, n_rows,

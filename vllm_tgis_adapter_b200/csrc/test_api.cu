@@ -131,6 +131,22 @@ int tgis_k_rmsnorm(const void* x_dev, void* residual_dev, const void* w_dev, voi
   return 0;
 }
 
+int tgis_k_rmsnorm_mult(const void* x_dev, void* residual_dev, const void* w_dev, void* out_dev, int32_t T,
+                        int32_t hidden, float eps, float res_mult) {
+  if (!residual_dev) return kfail("tgis_k_rmsnorm_mult needs a residual");
+  KCK(add_rmsnorm_launch((const bf16*)x_dev, (bf16*)residual_dev, (const bf16*)w_dev, (bf16*)out_dev, T, hidden, eps, 0,
+                         res_mult));
+  KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
+int tgis_k_embed(const void* tok_dev, const void* table_dev, void* out_dev, int32_t T, int32_t hidden, int32_t vocab,
+                 float mult) {
+  KCK(embed_gather_launch((const int32_t*)tok_dev, (const bf16*)table_dev, (bf16*)out_dev, T, hidden, vocab, 0, mult));
+  KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
 int tgis_k_opt_layernorm(const void* acc_dev, const void* acc_bias_dev, void* residual_dev, const void* w_dev,
                          const void* b_dev, void* out_dev, int32_t T, int32_t hidden, float eps) {
   KCK(opt_layernorm_launch((const float*)acc_dev, (const bf16*)acc_bias_dev, (bf16*)residual_dev, (const bf16*)w_dev,
@@ -484,9 +500,23 @@ int tgis_k_decode_items(const int32_t* seqs_host, int32_t n_seqs, const int32_t*
 
 // logits_bf16 = 0: fp32 logits, 1: bf16 logits.  iters > 1: the launch is repeated and us_out (optional) receives the
 // average device time per launch (CUDA events on the launching stream).
-int tgis_k_sampler_masked(const void* logits_dev, int32_t logits_bf16, int32_t ld, int32_t vocab, const void* rows_host,
-                          int32_t n_rows, void* seen_bitmap_dev, const void* allow_bitmap_dev, void* out_host,
-                          int32_t iters, float* us_out) {
+}  // extern "C"
+
+// logit_scale != 1: the logits are copied, scaled in place by logits_scale_launch (the engine's launch before the
+// sampler) and sampled from the copy; the caller's buffer is left as it was
+static int sampler_run(const void* logits_dev, int32_t logits_bf16, int32_t ld, int32_t vocab, const void* rows_host,
+                       int32_t n_rows, void* seen_bitmap_dev, const void* allow_bitmap_dev, void* out_host,
+                       int32_t iters, float* us_out, float logit_scale) {
+  Tmp<uint8_t> scaled;
+  if (logit_scale != 1.f) {
+    int max_row = 0;
+    for (int i = 0; i < n_rows; ++i) max_row = std::max(max_row, ((const SampleRow*)rows_host)[i].logits_row);
+    const size_t bytes = (size_t)(max_row + 1) * ld * (logits_bf16 ? 2 : 4);
+    KCK(scaled.alloc(bytes));
+    KCK(cudaMemcpy(scaled.p, logits_dev, bytes, cudaMemcpyDeviceToDevice));
+    KCK(logits_scale_launch(scaled.p, logits_bf16, ld, vocab, max_row + 1, logit_scale, 0));
+    logits_dev = scaled.p;
+  }
   Tmp<SampleRow> rows;
   Tmp<SampleOut> outs;
   Tmp<float> scratch;
@@ -529,6 +559,22 @@ int tgis_k_sampler_masked(const void* logits_dev, int32_t logits_bf16, int32_t l
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
   return 0;
+}
+
+extern "C" {
+
+int tgis_k_sampler_masked(const void* logits_dev, int32_t logits_bf16, int32_t ld, int32_t vocab, const void* rows_host,
+                          int32_t n_rows, void* seen_bitmap_dev, const void* allow_bitmap_dev, void* out_host,
+                          int32_t iters, float* us_out) {
+  return sampler_run(logits_dev, logits_bf16, ld, vocab, rows_host, n_rows, seen_bitmap_dev, allow_bitmap_dev, out_host,
+                     iters, us_out, 1.f);
+}
+
+int tgis_k_sampler_scaled(const void* logits_dev, int32_t logits_bf16, int32_t ld, int32_t vocab, const void* rows_host,
+                          int32_t n_rows, void* seen_bitmap_dev, const void* allow_bitmap_dev, void* out_host,
+                          float logit_scale) {
+  return sampler_run(logits_dev, logits_bf16, ld, vocab, rows_host, n_rows, seen_bitmap_dev, allow_bitmap_dev, out_host,
+                     1, nullptr, logit_scale);
 }
 
 int tgis_k_sampler_ex(const void* logits_dev, int32_t logits_bf16, int32_t ld, int32_t vocab, const void* rows_host,

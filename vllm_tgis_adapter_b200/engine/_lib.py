@@ -10,7 +10,7 @@ import ctypes as C
 import os
 from pathlib import Path
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 ARCH_LLAMA, ARCH_OPT = 0, 1
 MAX_REQUEST_ID = 96
 MAX_TOPN = 12
@@ -69,14 +69,14 @@ class TgisStatus(C.Structure):
 
 # Every symbol include/tgis_engine.h and include/tgis_kernels.h declare (tests/test_abi_cpu.py checks the export list)
 ENGINE_SYMBOLS = [
-    "tgis_last_error", "tgis_abi_version", "tgis_engine_create", "tgis_engine_load_weight", "tgis_engine_start",
+    "tgis_last_error", "tgis_abi_version", "tgis_engine_create", "tgis_engine_load_weight", "tgis_engine_set_model_scalars", "tgis_engine_start",
     "tgis_engine_add_request", "tgis_engine_abort", "tgis_engine_set_mask_provider", "tgis_engine_load_adapter_weight", "tgis_engine_clear_adapter", "tgis_engine_poll", "tgis_engine_status",
     "tgis_engine_max_model_len", "tgis_engine_set_profiling", "tgis_nccl_unique_id", "tgis_engine_worker_run", "tgis_engine_shutdown", "tgis_engine_destroy", "tgis_engine_run_until_idle",
 ]
 KERNEL_SYMBOLS = [
-    "tgis_k_last_error", "tgis_k_gemm_timeline", "tgis_k_step_timeline_enable", "tgis_k_step_timeline_read", "tgis_k_gemm", "tgis_k_rmsnorm", "tgis_k_opt_layernorm", "tgis_k_opt_bias_act", "tgis_k_opt_embed", "tgis_k_silu_mul", "tgis_k_rope_kv", "tgis_k_gemm_rope", "tgis_k_gemm_norm_chain", "tgis_k_attention", "tgis_k_rope_attention",
+    "tgis_k_last_error", "tgis_k_gemm_timeline", "tgis_k_step_timeline_enable", "tgis_k_step_timeline_read", "tgis_k_gemm", "tgis_k_rmsnorm", "tgis_k_rmsnorm_mult", "tgis_k_embed", "tgis_k_opt_layernorm", "tgis_k_opt_bias_act", "tgis_k_opt_embed", "tgis_k_silu_mul", "tgis_k_rope_kv", "tgis_k_gemm_rope", "tgis_k_gemm_norm_chain", "tgis_k_attention", "tgis_k_rope_attention",
     "tgis_k_attention_bench", "tgis_k_decode_items", "tgis_k_gemm_plan", "tgis_k_gemm_unit_rows", "tgis_k_gemm_blocks_per_sm",
-    "tgis_k_sampler", "tgis_k_sampler_ex", "tgis_k_sampler_masked", "tgis_k_lora", "tgis_k_lora_bench", "tgis_k_silu_mul_interleaved", "tgis_k_sizeof_sample_row", "tgis_k_sizeof_sample_out", "tgis_k_kv_block",
+    "tgis_k_sampler", "tgis_k_sampler_ex", "tgis_k_sampler_masked", "tgis_k_sampler_scaled", "tgis_k_lora", "tgis_k_lora_bench", "tgis_k_silu_mul_interleaved", "tgis_k_sizeof_sample_row", "tgis_k_sizeof_sample_out", "tgis_k_kv_block",
 ]
 
 _LIB: C.CDLL | None = None
@@ -110,6 +110,7 @@ def load_library() -> C.CDLL:
     lib.tgis_k_last_error.restype = C.c_char_p
     lib.tgis_engine_create.argtypes = [C.POINTER(TgisConfig), C.POINTER(vp)]
     lib.tgis_engine_load_weight.argtypes = [vp, C.c_char_p, vp, i64, i64, i32]
+    lib.tgis_engine_set_model_scalars.argtypes = [vp, f32, f32, f32, f32]
     lib.tgis_engine_start.argtypes = [vp]
     lib.tgis_engine_add_request.argtypes = [vp, C.c_char_p, C.POINTER(i32), i32, C.POINTER(TgisSamplingParams)]
     lib.tgis_engine_abort.argtypes = [vp, C.c_char_p]
@@ -128,6 +129,8 @@ def load_library() -> C.CDLL:
     lib.tgis_engine_run_until_idle.argtypes = [vp]
     lib.tgis_k_gemm.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(f32), i32]
     lib.tgis_k_rmsnorm.argtypes = [vp, vp, vp, vp, i32, i32, f32]
+    lib.tgis_k_rmsnorm_mult.argtypes = [vp, vp, vp, vp, i32, i32, f32, f32]
+    lib.tgis_k_embed.argtypes = [vp, vp, vp, i32, i32, i32, f32]
     lib.tgis_k_gemm_norm_chain.argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, i32, i32, i32,
                                            C.POINTER(f32)]
     lib.tgis_k_silu_mul.argtypes = [vp, vp, i32, i32]
@@ -144,6 +147,7 @@ def load_library() -> C.CDLL:
     lib.tgis_k_silu_mul_interleaved.argtypes = [vp, vp, i32, i32]
     lib.tgis_k_lora_bench.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, i32, C.POINTER(f32), C.POINTER(f32)]
     lib.tgis_k_sampler_masked.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, i32, C.POINTER(f32)]
+    lib.tgis_k_sampler_scaled.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, f32]
     _LIB = lib
     return lib
 

@@ -17,7 +17,10 @@ class EngineError(RuntimeError):
 class ModelConfig:
     """Decoder dims (HF config.json names in comments).  arch "llama": RMSNorm / RoPE / GQA / SwiGLU; arch "opt": learned
     positions / LayerNorm / biased projections / ReLU (n_kv_heads == n_q_heads, head_dim 64 or 128, ffn = ffn_dim,
-    rms_eps carries the LayerNorm epsilon, rope_theta unused) -- include/tgis_engine.h TGIS_ARCH_*."""
+    rms_eps carries the LayerNorm epsilon, rope_theta unused) -- include/tgis_engine.h TGIS_ARCH_*.
+
+    Granite (GraniteForCausalLM) is arch "llama" with the four scalars of its config.json set; their defaults are the
+    Llama stack (tgis_engine_set_model_scalars)."""
 
     n_layers: int        # num_hidden_layers
     hidden: int          # hidden_size
@@ -30,6 +33,16 @@ class ModelConfig:
     rms_eps: float = 1e-5
     max_model_len: int = 2048
     arch: str = "llama"
+    tie_word_embeddings: bool = False   # no lm_head.weight: the engine copies embed_tokens
+    embedding_multiplier: float = 1.0   # Granite: h = bf16(embed * m)
+    residual_multiplier: float = 1.0    # Granite: r = bf16(r + bf16(x * m)) after o_proj and down_proj
+    attention_multiplier: float = 0.0   # Granite: softmax scale; 0 = 1/sqrt(head_dim)
+    logits_scaling: float = 1.0         # Granite: logits = bf16(logits * (1 / logits_scaling))
+
+    @property
+    def is_granite(self) -> bool:
+        return (self.embedding_multiplier, self.residual_multiplier, self.attention_multiplier,
+                self.logits_scaling) != (1.0, 1.0, 0.0, 1.0)
 
 
 # Named architectures (real dims; this offline build runs them on synthetic weights — SURVEY.md §0)
@@ -46,6 +59,16 @@ PRESETS: dict[str, ModelConfig] = {
                              max_model_len=8192),
     "llama3-70b": ModelConfig(n_layers=80, hidden=8192, n_q_heads=64, n_kv_heads=8, ffn=28672, vocab=128256,
                               max_model_len=8192),
+    # Granite: a CPU-oracle-sized stack with an odd vocabulary and scalars that round (1/3 is not a power of two), and
+    # the Granite 3.x 8B shape.  The granite-3-8b values are those of the published ibm-granite/granite-3.1-8b config.json
+    # as recalled; they could not be checked against the file when this preset was written.
+    "granite-tiny": ModelConfig(n_layers=2, hidden=256, n_q_heads=4, n_kv_heads=2, ffn=512, vocab=1021,
+                                max_model_len=512, tie_word_embeddings=True, embedding_multiplier=12.0,
+                                residual_multiplier=0.22, attention_multiplier=1.0 / 128, logits_scaling=3.0),
+    "granite-3-8b": ModelConfig(n_layers=40, hidden=4096, n_q_heads=32, n_kv_heads=8, ffn=12800, vocab=49155,
+                                rope_theta=10000000.0, max_model_len=8192, tie_word_embeddings=True,
+                                embedding_multiplier=12.0, residual_multiplier=0.22, attention_multiplier=0.0078125,
+                                logits_scaling=16.0),
 }
 
 
@@ -131,6 +154,9 @@ class NativeEngine:
             cfg.shm_name = shm_name.encode()
         cfg.use_cuda_graphs, cfg.debug_gemm_ref, cfg.seed = int(use_cuda_graphs), 1 if debug_gemm_ref else 0, seed
         cfg.max_loras, cfg.max_lora_rank = int(max_loras), int(max_lora_rank) if max_loras else 0
+        if model.residual_multiplier != 1.0 and tp_size > 1:
+            raise EngineError("Granite (residual_multiplier != 1) is not supported with tensor parallelism: the "
+                              "row-parallel exchange kernels do not implement the multiplier (use tensor_parallel_size 1)")
         if model.arch not in ("llama", "opt"):
             raise EngineError(f"unknown architecture {model.arch!r}")
         cfg.arch = _lib.ARCH_OPT if model.arch == "opt" else _lib.ARCH_LLAMA
@@ -138,6 +164,12 @@ class NativeEngine:
         self._h = C.c_void_p()
         if self.lib.tgis_engine_create(C.byref(cfg), C.byref(self._h)) != 0:
             raise EngineError(f"tgis_engine_create failed: {_lib.last_error(self.lib)}")
+        if model.is_granite and self.lib.tgis_engine_set_model_scalars(
+                self._h, model.embedding_multiplier, model.residual_multiplier, model.attention_multiplier,
+                1.0 / model.logits_scaling) != 0:
+            msg = _lib.last_error(self.lib)
+            self.close()
+            raise EngineError(f"tgis_engine_set_model_scalars failed: {msg}")
         self._poll_buf = (TgisStepOutput * 512)()
 
     # -- weights ------------------------------------------------------------------------------------------------

@@ -23,6 +23,8 @@ def model_config_from_hf(path: Path, max_model_len: int | None) -> ModelConfig:
     archs = cfg.get("architectures") or []
     if cfg.get("model_type") == "opt" or any("OPT" in a for a in archs):
         return _opt_model_config(cfg, max_model_len)
+    if cfg.get("model_type") == "granite" or "GraniteForCausalLM" in archs:
+        return _granite_model_config(cfg, max_model_len)
     if cfg.get("model_type") != "llama" and not any("Llama" in a for a in archs):
         raise ValueError(f"unsupported model architecture {archs or cfg.get('model_type')}: only Llama-family "
                          "decoders (RMSNorm, RoPE, GQA, SwiGLU) and OPT are implemented")
@@ -39,6 +41,39 @@ def model_config_from_hf(path: Path, max_model_len: int | None) -> ModelConfig:
                        n_kv_heads=cfg.get("num_key_value_heads", heads), ffn=cfg["intermediate_size"],
                        vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=float(cfg.get("rope_theta", 10000.0)),
                        rms_eps=float(cfg.get("rms_norm_eps", 1e-5)), max_model_len=max_model_len or min(derived, 8192))
+
+
+def _granite_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
+    """ibm-granite GraniteForCausalLM config.json -> the Llama stack plus its four scalars (vllm
+    model_executor/models/granite.py).  Variants the engine would serve wrongly are refused, each with its reason."""
+    hidden, heads = cfg["hidden_size"], cfg["num_attention_heads"]
+    head_dim = cfg.get("head_dim") or hidden // heads
+    problems = []
+    if cfg.get("attention_bias") or cfg.get("mlp_bias"):
+        problems.append("attention_bias / mlp_bias (the Llama stack has no projection biases)")
+    if cfg.get("rope_scaling"):
+        problems.append("rope_scaling")
+    rope = cfg.get("rope_parameters") or {}
+    if rope.get("rope_type", "default") != "default" or set(rope) - {"rope_type", "rope_theta"}:
+        problems.append(f"rope_parameters {rope} (only the default rotary embedding is implemented)")
+    if head_dim != 128:
+        problems.append(f"head_dim {head_dim} (the attention kernels need 128; zero-padding smaller heads does not "
+                        "commute with RoPE)")
+    if problems:
+        raise ValueError("unsupported Granite variant: " + "; ".join(problems))
+    derived = cfg.get("max_position_embeddings", 4096)
+    if max_model_len is not None and max_model_len > derived:
+        raise ValueError(f"max_model_len {max_model_len} exceeds the model's max_position_embeddings {derived}")
+    theta = rope.get("rope_theta", cfg.get("rope_theta", 10000.0))
+    return ModelConfig(n_layers=cfg["num_hidden_layers"], hidden=hidden, n_q_heads=heads,
+                       n_kv_heads=cfg.get("num_key_value_heads", heads), ffn=cfg["intermediate_size"],
+                       vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=float(theta),
+                       rms_eps=float(cfg.get("rms_norm_eps", 1e-6)), max_model_len=max_model_len or min(derived, 8192),
+                       tie_word_embeddings=bool(cfg.get("tie_word_embeddings", True)),
+                       embedding_multiplier=float(cfg.get("embedding_multiplier", 1.0)),
+                       residual_multiplier=float(cfg.get("residual_multiplier", 1.0)),
+                       attention_multiplier=float(cfg.get("attention_multiplier") or 0.0),
+                       logits_scaling=float(cfg.get("logits_scaling", 1.0)))
 
 
 def _opt_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
@@ -116,7 +151,8 @@ def load_synthetic_weights(eng: NativeEngine, mc: ModelConfig, seed: int, device
     q_dim, kv_dim = mc.n_q_heads * mc.head_dim, mc.n_kv_heads * mc.head_dim
     ones = torch.ones(mc.hidden, dtype=torch.bfloat16, device=f"cuda:{device}")
     eng.load_weight("model.embed_tokens.weight", rnd(mc.vocab, mc.hidden))
-    eng.load_weight("lm_head.weight", rnd(mc.vocab, mc.hidden))
+    if not mc.tie_word_embeddings:   # tied (Granite): the engine copies embed_tokens into the lm_head at start
+        eng.load_weight("lm_head.weight", rnd(mc.vocab, mc.hidden))
     eng.load_weight("model.norm.weight", ones)
     for i in range(mc.n_layers):
         p = f"model.layers.{i}."
