@@ -209,6 +209,17 @@ int tgis_engine_load_weight(tgis_engine* e, const char* name, const void* ptr, i
  * The defaults 1, 1, 0, 1 are the Llama stack, bit for bit. */
 int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, float residual_multiplier,
                                   float attention_multiplier, float logit_scale);
+/* Automatic prefix caching (vLLM's enable_prefix_caching; default off here, on in vLLM).  Valid only between
+ * tgis_engine_create and tgis_engine_start.  A full 32-token KV block that a completed step wrote is keyed by (its
+ * parent's key, its 32 token ids, LoRA slot + the slot's generation, bumped by every clear / weight load of the slot);
+ * a new request reuses the blocks of its longest cached prefix, leaving at least one prompt token to compute.
+ * Unreferenced cached blocks are evicted least recently used first; tgis_status.free_blocks counts them as free.
+ * Requests with prompt_logprobs > 0 do not read the cache.  With caching on, prefill sequences of at most 128 query
+ * rows over at least 1024 earlier tokens run on the split-context attention kernel. */
+int tgis_engine_set_prefix_caching(tgis_engine* e, int32_t on);
+/* cumulative tokens looked up / found in the cache (vllm:prefix_cache_queries / _hits: as in vLLM, the lookups of a
+ * preempted request's recompute are not counted) and the keyed blocks right now */
+int tgis_engine_prefix_cache_stats(tgis_engine* e, int64_t* queried_tokens, int64_t* hit_tokens, int32_t* cached_blocks);
 int tgis_engine_start(tgis_engine* e);
 int tgis_engine_add_request(tgis_engine* e, const char* request_id, const int32_t* prompt_ids, int32_t n_prompt,
                             const tgis_sampling_params* params);

@@ -65,6 +65,17 @@ int tgis_k_gemm_norm_chain(const void* a_dev, int32_t a_rows_alloc, const void* 
 int tgis_k_attention(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, const int32_t* seqs_host,
                      int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride, void* out_dev,
                      int32_t n_q, int32_t n_kv, float scale);
+/* tgis_k_attention with a choice of prefill kernel: mode 0 = the existing prefill kernel (tgis_k_attention), 1 = the
+ * split-context cluster kernel for every prefill sequence, 2 = the engine's selection with prefix caching on (split-context
+ * for q_len <= 128 over >= 1024 earlier tokens, the existing kernel otherwise; two PDL-chained launches) */
+int tgis_k_attention_split(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                           const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
+                           int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale, int32_t mode);
+/* same, prefill launches only (decode sequences are skipped), timed over `iters` calls; us_out = avg device us per call */
+int tgis_k_attention_split_bench(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                                 const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                                 int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv,
+                                 float scale, int32_t mode, int32_t iters, float* us_out);
 /* this step's K / V rows written into the cache, then tgis_k_attention's launches, on one stream with no synchronisation
  * in between (the engine's layer step: the decode kernel streams cache blocks of earlier steps while the writer drains).
  * writer 0: RoPE + KV scatter (tgis_k_rope_kv) on qkv_dev in place, x_dev / w_dev / K unused; writer 1: qkv_dev = x . w^T

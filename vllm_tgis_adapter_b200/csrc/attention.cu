@@ -13,7 +13,10 @@
 //                      last-arriving split combines partials in split order (deterministic).
 // prefill (q_len >= 1): grid (16-query tile, kv_head); one warp per query head of the group; mma.sync m16n8k16 with
 //                      online softmax; KV blocks double-buffered through smem by TMA bulk copies.
+//                      Split-context variant (prefix-cache hits: a short suffix over a long cached context): a cluster of
+//                      PF_CLUSTER CTAs per (tile, kv head) splits the context and merges through DSMEM.
 #include <algorithm>
+#include <atomic>
 
 #include "kernels.h"
 #include "launch.cuh"
@@ -553,25 +556,41 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
 
 // ================================================================================================ prefill
 constexpr int PF_QROWS = 16;  // query tokens per tile
+static_assert(PF_QROWS % PF_CLUSTER == 0, "every CTA of a split cluster merges the same number of rows");
+constexpr int PF_SPLIT_SMEM_MAX = PF_QROWS * HEAD_DIM * 4 * 8;  // G = 8: the fp32 partial O of 8 heads x 16 rows
 
-// grid (n_tiles, n_kv); blockDim = 32 * G (warp = query head inside the GQA group)
+// grid (n_tiles, n_kv) / SPLIT: (n_tiles * PF_CLUSTER, n_kv) in clusters of PF_CLUSTER; blockDim = 32 * G (warp = query
+// head inside the GQA group).
+// SPLIT (split-context prefill): the PF_CLUSTER CTAs of a cluster share one (tile, kv head); CTA rank r streams the r-th
+// contiguous near-equal share of the tile's causal block range with the same per-block arithmetic, leaves its (o, m, l)
+// partial in its own shared memory (the KV stages once they are drained; dynamic shared memory, G * 8 KiB when that is
+// more), and after a cluster barrier merges the partials of rows [r * 16 / PF_CLUSTER, ...) from every rank through
+// distributed shared memory, in rank order, in fp32.  No global workspace and no atomics: the same bits on every run,
+// and the split points depend only on the tile's own block range.
+template <bool SPLIT>
 __global__ void __launch_bounds__(256)
 attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv_bfloat16* __restrict__ k_cache,
                     const __nv_bfloat16* __restrict__ v_cache, const AttnSeq* __restrict__ seqs,
                     const int32_t* __restrict__ tile_seq, const int32_t* __restrict__ tile_q0,
                     const int32_t* __restrict__ block_table, int bt_stride, __nv_bfloat16* __restrict__ out,
                     int out_ld, int n_kv, int G, float scale) {
-  __shared__ __align__(128) uint8_t kv_s[2 * 2 * TILE_BYTES];  // 2 stages x (K | V)
+  __shared__ __align__(128) uint8_t kv_static[SPLIT ? 16 : 2 * 2 * TILE_BYTES];  // 2 stages x (K | V)
+  extern __shared__ __align__(128) uint8_t kv_dyn[];
+  uint8_t* kv_s = SPLIT ? kv_dyn : kv_static;
   __shared__ uint64_t bars[2];
   griddep_launch();
   griddep_wait();
-  const int tile = blockIdx.x, kvh = blockIdx.y;
+  const int crank = SPLIT ? (int)cluster_ctarank() : 0;
+  const int tile = SPLIT ? blockIdx.x / PF_CLUSTER : blockIdx.x, kvh = blockIdx.y;
   const AttnSeq sq = seqs[tile_seq[tile]];
   const int q0 = tile_q0[tile];                      // first query (index within this step's q_len)
   const int n_rows = min(PF_QROWS, sq.q_len - q0);   // valid query rows in the tile
   const int pos0 = sq.kv_len - sq.q_len + q0;        // absolute position of row 0
   const int last_pos = pos0 + n_rows - 1;
   const int n_blk = last_pos / KV_BLOCK + 1;
+  // blocks [jb0, jb1) of the causal range are this CTA's (all of them without SPLIT; may be empty with SPLIT)
+  const int jb0 = SPLIT ? crank * n_blk / PF_CLUSTER : 0;
+  const int jb1 = SPLIT ? (crank + 1) * n_blk / PF_CLUSTER : n_blk;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int head = kvh * G + warp;
@@ -584,15 +603,15 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   __syncthreads();
   const int32_t* bt = block_table + (size_t)sq.block_row * bt_stride;
   auto issue = [&](int j) {
-    const int st = j & 1;
+    const int st = (j - jb0) & 1;
     const size_t tl = ((size_t)bt[j] * n_kv + kvh) * (KV_BLOCK * HEAD_DIM);
     mbar_arrive_expect_tx(&bars[st], 2 * TILE_BYTES);
     bulk_load_1d(kv_s + st * 2 * TILE_BYTES, k_cache + tl, TILE_BYTES, &bars[st]);
     bulk_load_1d(kv_s + st * 2 * TILE_BYTES + TILE_BYTES, v_cache + tl, TILE_BYTES, &bars[st]);
   };
   if (threadIdx.x == 0) {
-    issue(0);
-    if (n_blk > 1) issue(1);
+    if (jb1 > jb0) issue(jb0);
+    if (jb1 > jb0 + 1) issue(jb0 + 1);
   }
 
   // Q fragments (A operand), rows g and g+8 of the tile; rows past n_rows are clamped (results discarded)
@@ -618,9 +637,9 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   const float sl2 = scale * 1.4426950408889634f;  // exp2 domain
   const int row_pos[2] = {pos0 + g, pos0 + g + 8};
 
-  for (int j = 0; j < n_blk; ++j) {
-    const int st = j & 1;
-    mbar_wait(&bars[st], (j >> 1) & 1);
+  for (int j = jb0; j < jb1; ++j) {
+    const int st = (j - jb0) & 1;
+    mbar_wait(&bars[st], ((j - jb0) >> 1) & 1);
     const uint8_t* k_t = kv_s + st * 2 * TILE_BYTES;
     const uint8_t* v_t = k_t + TILE_BYTES;
     // ---- S = Q K^T : 4 n-tiles (8 tokens each) x 8 k-steps
@@ -699,13 +718,66 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
       }
     }
     __syncthreads();  // every warp is done with stage st
-    if (threadIdx.x == 0 && j + 2 < n_blk) issue(j + 2);
+    if (threadIdx.x == 0 && j + 2 < jb1) issue(j + 2);
   }
   // ---- normalise and store
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 1);
     l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 2);
+  }
+  if constexpr (SPLIT) {
+    // partial of this rank: po [head][row][dim] fp32 over the drained KV stages (the loop ended on a __syncthreads and
+    // no copy is in flight), (m, l) per (head, row); a rank with no blocks leaves m = -inf, l = 0, o = 0
+    __shared__ __align__(16) float4 ml_s[8 * PF_QROWS];
+    float* po = reinterpret_cast<float*>(kv_dyn);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = g + r * 8;
+      float* dst = po + (size_t)(warp * PF_QROWS + row) * HEAD_DIM + t * 2;
+#pragma unroll
+      for (int nd = 0; nd < 16; ++nd)
+        *reinterpret_cast<float2*>(dst + nd * 8) = make_float2(o[nd][r * 2], o[nd][r * 2 + 1]);
+      if (t == 0) ml_s[warp * PF_QROWS + row] = make_float4(m_r[r], l_r[r], 0.f, 0.f);
+    }
+    cluster_sync_all();
+    // merge: this CTA writes rows crank * RPC .. + RPC of every head; 16 threads per (head, row), 8 dims each
+    constexpr int RPC = PF_QROWS / PF_CLUSTER;
+    const int pr = threadIdx.x >> 4;
+    const int hd = pr / RPC, row = crank * RPC + pr % RPC, d0 = (threadIdx.x & 15) * 8;
+    const int idx = hd * PF_QROWS + row;
+    float2 mlk[PF_CLUSTER];
+    float m_f = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < PF_CLUSTER; ++k) {
+      const float4 v = ld_dsmem_f4(dsmem_addr(smem_u32(&ml_s[idx]), k));
+      mlk[k] = make_float2(v.x, v.y);
+      m_f = fmaxf(m_f, v.x);
+    }
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float l_f = 0.f;
+    const uint32_t po_addr = smem_u32(po + (size_t)idx * HEAD_DIM + d0);
+#pragma unroll
+    for (int k = 0; k < PF_CLUSTER; ++k) {
+      const float fs = (mlk[k].x == -INFINITY) ? 0.f : exp2f(mlk[k].x - m_f);
+      const float4 a = ld_dsmem_f4(dsmem_addr(po_addr, k));
+      const float4 b = ld_dsmem_f4(dsmem_addr(po_addr + 16, k));
+      l_f += mlk[k].y * fs;
+      acc[0] += a.x * fs; acc[1] += a.y * fs; acc[2] += a.z * fs; acc[3] += a.w * fs;
+      acc[4] += b.x * fs; acc[5] += b.y * fs; acc[6] += b.z * fs; acc[7] += b.w * fs;
+    }
+    cluster_sync_all();  // no CTA leaves while a peer may still read its shared memory
+    if (row < n_rows) {
+      const float inv = 1.f / l_f;
+      __nv_bfloat16* dst = out + (size_t)(sq.q_start + q0 + row) * out_ld + (size_t)(kvh * G + hd) * HEAD_DIM + d0;
+      uint4 pk;
+      pk.x = pack_bf16x2(acc[0] * inv, acc[1] * inv);
+      pk.y = pack_bf16x2(acc[2] * inv, acc[3] * inv);
+      pk.z = pack_bf16x2(acc[4] * inv, acc[5] * inv);
+      pk.w = pack_bf16x2(acc[6] * inv, acc[7] * inv);
+      *reinterpret_cast<uint4*>(dst) = pk;
+    }
+    return;
   }
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -729,8 +801,35 @@ cudaError_t attn_prefill_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv
   const int G = n_q / n_kv;
   if (G > 8) return cudaErrorInvalidValue;
   dim3 grid(n_tiles, n_kv);
-  return launch_k(attn_prefill_kernel, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq,
-                  tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale);
+  return launch_k(attn_prefill_kernel<false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
+                  tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale);
+}
+
+cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
+                                      const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
+                                      const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
+                                      __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
+                                      cudaStream_t stream) {
+  if (n_tiles <= 0) return cudaSuccess;
+  if (n_q % n_kv != 0) return cudaErrorInvalidValue;
+  const int G = n_q / n_kv;
+  if (G > 8) return cudaErrorInvalidValue;
+  // the shared-memory opt-in is per device: one bit per device ordinal, set once (racing setters set the same value)
+  static std::atomic<uint64_t> attr_set{0};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  const uint64_t bit = dev < 64 ? 1ull << dev : 0ull;
+  if (!(attr_set.load(std::memory_order_acquire) & bit)) {
+    e = cudaFuncSetAttribute(attn_prefill_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PF_SPLIT_SMEM_MAX);
+    if (e != cudaSuccess) return e;
+    attr_set.fetch_or(bit, std::memory_order_release);
+  }
+  const int smem = std::max(2 * 2 * TILE_BYTES, G * PF_QROWS * HEAD_DIM * 4);
+  dim3 grid(n_tiles * PF_CLUSTER, n_kv);
+  return launch_k_cluster(attn_prefill_kernel<true>, grid, dim3(32 * G), (size_t)smem, stream, PF_CLUSTER, qkv, qkv_ld,
+                          k_cache, v_cache, seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G,
+                          scale);
 }
 
 }  // namespace tgis

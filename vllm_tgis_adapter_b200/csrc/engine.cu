@@ -10,6 +10,8 @@
 //       All per-step metadata is packed into ONE pinned staging buffer and shipped with ONE H2D copy; results come
 //       back with ONE D2H copy of SampleOut records.
 #include <algorithm>
+#include <array>
+#include <list>
 #include <set>
 #include <atomic>
 #include <chrono>
@@ -117,6 +119,12 @@ struct Request {
   bool aborted = false;
   uint64_t seed = 0;
   int guided_fed = 0;  // generated tokens already reported to the mask provider (guided decoding)
+  // prefix caching: leading full blocks whose key is settled (registered or hit), the cache-entry uid of the last of
+  // them (parent of the next key), and the adapter generation this admission runs under
+  int pc_reg = 0;
+  uint64_t pc_chain = 0;
+  uint32_t lora_gen = 0;
+  bool preempted = false;  // recomputes after a preemption (not counted again in the prefix-cache statistics)
   double ts_arrival = 0, ts_first_sched = 0, ts_first_token = 0, ts_last_token = 0;
   int n_out() const { return (int)tokens.size() - n_prompt; }
 };
@@ -162,7 +170,7 @@ struct StepHeader {
   int32_t kind;          // 0: engine step; 1: prompt-logprob pass over R rows of the step just executed (T = its tokens,
   int32_t need_norm;     //    need_norm: the final RMSNorm has not run yet)
   int32_t lg_idx;        // index of this plan's logits gather inside the step (epoch = staged base + lg_idx)
-  int32_t pad;
+  int32_t n_ctiles;      // the last n_ctiles of the n_tiles prefill tiles run on the split-context kernel (prefix caching)
 };
 struct ShmCtl {
   std::atomic<uint64_t> seq;
@@ -190,6 +198,26 @@ __global__ void gather_relayout_kernel(const uint4* __restrict__ gathered, uint4
     out[(size_t)r * tp * Vl16 + (size_t)rk * Vl16 + v] = gathered[i];
   }
 }
+
+// Prefix caching: the identity of a full KV block's content.  parent = uid of the cache entry of the block before it (0:
+// the first block of a sequence), so a key names the whole token prefix; the adapter is (LoRA slot, its generation).
+// Keys are compared field by field (all 32 token ids included): a hash collision can never give a wrong hit.
+struct PcKey {
+  uint64_t parent = 0;
+  int32_t lora_slot = 0;
+  uint32_t lora_gen = 0;
+  std::array<int32_t, KV_BLOCK> toks{};
+  bool operator==(const PcKey& o) const {
+    return parent == o.parent && lora_slot == o.lora_slot && lora_gen == o.lora_gen && toks == o.toks;
+  }
+};
+struct PcKeyHash {
+  size_t operator()(const PcKey& k) const {
+    uint64_t h = k.parent * 0x9E3779B97F4A7C15ull ^ ((uint64_t)(uint32_t)k.lora_slot << 32 | k.lora_gen);
+    for (int32_t t : k.toks) h = (h ^ (uint32_t)t) * 0x100000001B3ull;
+    return (size_t)(h ^ (h >> 29));
+  }
+};
 
 constexpr int N_BT = 5;
 const int BT_VALUES[N_BT] = {16, 32, 64, 128, 256};
@@ -245,6 +273,29 @@ struct tgis_engine {
   size_t kv_layer_elems = 0;
   int num_blocks = 0;
   std::vector<int32_t> free_blocks;
+  // prefix caching (tgis_engine_set_prefix_caching; rank 0's scheduler only): per block a reference count and, for a
+  // full block whose KV a completed step wrote, its cache entry.  A keyed block nobody references sits in the evictable
+  // LRU (front = least recently used) and keeps its key until it is reallocated.
+  bool prefix_caching = false;
+  struct PcBlock {
+    int ref = 0;
+    uint64_t uid = 0;            // cache entry id (0: not keyed)
+    const PcKey* key = nullptr;  // its key inside pc_map
+    std::list<int>::iterator lru_it;  // valid while ref == 0 and uid != 0 (the block is evictable)
+  };
+  std::vector<PcBlock> pcb;
+  std::unordered_map<PcKey, int, PcKeyHash> pc_map;
+  std::list<int> pc_lru;
+  uint64_t pc_uid = 0;
+  std::unique_ptr<std::atomic<uint32_t>[]> lora_gen;  // per adapter slot, bumped by every clear / weight load
+  std::atomic<long long> pc_queried{0}, pc_hits{0};
+  // tokens a hit skips still belong to the repetition-penalty set (seen_bitmap): (slot, token) pairs of this step's hits,
+  // shipped with one copy and marked by one bitmap_set launch in front of the step
+  std::vector<int32_t> pc_seen_slot, pc_seen_tok;
+  int32_t* pc_seen_h = nullptr;  // pinned [2][cap]
+  DevBuf<int32_t> pc_seen_d;     // [2][cap]
+  size_t pc_seen_cap = 0;
+  int step_ctiles = 0;  // of the step being launched (StepHeader::n_ctiles)
   // activations
   DevBuf<bf16> resid, xn, qkv, attn_out, tmp, act, last_hidden;
   // lm_head output [rows, V].  bf16 = the model dtype, rounded once from the fp32 accumulator exactly where vLLM's
@@ -304,11 +355,12 @@ struct tgis_engine {
   // stats
   std::atomic<long long> n_steps{0}, n_tokens{0}, n_launches{0}, n_preempt{0};
   // scheduler-state snapshot for tgis_engine_status (the queues themselves belong to the engine thread)
-  std::atomic<int> snap_running{0}, snap_waiting{0}, snap_free_blocks{0};
+  std::atomic<int> snap_running{0}, snap_waiting{0}, snap_free_blocks{0}, snap_cached_blocks{0};
   void snapshot() {
     snap_running = (int)running.size();
     snap_waiting = (int)waiting.size();
-    snap_free_blocks = (int)free_blocks.size();
+    snap_free_blocks = (int)(free_blocks.size() + pc_lru.size());  // evictable cached blocks count as free
+    snap_cached_blocks = (int)pc_map.size();
   }
   double gpu_ms = 0, gpu_ms_decode = 0, gpu_ms_mixed = 0;
   long long decode_steps = 0, decode_tokens = 0, h2d_bytes = 0, d2h_bytes = 0;
@@ -390,6 +442,7 @@ struct tgis_engine {
     }
     if (h_stage) cudaFreeHost(h_stage);
     if (h_samp_out) cudaFreeHost(h_samp_out);
+    if (pc_seen_h) cudaFreeHost(pc_seen_h);
     if (h_allow) cudaFreeHost(h_allow);
     if (h_plp_out) cudaFreeHost(h_plp_out);
     if (shm) {
@@ -524,6 +577,7 @@ struct tgis_engine {
     tmp.alloc(T_alloc * H);
     act.alloc(T_alloc * F);
     if (opt) y32.alloc(T_alloc * std::max<size_t>({(size_t)qkv_dim, F, H}));
+    lora_gen.reset(new std::atomic<uint32_t>[std::max(c.max_loras, 0) + 1]());
     if (c.max_loras > 0) {
       max_loras = c.max_loras;
       lora_R = c.max_lora_rank;
@@ -1009,6 +1063,7 @@ struct tgis_engine {
   }
   int clear_adapter(int32_t slot) {
     if (int rc = lora_slot_check(slot)) return rc;
+    ++lora_gen[slot];  // blocks cached under the slot's earlier contents are never hit again
     CK(cudaSetDevice(cfg.device));
     lora_for_each(slot, [&](bf16* p, size_t n) { CK(cudaMemset(p, 0, n * sizeof(bf16))); });
     CK(cudaStreamSynchronize(cudaStreamLegacy));
@@ -1021,6 +1076,7 @@ struct tgis_engine {
     if (dot == std::string::npos) return fail("bad adapter weight name " + name);
     const int li = atoi(name.substr(7, dot - 7).c_str());
     if (li < 0 || li >= cfg.n_layers) return fail("layer index out of range in " + name);
+    ++lora_gen[slot];
     const std::string rest = name.substr(dot + 1);
     const size_t dot2 = rest.find('.');
     if (dot2 == std::string::npos) return fail("bad adapter weight name " + name);
@@ -1124,6 +1180,25 @@ struct tgis_engine {
   // quantity from the device staging buffer, so the same sequence can be captured once into a CUDA graph and replayed.
   size_t items_off(int S) const { return (off_bt + sizeof(int32_t) * (size_t)S * bt_stride + 255) / 256 * 256; }
 
+  // Prefill attention of a step: the tiles of the existing kernel, then (PDL-chained, prefix caching only) the last
+  // step_ctiles tiles on the split-context kernel.
+  void prefill_attention(const bf16* kc, const bf16* vc, float scale, int n_tiles) {
+    const AttnSeq* d_seqs = ds<AttnSeq>(off_seqs);
+    const int32_t* d_bt = ds<int32_t>(off_bt);
+    const int n_std = n_tiles - step_ctiles;
+    if (n_std > 0) {
+      CK(attn_prefill_launch(qkv.p, qkv_dim, kc, vc, d_seqs, ds<int32_t>(off_tileseq), ds<int32_t>(off_tileq0), n_std,
+                             d_bt, bt_stride, attn_out.p, q_dim, nq, nkv, scale, stream));
+      ++n_launches;
+    }
+    if (step_ctiles > 0) {
+      CK(attn_prefill_split_launch(qkv.p, qkv_dim, kc, vc, d_seqs, ds<int32_t>(off_tileseq) + n_std,
+                                   ds<int32_t>(off_tileq0) + n_std, step_ctiles, d_bt, bt_stride, attn_out.p, q_dim, nq,
+                                   nkv, scale, stream));
+      ++n_launches;
+    }
+  }
+
   void launch_step(size_t copy_bytes, int T, int n_dec, int n_tiles, int R, int max_dec_kv, int S, int samp_complex) {
     const tgis_config& c = cfg;
     const int H = c.hidden, F = Fl, V = c.vocab;  // F: local ffn shard
@@ -1225,11 +1300,7 @@ struct tgis_engine {
                               nkv, scale, num_sms, stream, attn_arrive.p));
         n_launches += (max_splits > 1 && !attn_inkernel_merge) ? 2 : 1;
       }
-      if (n_tiles > 0) {
-        CK(attn_prefill_launch(qkv.p, qkv_dim, kc, vc, d_seqs, ds<int32_t>(off_tileseq), ds<int32_t>(off_tileq0),
-                               n_tiles, d_bt, bt_stride, attn_out.p, q_dim, nq, nkv, scale, stream));
-        ++n_launches;
-      }
+      if (n_tiles > 0) prefill_attention(kc, vc, scale, n_tiles);
       gemm(xm_attn, l.m_o, attn_out.p, l.wo, ar_fused ? ar_buf(0) : tmp.p, T, H, q_dim, 0, &l.m_gu, T, 2 * F, H, 0, nullptr,
            norm_fused ? &prod_attn : nullptr);
       if (lora) {
@@ -1332,11 +1403,7 @@ struct tgis_engine {
                               nkv, attn_scale, num_sms, stream, attn_arrive.p));
         n_launches += (max_splits > 1 && !attn_inkernel_merge) ? 2 : 1;
       }
-      if (n_tiles > 0) {
-        CK(attn_prefill_launch(qkv.p, qkv_dim, kc, vc, d_seqs, ds<int32_t>(off_tileseq), ds<int32_t>(off_tileq0),
-                               n_tiles, d_bt, bt_stride, attn_out.p, q_dim, nq, nkv, attn_scale, stream));
-        ++n_launches;
-      }
+      if (n_tiles > 0) prefill_attention(kc, vc, attn_scale, n_tiles);
       gemm(xm_attn, l.m_o, attn_out.p, l.wo, y32.p, T, H, q_dim, /*out_f32=*/1, &l.m_gu, T, F, H);
       CK(opt_layernorm_launch(y32.p, l.b_o, resid.p, l.ln2, l.ln2_b, xn.p, T, H, c.rms_eps, stream));
       gemm(xm_xn, l.m_gu, xn.p, l.wgu, y32.p, T, F, H, /*out_f32=*/1, &l.m_d, T, H, F);
@@ -1440,6 +1507,7 @@ struct tgis_engine {
   // buffer, so the captured launch sequence is step-independent -- or the plain launch sequence otherwise.  Rank 0
   // and the tensor-parallel workers run the same function on the same header.
   void exec_step(const StepHeader& h) {
+    step_ctiles = h.kind == 0 ? h.n_ctiles : 0;
     if (h.kind == 1) {
       plp_pass(h.R, h.need_norm, h.T, h.copy_bytes, h.lg_idx);
       return;
@@ -1492,6 +1560,7 @@ struct tgis_engine {
     const tgis_config& c = cfg;
     const int H = c.hidden, V = c.vocab;
     int T = 0, n_dec = 0, n_tiles = 0, R = 0, max_dec_kv = 0, samp_complex = 0;
+    std::vector<int32_t> ctile_seq, ctile_q0;  // split-context tiles (prefix caching): listed after the others
     struct PromptRow {
       int row, target, pos;
       Request* r;
@@ -1535,6 +1604,11 @@ struct tgis_engine {
       if (q_len == 1) {
         decids[n_dec++] = s;
         max_dec_kv = std::max(max_dec_kv, kv_len);
+      } else if (prefix_caching && prefill_split_pick(q_len, kv_len)) {
+        for (int q0 = 0; q0 < q_len; q0 += 16) {
+          ctile_seq.push_back(s);
+          ctile_q0.push_back(q0);
+        }
       } else {
         for (int q0 = 0; q0 < q_len; q0 += 16) {
           tileseq[n_tiles] = s;
@@ -1605,6 +1679,11 @@ struct tgis_engine {
       }
       T += q_len;
     }
+    const int n_ctiles = (int)ctile_seq.size();
+    for (int i = 0; i < n_ctiles; ++i) {
+      tileseq[n_tiles] = ctile_seq[i];
+      tileq0[n_tiles++] = ctile_q0[i];
+    }
     // ---- ship metadata + run the layer stack (one CUDA graph launch for a pure-decode step when enabled)
     // decode work items: (sequence, DECODE_SPLIT-token split) entries; the copy covers the worst case for this
     // (S, max_splits) so that its size is a function of the CUDA-graph key
@@ -1614,7 +1693,8 @@ struct tgis_engine {
     const double t_ev0 = debug_launch ? now_s() : 0.0;
     CK(cudaEventRecord(ev0, stream));
     const bool graphable = cfg.use_cuda_graphs && (tp == 1 || tp_graphs) && !profiling && n_tiles == 0 && n_dec == S && R == S;
-    StepHeader hdr{T, n_dec, n_tiles, R, max_dec_kv, S, graphable ? 1 : 0, samp_complex, (uint64_t)copy_bytes, 0, 0, 1, 0};
+    StepHeader hdr{T, n_dec, n_tiles, R, max_dec_kv, S, graphable ? 1 : 0, samp_complex, (uint64_t)copy_bytes, 0, 0, 1,
+                   n_ctiles};
     if (tp > 1) {
       // exchange epochs of this step = staged base + index inside the step (ar_add_rmsnorm_kernel)
       uint32_t* eb = hs<uint32_t>(off_epoch);
@@ -1702,13 +1782,36 @@ struct tgis_engine {
 
   // ------------------------------------------------------------------------------------------------ scheduler
   void free_request(Request& r) {
-    for (int b : r.blocks) free_blocks.push_back(b);
+    if (prefix_caching) {
+      // tail first, so that a sequence's last blocks are evicted before its first ones (vLLM's order)
+      for (auto it = r.blocks.rbegin(); it != r.blocks.rend(); ++it) {
+        PcBlock& pb = pcb[*it];
+        if (--pb.ref > 0) continue;
+        if (pb.uid != 0) {
+          pb.lru_it = pc_lru.insert(pc_lru.end(), *it);
+        } else {
+          free_blocks.push_back(*it);
+        }
+      }
+      r.pc_reg = 0;
+      r.pc_chain = 0;
+    } else {
+      for (int b : r.blocks) free_blocks.push_back(b);
+    }
     r.blocks.clear();
     if (r.slot >= 0) free_slots.push_back(r.slot);
     r.slot = -1;
   }
   bool ensure_blocks(Request& r, int n_tokens) {
     const int need = (n_tokens + KV_BLOCK - 1) / KV_BLOCK;
+    if (prefix_caching) {
+      while ((int)r.blocks.size() < need) {
+        const int b = pc_alloc();
+        if (b < 0) return false;
+        r.blocks.push_back(b);
+      }
+      return true;
+    }
     while ((int)r.blocks.size() < need) {
       if (free_blocks.empty()) return false;
       r.blocks.push_back(free_blocks.back());
@@ -1716,6 +1819,87 @@ struct tgis_engine {
     }
     return true;
   }
+  // ---- prefix cache
+  // a block for a new owner: from the free list first, else the least recently used cached block (its key is dropped)
+  int pc_alloc() {
+    int b;
+    if (!free_blocks.empty()) {
+      b = free_blocks.back();
+      free_blocks.pop_back();
+    } else if (!pc_lru.empty()) {
+      b = pc_lru.front();
+      pc_lru.pop_front();
+      PcBlock& pb = pcb[b];
+      const PcKey k = *pb.key;
+      pc_map.erase(k);
+      pb.key = nullptr;
+      pb.uid = 0;
+    } else {
+      return -1;
+    }
+    pcb[b].ref = 1;
+    return b;
+  }
+  PcKey pc_key(const Request& r, int blk, uint64_t parent) const {
+    PcKey k;
+    k.parent = parent;
+    k.lora_slot = r.sp.lora_slot;
+    k.lora_gen = r.lora_gen;
+    std::copy(r.tokens.begin() + (size_t)blk * KV_BLOCK, r.tokens.begin() + (size_t)(blk + 1) * KV_BLOCK, k.toks.begin());
+    return k;
+  }
+  // the cached blocks holding r's leading full blocks; at least one token is left to compute (its logits are needed)
+  void pc_lookup(const Request& r, std::vector<int>& hit) const {
+    const int max_blocks = ((int)r.tokens.size() - 1) / KV_BLOCK;
+    uint64_t parent = 0;
+    for (int i = 0; i < max_blocks; ++i) {
+      auto it = pc_map.find(pc_key(r, i, parent));
+      if (it == pc_map.end()) break;
+      hit.push_back(it->second);
+      parent = pcb[it->second].uid;
+    }
+  }
+  // the repetition-penalty bits of the tokens this step's hits skipped (after the admissions' bitmap clears, before the
+  // step).  The pinned staging is reused only after the step has been waited for; growing it waits for the stream.
+  void pc_mark_seen() {
+    const size_t n = pc_seen_tok.size();
+    if (n > pc_seen_cap) {
+      CK(cudaStreamSynchronize(stream));
+      if (pc_seen_h) CK(cudaFreeHost(pc_seen_h));
+      pc_seen_cap = std::max(n, 2 * pc_seen_cap);
+      CK(cudaHostAlloc(&pc_seen_h, sizeof(int32_t) * 2 * pc_seen_cap, cudaHostAllocDefault));
+      if (pc_seen_d.p) CK(cudaFree(pc_seen_d.p));
+      pc_seen_d.p = nullptr;
+      pc_seen_d.alloc(2 * pc_seen_cap);
+    }
+    memcpy(pc_seen_h, pc_seen_slot.data(), sizeof(int32_t) * n);
+    memcpy(pc_seen_h + n, pc_seen_tok.data(), sizeof(int32_t) * n);
+    CK(cudaMemcpyAsync(pc_seen_d.p, pc_seen_h, sizeof(int32_t) * 2 * n, cudaMemcpyHostToDevice, stream));
+    CK(bitmap_set_launch(seen_bitmap.p, bitmap_words, pc_seen_d.p, pc_seen_d.p + n, (int)n, stream));
+    ++n_launches;
+    h2d_bytes += (long long)(sizeof(int32_t) * 2 * n);
+    pc_seen_slot.clear();
+    pc_seen_tok.clear();
+  }
+  // after a completed step: key every block of r that is now full.  Content that is cached already (an identical prompt
+  // that ran alongside) keeps its existing entry; r's own copy stays unkeyed and returns to the free list when released.
+  void pc_register(Request& r) {
+    const int full = r.n_computed / KV_BLOCK;
+    for (; r.pc_reg < full; ++r.pc_reg) {
+      PcKey k = pc_key(r, r.pc_reg, r.pc_chain);
+      auto it = pc_map.find(k);
+      if (it != pc_map.end()) {
+        r.pc_chain = pcb[it->second].uid;
+        continue;
+      }
+      const int b = r.blocks[r.pc_reg];
+      PcBlock& pb = pcb[b];
+      pb.uid = ++pc_uid;
+      pb.key = &pc_map.emplace(std::move(k), b).first->first;
+      r.pc_chain = pb.uid;
+    }
+  }
+
   void emit_prompt(const Request& r, int pos, const SampleOut& so) {
     tgis_step_output o;
     memset(&o, 0, sizeof(o));
@@ -1816,6 +2000,7 @@ struct tgis_engine {
         running.pop_back();
         free_request(*victim);
         victim->n_computed = 0;
+        victim->preempted = true;
         ++n_preempt;
         waiting.push_front(std::move(victim));
         ok = ensure_blocks(r, r.n_computed + q);
@@ -1825,6 +2010,7 @@ struct tgis_engine {
         running.pop_back();
         free_request(*victim);
         victim->n_computed = 0;
+        victim->preempted = true;
         ++n_preempt;
         waiting.push_front(std::move(victim));
         break;
@@ -1836,15 +2022,44 @@ struct tgis_engine {
     const double t_now = now_s();
     while (!waiting.empty() && budget > 0 && (int)running.size() < S_max && !free_slots.empty()) {
       Request& r = *waiting.front();
+      if (prefix_caching) {
+        // a hit is a chunked prefill whose first chunks an earlier request computed.  Evictable blocks count as free,
+        // hit blocks need no allocation: a request that fits with caching off always fits.  Requests that want prompt
+        // logprobs do not read the cache (vLLM: skip_reading_prefix_cache), but their blocks are registered.
+        r.lora_gen = r.sp.lora_slot > 0 ? lora_gen[r.sp.lora_slot].load() : 0;
+        std::vector<int> hit;
+        const bool read = r.sp.prompt_logprobs <= 0;
+        if (read) pc_lookup(r, hit);
+        int hit_evictable = 0;
+        for (int b : hit) hit_evictable += pcb[b].ref == 0 ? 1 : 0;
+        const int need = ((int)r.tokens.size() + KV_BLOCK) / KV_BLOCK - (int)hit.size();
+        if ((int)(free_blocks.size() + pc_lru.size()) - hit_evictable < need) break;
+        if (read && !r.preempted) {  // vLLM counts a preempted request's recompute apart (preempted_queries / _hits)
+          pc_queried += (long long)r.tokens.size();
+          pc_hits += (long long)hit.size() * KV_BLOCK;
+        }
+        for (int b : hit) {
+          PcBlock& pb = pcb[b];
+          if (pb.ref++ == 0) pc_lru.erase(pb.lru_it);
+          r.blocks.push_back(b);
+        }
+        r.n_computed = (int)hit.size() * KV_BLOCK;
+        r.pc_reg = (int)hit.size();
+        r.pc_chain = hit.empty() ? 0 : pcb[hit.back()].uid;
+      }
       const int remaining = (int)r.tokens.size() - r.n_computed;
       const int q = std::min(remaining, budget);
       // admit only if the whole sequence so far fits (keeps chunked prefill from dead-locking the cache)
-      if ((int)free_blocks.size() < ((int)r.tokens.size() + KV_BLOCK) / KV_BLOCK) break;
+      if (!prefix_caching && (int)free_blocks.size() < ((int)r.tokens.size() + KV_BLOCK) / KV_BLOCK) break;
       r.slot = free_slots.back();
       free_slots.pop_back();
       ensure_blocks(r, r.n_computed + q);
       CK(bitmap_clear_launch(seen_bitmap.p, bitmap_words, r.slot, stream));
       ++n_launches;
+      for (int p = 0; p < r.n_computed; ++p) {  // cache hit: these tokens never pass through a step
+        pc_seen_slot.push_back(r.slot);
+        pc_seen_tok.push_back(r.tokens[p]);
+      }
       if (r.ts_first_sched == 0) r.ts_first_sched = t_now;
       budget -= q;
       Sched s{&r, q, r.n_computed + q == (int)r.tokens.size()};
@@ -1852,6 +2067,7 @@ struct tgis_engine {
       running.push_back(std::move(waiting.front()));
       waiting.pop_front();
     }
+    if (!pc_seen_tok.empty()) pc_mark_seen();
     std::vector<Sched> batch;
     batch.reserve(dec.size() + pre.size());
     batch.insert(batch.end(), dec.begin(), dec.end());
@@ -1885,6 +2101,7 @@ struct tgis_engine {
     for (Sched& s : batch) {
       Request& r = *s.r;
       r.n_computed += s.q_len;
+      if (prefix_caching) pc_register(r);  // this step has completed: its full blocks become hittable
       if (!s.sample) continue;
       const SampleOut& so = h_samp_out[R++];
       r.tokens.push_back(so.token);
@@ -2048,6 +2265,22 @@ int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, fl
   e->attn_scale = attention_multiplier > 0.f ? attention_multiplier : 1.0f / std::sqrt((float)e->model_head_dim);
   // the TGIS_FUSE_NORM experiment folds the residual add into the GEMMs without the multiplier
   if (residual_multiplier != 1.f) e->fuse_norm = false;
+  return 0;
+}
+
+int tgis_engine_set_prefix_caching(tgis_engine* e, int32_t on) {
+  if (!e) return fail("null engine");
+  if (e->started) return fail("prefix caching must be set before tgis_engine_start");
+  e->prefix_caching = on != 0;
+  e->pcb.assign(e->prefix_caching ? e->num_blocks : 0, tgis_engine::PcBlock{});
+  return 0;
+}
+
+int tgis_engine_prefix_cache_stats(tgis_engine* e, int64_t* queried_tokens, int64_t* hit_tokens, int32_t* cached_blocks) {
+  if (!e || !queried_tokens || !hit_tokens || !cached_blocks) return fail("null argument");
+  *queried_tokens = e->pc_queried;
+  *hit_tokens = e->pc_hits;
+  *cached_blocks = e->snap_cached_blocks;
   return 0;
 }
 

@@ -282,22 +282,24 @@ namespace {
 // before anything is launched, so that the launches can follow a cache-writing kernel on the same stream with no
 // synchronisation in between, as in the engine's step.
 struct AttnCall {
-  int n_q = 0, n_kv = 0, n_dec = 0, n_tiles = 0, max_splits = 1, bt_stride = 0;
+  int n_q = 0, n_kv = 0, n_dec = 0, n_tiles = 0, n_ctiles = 0, max_splits = 1, bt_stride = 0;
   Tmp<AttnSeq> seqs;
   Tmp<int32_t> dec, tseq, tq0, bt;
   Tmp<float> po, pml;
   Tmp<DecItem> items;
   Tmp<int> arrive;  // arrival counters of the in-kernel split merge (the launcher ignores them when that path is off)
 
+  // split_mode: 0 every prefill tile on the existing kernel, 1 every one on the split-context kernel, 2 the engine's
+  // selection (prefill_split_pick); split-context tiles are listed last, as in the engine's step
   int prepare(const int32_t* seqs_host, int n_seqs, const int32_t* block_table_host, int bt_rows, int stride, int nq,
-              int nkv) {
+              int nkv, int split_mode = 0) {
     if (nkv <= 0 || nq % nkv) return kfail("bad head counts");
     n_q = nq;
     n_kv = nkv;
     bt_stride = stride;
     const int G = n_q / n_kv;
     std::vector<AttnSeq> h_seqs(n_seqs);
-    std::vector<int32_t> h_dec, h_tseq, h_tq0;
+    std::vector<int32_t> h_dec, h_tseq, h_tq0, c_tseq, c_tq0;
     int max_kv = 1;
     for (int s = 0; s < n_seqs; ++s) {
       h_seqs[s] = AttnSeq{seqs_host[4 * s], seqs_host[4 * s + 1], seqs_host[4 * s + 2], seqs_host[4 * s + 3]};
@@ -305,13 +307,18 @@ struct AttnCall {
         h_dec.push_back(s);
         max_kv = std::max(max_kv, h_seqs[s].kv_len);
       } else {
+        const bool split =
+            split_mode == 1 || (split_mode == 2 && prefill_split_pick(h_seqs[s].q_len, h_seqs[s].kv_len));
         for (int q0 = 0; q0 < h_seqs[s].q_len; q0 += 16) {
-          h_tseq.push_back(s);
-          h_tq0.push_back(q0);
+          (split ? c_tseq : h_tseq).push_back(s);
+          (split ? c_tq0 : h_tq0).push_back(q0);
         }
       }
     }
     n_dec = (int)h_dec.size();
+    n_ctiles = (int)c_tseq.size();
+    h_tseq.insert(h_tseq.end(), c_tseq.begin(), c_tseq.end());
+    h_tq0.insert(h_tq0.end(), c_tq0.begin(), c_tq0.end());
     n_tiles = (int)h_tseq.size();
     KCK(seqs.upload(h_seqs.data(), n_seqs));
     KCK(dec.upload(h_dec.data(), h_dec.size()));
@@ -329,15 +336,20 @@ struct AttnCall {
     KCK(cudaMemset(arrive.p, 0, sizeof(int) * nd * n_kv));
     return 0;
   }
-  // decode (+ split merge), then prefill: the engine's order
+  // decode (+ split merge), then prefill, then split-context prefill: the engine's order
   int launch(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, void* out_dev, float scale,
-             cudaStream_t st) {
+             cudaStream_t st, bool decode = true) {
     const int qkv_ld = (n_q + 2 * n_kv) * HEAD_DIM, out_ld = n_q * HEAD_DIM;
-    KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, items.p,
-                           n_dec * max_splits, seqs.p, dec.p, n_dec, max_splits, po.p, pml.p, (bf16*)out_dev, out_ld,
-                           n_q, n_kv, scale, test_num_sms(), st, arrive.p));
+    if (decode)
+      KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, items.p,
+                             n_dec * max_splits, seqs.p, dec.p, n_dec, max_splits, po.p, pml.p, (bf16*)out_dev, out_ld,
+                             n_q, n_kv, scale, test_num_sms(), st, arrive.p));
+    const int n_std = n_tiles - n_ctiles;
     KCK(attn_prefill_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, seqs.p,
-                            tseq.p, tq0.p, n_tiles, bt.p, bt_stride, (bf16*)out_dev, out_ld, n_q, n_kv, scale, st));
+                            tseq.p, tq0.p, n_std, bt.p, bt_stride, (bf16*)out_dev, out_ld, n_q, n_kv, scale, st));
+    KCK(attn_prefill_split_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev,
+                                  seqs.p, tseq.p + n_std, tq0.p + n_std, n_ctiles, bt.p, bt_stride, (bf16*)out_dev,
+                                  out_ld, n_q, n_kv, scale, st));
     return 0;
   }
 };
@@ -350,6 +362,44 @@ int tgis_k_attention(const void* qkv_dev, const void* k_cache_dev, const void* v
   if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv) != 0) return -1;
   if (call.launch(qkv_dev, k_cache_dev, v_cache_dev, out_dev, scale, 0) != 0) return -1;
   KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
+int tgis_k_attention_split(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                           const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
+                           int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale, int32_t mode) {
+  if (mode < 0 || mode > 2) return kfail("mode must be 0 (existing prefill kernel), 1 (split-context) or 2 (selection)");
+  AttnCall call;
+  if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv, mode) != 0) return -1;
+  if (call.launch(qkv_dev, k_cache_dev, v_cache_dev, out_dev, scale, 0) != 0) return -1;
+  KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
+// prefill attention only (decode sequences in seqs_host are skipped), timed: `iters` launches of the mode's prefill
+// kernels after two warm-up launches; us_out = average device microseconds per call
+int tgis_k_attention_split_bench(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                                 const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                                 int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv,
+                                 float scale, int32_t mode, int32_t iters, float* us_out) {
+  if (mode < 0 || mode > 2) return kfail("mode must be 0, 1 or 2");
+  if (iters < 1 || !us_out) return kfail("iters >= 1 and us_out are required");
+  AttnCall call;
+  if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv, mode) != 0) return -1;
+  cudaEvent_t e0, e1;
+  KCK(cudaEventCreate(&e0));
+  KCK(cudaEventCreate(&e1));
+  for (int it = -2; it < iters; ++it) {
+    if (it == 0) KCK(cudaEventRecord(e0, 0));
+    if (call.launch(qkv_dev, k_cache_dev, v_cache_dev, out_dev, scale, 0, /*decode=*/false) != 0) return -1;
+  }
+  KCK(cudaEventRecord(e1, 0));
+  KCK(cudaDeviceSynchronize());
+  float ms = 0.f;
+  KCK(cudaEventElapsedTime(&ms, e0, e1));
+  *us_out = ms * 1000.f / iters;
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
   return 0;
 }
 

@@ -130,7 +130,8 @@ class NativeEngine:
     def __init__(self, model: ModelConfig, *, max_num_seqs: int = 64, max_batched_tokens: int = 2048,
                  kv_cache_bytes: int = 0, gpu_mem_fraction: float = 0.85, device: int = 0, seed: int = 0,
                  debug_gemm_ref: bool = False, use_cuda_graphs: bool | None = None, tp_size: int = 1, tp_rank: int = 0,
-                 nccl_id: bytes | None = None, shm_name: str = "", max_loras: int = 0, max_lora_rank: int = 16):
+                 nccl_id: bytes | None = None, shm_name: str = "", max_loras: int = 0, max_lora_rank: int = 16,
+                 enable_prefix_caching: bool = False):
         self.lib = _lib.load_library()
         self.model = model
         if use_cuda_graphs is None:   # default on; TGIS_CUDA_GRAPHS=0 turns decode-step graph replay off
@@ -170,6 +171,11 @@ class NativeEngine:
             msg = _lib.last_error(self.lib)
             self.close()
             raise EngineError(f"tgis_engine_set_model_scalars failed: {msg}")
+        self.enable_prefix_caching = bool(enable_prefix_caching)
+        if self.enable_prefix_caching and self.lib.tgis_engine_set_prefix_caching(self._h, 1) != 0:
+            msg = _lib.last_error(self.lib)
+            self.close()
+            raise EngineError(f"tgis_engine_set_prefix_caching failed: {msg}")
         self._poll_buf = (TgisStepOutput * 512)()
 
     # -- weights ------------------------------------------------------------------------------------------------
@@ -251,6 +257,13 @@ class NativeEngine:
         st = TgisStatus()
         self.lib.tgis_engine_status(self._h, C.byref(st))
         return st
+
+    def prefix_cache_stats(self) -> tuple[int, int, int]:
+        """(tokens looked up in the prefix cache, tokens found there, keyed blocks now); all 0 with caching off."""
+        q, h, n = C.c_int64(0), C.c_int64(0), C.c_int32(0)
+        if self.lib.tgis_engine_prefix_cache_stats(self._h, C.byref(q), C.byref(h), C.byref(n)) != 0:
+            raise EngineError(_lib.last_error(self.lib))
+        return q.value, h.value, n.value
 
     @staticmethod
     def nccl_unique_id() -> bytes:

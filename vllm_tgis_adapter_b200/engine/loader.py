@@ -210,7 +210,8 @@ def _make_native_engine(args, mc: ModelConfig, path, device: int, **tp_kw) -> Na
     eng = NativeEngine(mc, max_num_seqs=args.max_num_seqs, max_batched_tokens=args.max_num_batched_tokens,
                        gpu_mem_fraction=args.gpu_memory_utilization, device=device, seed=args.seed,
                        max_loras=args.max_loras if getattr(args, "enable_lora", False) else 0,
-                       max_lora_rank=getattr(args, "max_lora_rank", 16), **tp_kw)
+                       max_lora_rank=getattr(args, "max_lora_rank", 16),
+                       enable_prefix_caching=bool(getattr(args, "enable_prefix_caching", False)), **tp_kw)
     if path is not None:
         load_safetensors_dir(eng, path)      # full tensors: a tensor-parallel engine keeps its rank's shard
     else:

@@ -16,7 +16,14 @@ def _metrics(engine) -> bytes:
         st = engine.engine.status()
     except Exception:  # noqa: BLE001
         st = None
-    return engine.metrics.render(st)
+    pc = None
+    stats = getattr(engine.engine, "prefix_cache_stats", None)
+    if stats is not None:
+        try:
+            pc = stats()[:2]
+        except Exception:  # noqa: BLE001
+            pc = None
+    return engine.metrics.render(st, pc)
 
 
 async def run_http_server(args, engine) -> None:

@@ -39,6 +39,15 @@ class EngineMetrics:
         self.queue_time = hist("vllm:request_queue_time_seconds", "Histogram of time spent in WAITING phase.", _LAT)
         self.req_prompt = hist("vllm:request_prompt_tokens", "Number of prefill tokens processed per request.", _TOK)
         self.req_gen = hist("vllm:request_generation_tokens", "Number of generation tokens processed per request.", _TOK)
+        # prefix caching, in tokens (vLLM V1's names); fed at scrape time with the increase of the engine's counters.
+        # As in vLLM, a request counts once: the recompute of a preempted request is not queried again.
+        self.prefix_cache_queries = Counter(
+            "vllm:prefix_cache_queries", "Prefix cache queries, in terms of number of queried tokens.", lab,
+            registry=self.registry).labels(*self._lv)
+        self.prefix_cache_hits = Counter(
+            "vllm:prefix_cache_hits", "Prefix cache hits, in terms of number of cached tokens.", lab,
+            registry=self.registry).labels(*self._lv)
+        self._pc_seen = (0, 0)
         self.steps = gauge("tgis_engine_steps", "Engine steps executed.")
         self.launches = gauge("tgis_engine_kernel_launches", "CUDA kernels launched by the engine.")
         self.gpu_busy = gauge("tgis_engine_gpu_busy_seconds", "Device time spent in engine steps.")
@@ -60,8 +69,14 @@ class EngineMetrics:
         if n_generated > 1 and last_token and first_token:
             self.tpot.observe(max(0.0, (last_token - first_token) / (n_generated - 1)))
 
-    def render(self, status) -> bytes:
-        """status: the engine's tgis_status (or None when the engine cannot be queried any more)."""
+    def render(self, status, prefix_cache: tuple[int, int] | None = None) -> bytes:
+        """status: the engine's tgis_status (or None when the engine cannot be queried any more); prefix_cache: the
+        engine's cumulative (queried tokens, hit tokens), or None."""
+        if prefix_cache is not None:
+            q, h = int(prefix_cache[0]), int(prefix_cache[1])
+            self.prefix_cache_queries.inc(max(0, q - self._pc_seen[0]))
+            self.prefix_cache_hits.inc(max(0, h - self._pc_seen[1]))
+            self._pc_seen = (max(q, self._pc_seen[0]), max(h, self._pc_seen[1]))
         if status is not None:
             self.running.set(status.n_running)
             self.waiting.set(status.n_waiting)

@@ -40,7 +40,7 @@ def _switch_action_default(action: argparse.Action) -> None:
     if not env_val:
         return
     if action.type is bool or type(action) in (argparse._StoreTrueAction, argparse._StoreFalseAction,  # noqa: SLF001
-                                               StoreBoolean):
+                                               StoreBoolean, argparse.BooleanOptionalAction):
         val: bool | str = _bool_from_string(env_val)
     else:
         val = env_val
@@ -98,6 +98,9 @@ def make_engine_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--enable-lora", action="store_true")
     p.add_argument("--max-loras", type=int, default=4, help="adapter slots resident on the GPU")
     p.add_argument("--max-lora-rank", type=int, default=16, help="rank capacity of a slot (multiple of 8, <= 64)")
+    # vLLM's flag pair (vllm config/cache.py enable_prefix_caching).  vLLM defaults to on; this engine defaults to off.
+    p.add_argument("--enable-prefix-caching", action=argparse.BooleanOptionalAction, default=False,
+                   help="reuse the KV blocks of prompt prefixes that earlier requests computed")
     return p
 
 
