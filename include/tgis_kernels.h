@@ -55,12 +55,6 @@ int tgis_k_rope_kv(void* qkv_dev, const int32_t* positions_host, const int32_t* 
 int tgis_k_gemm_rope(const void* x_dev, const void* w_dev, void* y_dev, int32_t T, int32_t n_q, int32_t n_kv, int32_t K,
                      int32_t x_rows_alloc, const int32_t* positions_host, const int32_t* slot_mapping_host,
                      const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev);
-/* a[T, K1] -> GEMM w1[H, K1] -> residual += . ; RMSNorm(residual) * w_norm -> GEMM w2[N2, H] (out_mode2: 0 bf16, 2 fused
- * SwiGLU) -> y2.  fused = 0: three launches (gemm, add_rmsnorm, gemm); fused = 1: the add + norm folded into the two GEMMs
- * (GemmNorm, kernels.h).  Returns 1 (nothing computed) when the launch plan cannot fuse the shape. */
-int tgis_k_gemm_norm_chain(const void* a_dev, int32_t a_rows_alloc, const void* w1_dev, void* residual_dev,
-                           const void* w_norm_dev, const void* w2_dev, void* y2_dev, int32_t T, int32_t K1, int32_t H,
-                           int32_t N2, float eps, int32_t out_mode2, int32_t fused, int32_t iters, float* us_out);
 /* seqs_host: n_seqs x {q_start, q_len, kv_len, block_row}; block_table_host: [rows][bt_stride] */
 int tgis_k_attention(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, const int32_t* seqs_host,
                      int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride, void* out_dev,
@@ -89,8 +83,6 @@ int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, 
 /* host-only: GEMM launch plan for a shape: token tile (16..256), grid, even-split factor (0: stream-K + global fix-up) */
 int tgis_k_gemm_plan(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* bt_out, int32_t* grid_out,
                      int32_t* even_split_out);
-/* weight rows per GEMM unit for a T-token launch (128 x weight tiles per shared activation tile) */
-int tgis_k_gemm_unit_rows(int32_t T);
 /* CTAs per SM of the GEMM instantiation a T-token launch runs (lean = 0: the one-CTA-per-SM instantiation) */
 int tgis_k_gemm_blocks_per_sm(int32_t T, int32_t lean, int32_t* out);
 /* host-only: the decode work-item list of a step (csrc/kernels.h DecItem: q_row, kv_len, seq | split << 16, 0,

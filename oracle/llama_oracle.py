@@ -22,8 +22,8 @@ HF-format Llama checkpoint.  Restated here, with the file:line each step follows
                      the model dtype, i.e. the fp32 accumulator rounded ONCE to bf16; the sampler then casts to fp32
                      (v1/sample/sampler.py:91).  Exact ties between bf16 logits (thousands per 128k-vocab row) are
                      therefore part of the reference's behaviour: they inflate `rank` and decide greedy argmax by
-                     lowest token id.  (Round 1 kept fp32 logits here and in the engine; `logits_fp32=True` restores
-                     that for the experiment switch TGIS_LOGITS_FP32.)
+                     lowest token id.  (Round 1 kept fp32 logits here and in the engine; `logits_fp32=True` keeps
+                     that variant of the reference for oracle-level comparisons; the engine always rounds to bf16.)
 
 PARITY PINNING: the reference's own tests hold no numeric golden vector for this path (SURVEY.md §8c: "parity
 unpinned" for token ids / logprobs).  This oracle is therefore pinned against the third-party implementation it

@@ -18,7 +18,6 @@ for st in $STAGES; do
     bench) timeout 900 python bench.py > gpurun_out/bench.log 2> gpurun_out/bench.err; echo "bench rc=$?" ;;
     bench_small) timeout 300 python bench.py --model small --batch 8 --prompt-len 128 --gen-len 32 --no-cpu-baseline > gpurun_out/bench_small.log 2> gpurun_out/bench_small.err; echo "bench_small rc=$?" ;;
     bench_modes) for gr in 0 1; do TGIS_CUDA_GRAPHS=$gr timeout 400 python bench.py --no-cpu-baseline --steps 2 --warmup 3 > gpurun_out/bench_graph${gr}.log 2> gpurun_out/bench_graph${gr}.err; done; echo "bench_modes rc=$?" ;;
-    bench_pf) for pf in 0 8 20 40; do TGIS_L2_PREFETCH_KB=$pf timeout 400 python bench.py --no-cpu-baseline --steps 2 --warmup 3 > gpurun_out/bench_pf${pf}.log 2> gpurun_out/bench_pf${pf}.err; done; echo "bench_pf rc=$?" ;;
     bench_gpu) timeout 600 python bench.py --no-cpu-baseline > gpurun_out/bench_gpu.log 2> gpurun_out/bench_gpu.err; echo "bench_gpu rc=$?" ;;
     bench_ref) timeout 400 python bench.py --impl reference --steps 1 --warmup 1 > gpurun_out/bench_ref.log 2> gpurun_out/bench_ref.err; echo "bench_ref rc=$?" ;;
     prof_list) timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv python scripts/profile_decode.py 4 32 512 6 0 > gpurun_out/prof_list.log 2>&1; echo "prof_list rc=$?" ;;

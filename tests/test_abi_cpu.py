@@ -93,7 +93,7 @@ def test_decode_work_items_host_logic():
                                    items.ctypes.data_as(C.POINTER(C.c_int32)), 3) == -1
 
 
-def test_gemm_launch_plan_host_logic():
+def test_gemm_launch_plan_host_logic_with_128_row_units():
     """Pure host arithmetic of the GEMM launcher (gemm_wgmma.cu): for the decode shapes of the 8B and 70B/TP8 layer
     stacks the plan must (a) never use more CTAs than SMs (the stream-K fix-up and the chain kernel rely on co-residency),
     (b) in even-split mode give every CTA a k-range inside ONE tile (the cluster epilogue reduces exactly one unit per
@@ -110,9 +110,7 @@ def test_gemm_launch_plan_host_logic():
                 bt, grid, split = bt.value, grid.value, split.value
                 assert bt >= T and bt in (16, 32, 64, 128, 256)
                 assert 1 <= grid <= sms
-                unit = lib.tgis_k_gemm_unit_rows(T)       # 128; 256 with the TGIS_GEMM_NW=2 experiment
-                assert unit in (128, 256)
-                n_tiles, kb = (N + unit - 1) // unit, (K + 63) // 64
+                n_tiles, kb = (N + 127) // 128, (K + 63) // 64          # a unit is one 128-row weight tile
                 total = n_tiles * kb
                 bounds = [total * c // grid for c in range(grid + 1)]
                 assert bounds[0] == 0 and bounds[-1] == total and all(b1 > b0 for b0, b1 in zip(bounds, bounds[1:]))

@@ -62,42 +62,6 @@ def test_gemm_fp32_output_for_logits(g):
     assert float((y - ref).abs().max()) < 2e-5 * float(ref.abs().max()) + 1e-5
 
 
-_NW2_CHILD = """
-import sys
-sys.path[:0] = [sys.argv[1], sys.argv[1] + "/tests"]
-import torch
-import tgis_gpu_utils as g
-assert g.lib().tgis_k_gemm_unit_rows(32) == 256 and g.lib().tgis_k_gemm_unit_rows(200) == 128
-for T, N, K in [(7, 256, 512), (16, 384, 4096), (32, 6144, 4096), (33, 1000, 520), (64, 4096, 14336), (128, 1024, 4096)]:
-    gen = torch.Generator(device="cuda").manual_seed(T * 7 + N + K)
-    x = (torch.randn(T, K, generator=gen, device="cuda") * 0.5).bfloat16()
-    w = (torch.randn(N, K, generator=gen, device="cuda") * 0.05).bfloat16()
-    y, _ = g.gemm(x, w)
-    ref = x.float() @ w.float().t()
-    ulp = g.bf16_ulp_diff(y, ref.bfloat16())
-    bad = (ulp > 1.01) & ((y.float() - ref).abs() > 1e-3 * ref.abs().mean())
-    assert int(bad.sum()) == 0, (T, N, K, float(ulp.max()))
-    assert float((ulp == 0).float().mean()) > 0.97, (T, N, K)
-    assert torch.equal(y, g.gemm(x, w)[0])
-print("NW2_OK")
-"""
-
-
-def test_gemm_two_weight_tiles_per_unit_experiment():
-    """TGIS_GEMM_NW=2 (off by default; read once per process, hence a child process): launches of at most 128 tokens
-    share one activation tile between two weight tiles (two accumulators per consumer thread).  Same tolerance as
-    test_gemm_tcgen05_matches_fp32_reference, bit-deterministic; larger token tiles keep one weight tile per unit."""
-    import os
-    import subprocess
-    import sys
-    from pathlib import Path
-
-    root = str(Path(__file__).resolve().parent.parent)
-    r = subprocess.run([sys.executable, "-c", _NW2_CHILD, root], env=dict(os.environ, TGIS_GEMM_NW="2"),
-                       capture_output=True, text=True, timeout=600)
-    assert "NW2_OK" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
-
-
 @pytest.mark.parametrize("T,F,K", [(32, 1536, 512), (7, 14336, 4096), (300, 1024, 256)])
 def test_gemm_fused_swiglu_epilogue(g, T, F, K):
     """gate_up GEMM with SwiGLU fused in the epilogue (rows interleaved gate_j, up_j) == GEMM -> bf16 -> silu*mul."""
@@ -258,45 +222,6 @@ def test_qkv_gemm_with_fused_rope_epilogue_is_bit_identical(g, T, heads):
     assert float(kc1.float().abs().sum()) > 0 and float(vc1.float().abs().sum()) > 0
 
 
-@pytest.mark.parametrize("T,K1,H,N2,mode2", [
-    (32, 4096, 4096, 28672, 2),     # o-proj -> post-attention norm -> gate_up (+SwiGLU), Llama-3-8B
-    (32, 14336, 4096, 6144, 0),     # down-proj -> next layer's input norm -> qkv
-    (64, 4096, 4096, 6144, 0),
-    (7, 1024, 1024, 2048, 0),       # ragged token tile (BT = 16), small hidden
-    (17, 512, 768, 2304, 0),        # 125m dims
-])
-def test_fused_residual_rmsnorm_in_gemms_matches_three_launch_path(g, T, K1, H, N2, mode2):
-    """residual add + RMSNorm folded into the producing GEMM's cluster reduction and the consuming GEMM's operand staging
-    (GemmNorm) against gemm -> add_rmsnorm -> gemm: the residual stream must be bit-identical; the normalised operand
-    differs only through the fp32 summation order of sum(h^2), so y2 is allowed rare one-bf16-ulp flips."""
-    torch.manual_seed(5)
-    rows = 256
-    a = torch.zeros(rows, K1, dtype=torch.bfloat16, device="cuda")
-    a[:T] = (torch.randn(T, K1, device="cuda") * 0.5).bfloat16()
-    w1 = (torch.randn(H, K1, device="cuda") * 0.03).bfloat16()
-    w2 = (torch.randn(N2, H, device="cuda") * 0.03).bfloat16()
-    wn = (1.0 + 0.1 * torch.randn(H, device="cuda")).bfloat16()
-    res0 = torch.randn(rows, H, device="cuda").bfloat16()
-    outs = []
-    for fused in (0, 1):
-        res = res0.clone()
-        y2 = torch.zeros(T, N2 // 2 if mode2 == 2 else N2, dtype=torch.bfloat16, device="cuda")
-        us = C.c_float(0)
-        rc = g.lib().tgis_k_gemm_norm_chain(g.ptr(a), rows, g.ptr(w1), g.ptr(res), g.ptr(wn), g.ptr(w2), g.ptr(y2), T, K1,
-                                            H, N2, 1e-5, mode2, fused, 1, C.byref(us))
-        assert rc in (0, 1), g.kerr()
-        if rc == 1:
-            pytest.skip("the launch plan does not reduce this producer shape in cluster mode on this device")
-        outs.append((res, y2))
-    (r0, y0), (r1, y1) = outs
-    assert torch.equal(r0[:T], r1[:T])                      # residual stream: same arithmetic, same rounding points
-    assert torch.equal(r0[T:], res0[T:]) and torch.equal(r1[T:], res0[T:])
-    d = (y0.float() - y1.float()).abs()
-    assert float(d.max()) <= 2.0 ** -7 * float(y0.float().abs().max()), float(d.max())   # <= one bf16 ulp of the largest output
-    assert float((d > 0).float().mean()) < 0.02, float((d > 0).float().mean())
-    assert float(y0.float().abs().sum()) > 0
-
-
 def _attention_case(g, n_q, n_kv, seq_specs, seed):
     """seq_specs: list of (context_len_before, q_len).  Returns (out_gpu, float64 reference) on the CPU."""
     gen = torch.Generator().manual_seed(seed)
@@ -346,20 +271,6 @@ def test_attention_decode_split_kv(g, n_q, n_kv):
     n_bad, exact, worst = g.attention_bar(out, ref)
     assert n_bad == 0, worst
     assert exact >= 0.99, exact
-
-
-@pytest.mark.parametrize("n_q,n_kv", [(8, 2), (8, 1), (2, 2)])
-def test_attention_inkernel_split_merge_is_bit_identical(g, n_q, n_kv, monkeypatch):
-    """The split merge done inside the streaming kernel by the last-arriving warp (TGIS_ATTN_INKERNEL_MERGE=1) against the
-    separate attn_merge_kernel (default): same sums in the same split order -> identical bits, run twice to
-    cover the self re-arming arrival counters."""
-    specs = [(c, 1) for c in (127, 128, 129, 255, 300, 575, 576, 1000, 2047, 31)]
-    outs = []
-    for flag in ("0", "1", "1"):
-        monkeypatch.setenv("TGIS_ATTN_INKERNEL_MERGE", flag)
-        out, ref = _attention_case(g, n_q, n_kv, specs, seed=5)
-        outs.append(out)
-    assert torch.equal(outs[0], outs[1]) and torch.equal(outs[1], outs[2])
 
 
 @pytest.mark.parametrize("n_q,n_kv", [(4, 2), (8, 2), (6, 2), (8, 1)])

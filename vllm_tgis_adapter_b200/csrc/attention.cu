@@ -105,8 +105,7 @@ __global__ void __launch_bounds__(DEC_THREADS, TGIS_DEC_MINB)
 attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv_bfloat16* __restrict__ k_cache,
                    const __nv_bfloat16* __restrict__ v_cache, const DecItem* __restrict__ items,
                    int max_splits, float* __restrict__ part_o, float* __restrict__ part_ml,
-                   __nv_bfloat16* __restrict__ out, int out_ld, int n_kv, float scale, int* __restrict__ arrive,
-                   int prefetch_old) {
+                   __nv_bfloat16* __restrict__ out, int out_ld, int n_kv, float scale, int prefetch_old) {
   static_assert(G <= 8, "query heads of a group are rows 0..7 of the MMA tile");
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -362,73 +361,6 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
           if (2 * t4 + hh < G)
             *reinterpret_cast<float2*>(part_ml + ((pbase + split) * G + 2 * t4 + hh) * 2) = make_float2(m_r[hh], l_r[hh]);
       }
-      if (arrive != nullptr) {
-        // In-kernel split merge: the warp that delivers the LAST partial of a (sequence, kv head) merges all of them,
-        // in split order (the arithmetic of attn_merge_kernel, so the result does not depend on who merges).  Publish:
-        // warp barrier, then ONE acq_rel atomic by lane 0 (cumulative over the barrier) -- no membar.
-        __syncwarp();
-        int old = 0;
-        if (lane == 0)
-          asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], 1;\n"
-                       : "=r"(old)
-                       : "l"(arrive + seq * n_kv + kvh)
-                       : "memory");
-        old = __shfl_sync(0xffffffffu, old, 0);
-        if (old == n_splits - 1) {
-          // lane -> dims 4*lane .. 4*lane+3 of every head; all loads of a chunk of splits are issued before the math
-          float m_f[G], l_f[G];
-          float4 o_f[G];
-#pragma unroll
-          for (int g = 0; g < G; ++g) {
-            m_f[g] = -INFINITY;
-            l_f[g] = 0.f;
-            o_f[g] = make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-          for (int sp = 0; sp < n_splits; ++sp)
-#pragma unroll
-            for (int g = 0; g < G; ++g) m_f[g] = fmaxf(m_f[g], __ldcg(part_ml + ((pbase + sp) * G + g) * 2));
-          constexpr int SPB = 4;
-          for (int sp0 = 0; sp0 < n_splits; sp0 += SPB) {
-            float4 ov[SPB][G];
-            float2 ml[SPB][G];
-#pragma unroll
-            for (int j = 0; j < SPB; ++j)
-#pragma unroll
-              for (int g = 0; g < G; ++g) {
-                const bool v = sp0 + j < n_splits;
-                ov[j][g] = v ? __ldcg(reinterpret_cast<const float4*>(part_o + ((pbase + sp0 + j) * G + g) * HEAD_DIM) + lane)
-                             : make_float4(0.f, 0.f, 0.f, 0.f);
-                ml[j][g] = v ? __ldcg(reinterpret_cast<const float2*>(part_ml + ((pbase + sp0 + j) * G + g) * 2))
-                             : make_float2(-INFINITY, 0.f);
-              }
-#pragma unroll
-            for (int j = 0; j < SPB; ++j) {
-              if (sp0 + j < n_splits) {
-#pragma unroll
-                for (int g = 0; g < G; ++g) {
-                  const float fs = exp2f(ml[j][g].x - m_f[g]);
-                  l_f[g] += ml[j][g].y * fs;
-                  o_f[g].x += ov[j][g].x * fs;
-                  o_f[g].y += ov[j][g].y * fs;
-                  o_f[g].z += ov[j][g].z * fs;
-                  o_f[g].w += ov[j][g].w * fs;
-                }
-              }
-            }
-          }
-          __nv_bfloat16* o_row = out + (size_t)c_it.x * out_ld + (size_t)kvh * G * HEAD_DIM + 4 * lane;
-#pragma unroll
-          for (int g = 0; g < G; ++g) {
-            const __nv_bfloat162 lo2 = __floats2bfloat162_rn(o_f[g].x / l_f[g], o_f[g].y / l_f[g]);
-            const __nv_bfloat162 hi2 = __floats2bfloat162_rn(o_f[g].z / l_f[g], o_f[g].w / l_f[g]);
-            uint2 pk;
-            pk.x = *reinterpret_cast<const uint32_t*>(&lo2);
-            pk.y = *reinterpret_cast<const uint32_t*>(&hi2);
-            *reinterpret_cast<uint2*>(o_row + g * HEAD_DIM) = pk;
-          }
-          if (lane == 0) arrive[seq * n_kv + kvh] = 0;  // re-armed for the next launch (stream order)
-        }
-      }
     }
     c_it = c_nxt;
   }
@@ -505,7 +437,7 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
                                    const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                    const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits,
                                    float* part_o, float* part_ml, __nv_bfloat16* out, int out_ld, int n_kv,
-                                   float scale, int num_sms, cudaStream_t stream, int* arrive) {
+                                   float scale, int num_sms, cudaStream_t stream) {
   static bool attr = false;
   if (!attr) {
     cudaError_t e =
@@ -515,18 +447,11 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
   }
   const long long max_flat = (long long)max_entries * n_kv;
   const int grid = (int)std::min<long long>((long long)TGIS_DEC_MINB * num_sms, (max_flat + DEC_WARPS - 1) / DEC_WARPS);
-  // split merge: the PDL-chained attn_merge_kernel (default), or inside the streaming kernel by the last-arriving warp
-  // (TGIS_ATTN_INKERNEL_MERGE=1, bit-identical).  Folding the merge saves its launch, but the o-proj GEMM that follows
-  // then loses the window in which it prefetched its weights next to the small merge kernel (attention CTAs fill the
-  // SM's shared memory).  The separate kernel is the default.
-  const char* env_merge = getenv("TGIS_ATTN_INKERNEL_MERGE");  // read per launch: the A/B test flips it in-process
-  const int inkernel = (env_merge && env_merge[0] == '1') ? 1 : 0;
   const char* env_pre = getenv("TGIS_ATTN_PREFETCH");  // 0: no cache reads before the grid-dependency wait
   const int prefetch_old = (env_pre && env_pre[0] == '0') ? 0 : 1;
-  int* arr = (inkernel && max_splits > 1) ? arrive : nullptr;
   cudaError_t e = launch_k(attn_decode_kernel<G>, dim3(grid), dim3(DEC_THREADS), DEC_SMEM, stream, qkv, qkv_ld,
-                           k_cache, v_cache, items, max_splits, part_o, part_ml, out, out_ld, n_kv, scale, arr, prefetch_old);
-  if (e != cudaSuccess || max_splits <= 1 || arr != nullptr) return e;
+                           k_cache, v_cache, items, max_splits, part_o, part_ml, out, out_ld, n_kv, scale, prefetch_old);
+  if (e != cudaSuccess || max_splits <= 1) return e;
   return launch_k(attn_merge_kernel<G>, dim3(n_seqs, n_kv), dim3(HEAD_DIM), 0, stream, seqs, seq_ids, max_splits,
                   (const float*)part_o, (const float*)part_ml, out, out_ld, n_kv);
 }
@@ -535,14 +460,14 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
                                const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits, float* part_o,
                                float* part_ml, __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                               int num_sms, cudaStream_t stream, int* arrive) {
+                               int num_sms, cudaStream_t stream) {
   if (max_entries <= 0 || n_seqs <= 0) return cudaSuccess;
   if (n_q % n_kv != 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
 #define TGIS_DEC(GG)                                                                                               \
   case GG:                                                                                                         \
     return decode_launch_g<GG>(qkv, qkv_ld, k_cache, v_cache, items, max_entries, seqs, seq_ids, n_seqs, max_splits, \
-                               part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream, arrive)
+                               part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream)
   switch (G) {
     TGIS_DEC(1);
     TGIS_DEC(2);

@@ -301,14 +301,11 @@ struct tgis_engine {
   // lm_head output [rows, V].  bf16 = the model dtype, rounded once from the fp32 accumulator exactly where vLLM's
   // lm_head rounds (vllm model_executor/layers/logits_processor.py:89-104 -> F.linear in bf16; the sampler then casts to
   // fp32, v1/sample/sampler.py:91): exact ties between bf16 logits, and the ranks / lowest-id argmax they cause, are
-  // reproduced.  TGIS_LOGITS_FP32=1 keeps the raw fp32 accumulator (round 1's behaviour; an experiment switch).
+  // reproduced.
   DevBuf<uint8_t> logits;
-  bool logits_bf16 = true;
-  size_t lsz = 2;  // bytes per logit
-  CUtensorMap xm_xn[N_BT], xm_attn[N_BT], xm_act[N_BT], xm_last[N_BT], xm_resid[N_BT];
+  CUtensorMap xm_xn[N_BT], xm_attn[N_BT], xm_act[N_BT], xm_last[N_BT];
   DevBuf<float> gemm_ws, part_o, part_ml, samp_scratch;
-  DevBuf<int> gemm_counters, attn_arrive;
-  DevBuf<float> norm_ssq;  // [2][GEMM_NORM_MAX_T][hidden / 128] partial sums of h^2 (fused residual RMSNorm)
+  DevBuf<int> gemm_counters;
   DevBuf<uint32_t> seen_bitmap;
   // guided decoding: allowed-token bits of the step, one row per sequence slot (same geometry as seen_bitmap); the
   // provider writes the pinned host row, the row is copied in front of the step, the sampler reads it for SAMPLE_MASKED rows
@@ -370,15 +367,11 @@ struct tgis_engine {
   bool fuse_rope = true;
   int rope_fuse_max_t = 32;
   int rope_fuse_cluster_max_t = 256;
-  // residual add + RMSNorm folded into the o / down projections' cluster reduction and the gate_up / qkv projections'
-  // operand staging (GemmNorm, gemm_wgmma.cu): tp == 1, steps of at most GEMM_NORM_MAX_T tokens.  TGIS_FUSE_NORM=0: off
-  bool fuse_norm = false;
   // tensor parallelism, decode-shaped steps: one-shot all-reduce + residual + RMSNorm over NVLink peer memory
   // (ar_add_rmsnorm_kernel) instead of ncclAllReduce + rmsnorm kernel.  TGIS_TP_FUSED_AR=0: NCCL baseline.
   bool tp_fused_ar = true;
   int tp_exchange_force = -1;                 // TGIS_TP_EXCHANGE
   size_t tp_oneshot_max_bytes = 2u << 20;     // TGIS_TP_ONESHOT_MAX_KB
-  bool tp_graphs = true;  // TGIS_TP_GRAPHS=0: tensor-parallel decode steps are launched kernel by kernel (round 1)
   static constexpr int AR_MAX_T = AR_MAX_ROWS;
   uint8_t* ar_mem = nullptr;        // [2 parities] receive areas (ar_recv_bytes each), then the two local partial buffers
   uint8_t* ar_peer[8] = {};         // the same allocation of every rank, mapped here (cudaIpc)
@@ -387,7 +380,6 @@ struct tgis_engine {
   uint32_t lg_epoch = 0;             // rank 0: epoch of the last logits gather (staged per step: off_epoch[2])
   int lg_idx_step = 0;               // rank 0: gathers issued for the current step (the step's own, then prompt-logprob passes)
   size_t lg_off = 0;                 // inside ar_mem: [S_max, V] logits receive buffer (rank 0's is the one used), then flags
-  int l2_prefetch_kb = 0;   // (off: measured no gain, costs DRAM traffic in the issuing kernel) k-blocks (16 KiB each) per CTA of the NEXT GEMM pulled into L2 by the current one
   std::vector<cudaEvent_t> prof_events;
   size_t prof_used = 0;
   std::vector<double> prof_bytes;  // algorithmic bytes of the GEMM between events 2i and 2i+1 (< 0: an exchange)
@@ -411,15 +403,7 @@ struct tgis_engine {
   std::unordered_map<uint64_t, cudaGraphExec_t> graphs;
   std::unordered_map<uint64_t, long long> graph_nodes;
   long long n_graph_launches = 0;
-  // Experiment switches for the step-to-step turnaround (scripts/step_timeline.py measured ~1 ms between the end of one
-  // graph replay and the first kernel of the next, against ~26 us when the same step is launched kernel by kernel):
-  bool sync_spin = true;              // TGIS_SYNC_SPIN: wait for the step by polling its end event instead of
-                                      // cudaStreamSynchronize (no blocking-wait wake-up latency)
-  bool graph_copy_outside = true;     // TGIS_GRAPH_COPY_OUTSIDE: metadata H2D / result D2H as plain stream copies
-                                      // around the graph launch instead of memcpy nodes inside the graph
   bool capturing = false;
-  bool attn_inkernel_merge = false;   // TGIS_ATTN_INKERNEL_MERGE (read by attention.cu as well): launch accounting only
-  int debug_step_sleep_us = 0;        // TGIS_STEP_SLEEP_US (experiment)
   bool debug_launch = false;          // TGIS_DEBUG_LAUNCH=1: host time spent inside cudaGraphLaunch, printed at destroy
   double graph_launch_host_s = 0;
   // TGIS_DEBUG_LAUNCH: host-side phase times of the last steps: [sched+build, launch, wait, post] in microseconds
@@ -500,26 +484,17 @@ struct tgis_engine {
     const size_t T_alloc = std::max(T_max, 256), S_alloc = std::max(S_max, 256);
     tiles_max = T_max / 16 + S_max + 1;
     rng.seed(c.seed ? c.seed : 0x5DEECE66Dull);
-    if (const char* e = getenv("TGIS_L2_PREFETCH_KB")) l2_prefetch_kb = atoi(e);
     if (const char* e = getenv("TGIS_FUSE_ROPE")) fuse_rope = atoi(e) != 0;
     if (const char* e = getenv("TGIS_FUSE_ROPE_MAX_T")) rope_fuse_max_t = atoi(e);
     if (const char* e = getenv("TGIS_FUSE_ROPE_CLUSTER_MAX_T")) rope_fuse_cluster_max_t = atoi(e);
-    if (const char* e = getenv("TGIS_FUSE_NORM")) fuse_norm = atoi(e) != 0;
     if (const char* e = getenv("TGIS_TP_FUSED_AR")) tp_fused_ar = atoi(e) != 0;
-    if (const char* e = getenv("TGIS_LOGITS_FP32")) logits_bf16 = atoi(e) == 0;
     if (const char* e = getenv("TGIS_TP_TIMEOUT_S")) tp_timeout_s = atof(e);
     if (const char* e = getenv("TGIS_DEBUG_LAUNCH")) debug_launch = atoi(e) != 0;
-    if (const char* e = getenv("TGIS_SYNC_SPIN")) sync_spin = atoi(e) != 0;
-    if (const char* e = getenv("TGIS_ATTN_INKERNEL_MERGE")) attn_inkernel_merge = atoi(e) != 0;
-    if (const char* e = getenv("TGIS_STEP_SLEEP_US")) debug_step_sleep_us = atoi(e);
-    if (const char* e = getenv("TGIS_GRAPH_COPY_OUTSIDE")) graph_copy_outside = atoi(e) != 0;
-    if (const char* e = getenv("TGIS_TP_GRAPHS")) tp_graphs = atoi(e) != 0;
     if (const char* e = getenv("TGIS_TP_ONESHOT_MAX_KB")) tp_oneshot_max_bytes = (size_t)atol(e) << 10;
     if (const char* e = getenv("TGIS_TP_EXCHANGE")) {
       const std::string v = e;
       tp_exchange_force = v == "nccl" ? 0 : v == "oneshot" ? 1 : v == "twoshot" ? 2 : -1;
     }
-    lsz = logits_bf16 ? 2 : 4;
 
     // ---- weights: one arena
     const size_t H = c.hidden, F = Fl, V = c.vocab, L = c.n_layers;  // F: this rank's ffn shard
@@ -605,18 +580,15 @@ struct tgis_engine {
       gu_buf.alloc(T_alloc * (size_t)2 * F);
     }
     last_hidden.alloc(S_alloc * H);
-    logits.alloc((size_t)S_max * Vp * lsz);
+    logits.alloc((size_t)S_max * Vp * sizeof(bf16));
     if (tp > 1) {
-      logits_shard.alloc((size_t)S_max * Vl * lsz);
-      logits_gather.alloc((size_t)tp * S_max * Vl * lsz);
+      logits_shard.alloc((size_t)S_max * Vl * sizeof(bf16));
+      logits_gather.alloc((size_t)tp * S_max * Vl * sizeof(bf16));
     }
     xn.zero(); attn_out.zero(); act.zero(); last_hidden.zero();
     gemm_ws.alloc(gemm_workspace_bytes(num_sms) / sizeof(float));
     gemm_counters.alloc(1 << 16);
     gemm_counters.zero();
-    attn_arrive.alloc((size_t)S_max * std::max(nkv, 1));
-    attn_arrive.zero();
-    norm_ssq.alloc((size_t)2 * GEMM_NORM_MAX_T * (c.hidden / 128 + 1));
     const int G = c.n_q_heads / c.n_kv_heads;
     part_o.alloc((size_t)S_max * nkv * max_splits_cap * G * HEAD_DIM);
     part_ml.alloc((size_t)S_max * nkv * max_splits_cap * G * 2);
@@ -678,7 +650,6 @@ struct tgis_engine {
           throw CudaError("cuTensorMapEncodeTiled(activation) failed");
       };
       xmap(&xm_xn[i], xn.p, T_alloc, H);
-      xmap(&xm_resid[i], resid.p, T_alloc, H);  // fused-norm consumers read the residual stream
       xmap(&xm_attn[i], attn_out.p, T_alloc, q_dim);
       xmap(&xm_act[i], act.p, T_alloc, F);
       xmap(&xm_last[i], last_hidden.p, S_alloc, H);
@@ -759,7 +730,7 @@ struct tgis_engine {
   }
 
   size_t ar_buf_bytes() const { return (size_t)AR_MAX_T * cfg.hidden * sizeof(bf16); }
-  size_t lg_logits_bytes() const { return ((size_t)S_max * cfg.vocab * lsz + 255) / 256 * 256; }
+  size_t lg_logits_bytes() const { return ((size_t)S_max * cfg.vocab * sizeof(bf16) + 255) / 256 * 256; }
   // rank 0's full-vocabulary logits: inside the peer-mapped allocation when the ranks can reach each other's memory
   uint8_t* logits_ptr() { return (tp > 1 && tp_fused_ar && ar_mem) ? ar_mem + lg_off : logits.p; }
   size_t ar2_area_stride() const { return (ar2_area_bytes(cfg.hidden) + 255) / 256 * 256; }
@@ -1131,11 +1102,8 @@ struct tgis_engine {
   }
 
   // ------------------------------------------------------------------------------------------------ device step
-  // next_wm / nT,nN,nK describe the GEMM that follows this one in the layer stack: its first weight boxes are
-  // prefetched into L2 by this launch's producer warp (gemm_wgmma.cu)
   void gemm(const CUtensorMap* xmaps, const CUtensorMap& wm, const bf16* X, const bf16* W, void* Y, int T, int N, int K,
-            int out_f32 = 0, const CUtensorMap* next_wm = nullptr, int nT = 0, int nN = 0, int nK = 0, int ldy = 0,
-            const GemmRope* rope = nullptr, const GemmNorm* norm = nullptr) {
+            int out_f32 = 0, int ldy = 0, const GemmRope* rope = nullptr) {
     if (ldy == 0) ldy = N;
     cudaEvent_t pe0 = nullptr, pe1 = nullptr;
     if (profiling && (!prof_decode_only || step_is_decode)) {
@@ -1154,10 +1122,8 @@ struct tgis_engine {
     if (cfg.debug_gemm_ref) {
       CK(gemm_bf16_ref_launch(X, K, W, Y, ldy, T, N, K, stream, out_f32));
     } else {
-      GemmNext nx{};
-      if (next_wm && l2_prefetch_kb > 0) nx = gemm_next_desc(nT, nN, nK, num_sms, l2_prefetch_kb);
       CK(gemm_bf16_launch(wm, xmaps[bt_index(T)], Y, ldy, T, N, K, gemm_ws.p, gemm_counters.p, num_sms, stream, out_f32,
-                          nx.kb_prefetch > 0 ? next_wm : nullptr, nx.kb_prefetch > 0 ? &nx : nullptr, rope, norm));
+                          rope));
     }
     if (pe1) CK(cudaEventRecord(pe1, stream));
     ++n_launches;
@@ -1202,7 +1168,7 @@ struct tgis_engine {
   void launch_step(size_t copy_bytes, int T, int n_dec, int n_tiles, int R, int max_dec_kv, int S, int samp_complex) {
     const tgis_config& c = cfg;
     const int H = c.hidden, F = Fl, V = c.vocab;  // F: local ffn shard
-    const bool copies_here = !(capturing && graph_copy_outside);
+    const bool copies_here = !capturing;
     CK(stl_marker_launch(20, stream));  // timeline builds: step begin (before the metadata copy)
     if (copies_here) CK(cudaMemcpyAsync(d_stage.p, h_stage, copy_bytes, cudaMemcpyHostToDevice, stream));
     CK(stl_marker_launch(21, stream));  // metadata landed
@@ -1245,26 +1211,12 @@ struct tgis_engine {
     if (lora) ++lora_steps;
     const bool rope_fused = !lora && fuse_rope && !cfg.debug_gemm_ref && gemm_even_split(T, qkv_dim, H, num_sms) >= 2 &&
                             T <= (qkv_cluster > 0 ? std::max(rope_fuse_max_t, rope_fuse_cluster_max_t) : rope_fuse_max_t);
-    // residual add + RMSNorm inside the GEMMs either side of it (single GPU, small steps, both row-"producers" reduced
-    // on chip): o-proj -> [post-attention norm] -> gate_up and down-proj -> [next layer's input norm] -> qkv
-    const bool norm_fused = !lora && fuse_norm && tp == 1 && !cfg.debug_gemm_ref && T <= GEMM_NORM_MAX_T && H % 128 == 0 && H / 128 <= GEMM_NORM_MAX_PARTS &&
-                            gemm_cluster_split(T, H, q_dim, num_sms) > 0 && gemm_cluster_split(T, H, F, num_sms) > 0;
-    const int n_parts = H / 128;
-    float* ssq_attn = norm_ssq.p;                                      // written by o-proj, read by gate_up
-    float* ssq_mlp = norm_ssq.p + (size_t)GEMM_NORM_MAX_T * n_parts;   // written by down-proj, read by the next qkv
-    const GemmNorm prod_attn{resid.p, ssq_attn, nullptr, nullptr, nullptr, 0, 0.f};
-    const GemmNorm prod_mlp{resid.p, ssq_mlp, nullptr, nullptr, nullptr, 0, 0.f};
     for (int li = 0; li < (opt ? 0 : c.n_layers); ++li) {  // Llama stack (OPT: opt_layers() above)
       LayerW& l = layers[li];
-      const GemmNorm cons_qkv{nullptr, nullptr, resid.p, ssq_mlp, l.ln1, n_parts, c.rms_eps};
-      const GemmNorm cons_gu{nullptr, nullptr, resid.p, ssq_attn, l.ln2, n_parts, c.rms_eps};
-      const bool qkv_norm_in = norm_fused && li > 0;
       {
         if (li == 0) {
           CK(rmsnorm_launch(resid.p, l.ln1, xn.p, T, H, c.rms_eps, stream));
           ++n_launches;
-        } else if (qkv_norm_in) {
-          // the previous layer's down-proj left h in resid and sum(h^2) in ssq_mlp; the qkv GEMM normalises on the fly
         } else if (ar_fused) {
           fused_ar_norm(1, l.ln1, T);  // previous layer's down-proj partials
         } else {
@@ -1273,8 +1225,7 @@ struct tgis_engine {
         }
         const GemmRope rp{ds<int32_t>(off_pos), ds<int32_t>(off_slotmap), cos_sin,
                           k_cache.p + (size_t)li * kv_layer_elems, v_cache.p + (size_t)li * kv_layer_elems, nq, nkv};
-        gemm(qkv_norm_in ? xm_resid : xm_xn, l.m_qkv, xn.p, l.wqkv, qkv.p, T, qkv_dim, H, 0, &l.m_o, T, H, q_dim, 0,
-             rope_fused ? &rp : nullptr, qkv_norm_in ? &cons_qkv : nullptr);
+        gemm(xm_xn, l.m_qkv, xn.p, l.wqkv, qkv.p, T, qkv_dim, H, 0, 0, rope_fused ? &rp : nullptr);
         if (lora) {
           const LoraLayerW& ll = lora_layers[li];
           LoraGroup g{};
@@ -1297,12 +1248,11 @@ struct tgis_engine {
         const int max_splits = (max_dec_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
         CK(attn_decode_launch(qkv.p, qkv_dim, kc, vc, ds<DecItem>(items_off(S)), n_dec * max_splits, d_seqs,
                               ds<int32_t>(off_decids), n_dec, max_splits, part_o.p, part_ml.p, attn_out.p, q_dim, nq,
-                              nkv, scale, num_sms, stream, attn_arrive.p));
-        n_launches += (max_splits > 1 && !attn_inkernel_merge) ? 2 : 1;
+                              nkv, scale, num_sms, stream));
+        n_launches += max_splits > 1 ? 2 : 1;
       }
       if (n_tiles > 0) prefill_attention(kc, vc, scale, n_tiles);
-      gemm(xm_attn, l.m_o, attn_out.p, l.wo, ar_fused ? ar_buf(0) : tmp.p, T, H, q_dim, 0, &l.m_gu, T, 2 * F, H, 0, nullptr,
-           norm_fused ? &prod_attn : nullptr);
+      gemm(xm_attn, l.m_o, attn_out.p, l.wo, ar_fused ? ar_buf(0) : tmp.p, T, H, q_dim);
       if (lora) {
         LoraGroup g{};
         g.n_mods = 1;
@@ -1310,8 +1260,7 @@ struct tgis_engine {
         g.mod[0] = LoraModule{lora_layers[li].A_o, lora_layers[li].B_o, q_dim, H, LR, 0, 0};
         lora_apply(g, attn_out.p, q_dim, tmp.p, H);
       }
-      if (norm_fused) {
-      } else if (ar_fused) {
+      if (ar_fused) {
         fused_ar_norm(0, l.ln2, T);
       } else {
         all_reduce_tmp(T);  // row-parallel partial sums (tp > 1)
@@ -1321,7 +1270,7 @@ struct tgis_engine {
       // gate_up GEMM with SwiGLU fused into its epilogue: writes act[T, F] directly (no gate_up round trip)
       if (lora) {
         // raw interleaved gate_up -> + adapter deltas (gate and up as one module of capacity 2R) -> SwiGLU
-        gemm(xm_xn, l.m_gu, xn.p, l.wgu, gu_buf.p, T, 2 * F, H, /*out_mode=*/0, &l.m_d, T, H, F, /*ldy=*/2 * F);
+        gemm(xm_xn, l.m_gu, xn.p, l.wgu, gu_buf.p, T, 2 * F, H, /*out_mode=*/0, /*ldy=*/2 * F);
         LoraGroup g{};
         g.n_mods = 1;
         g.v_ld = 3 * LR;
@@ -1330,13 +1279,9 @@ struct tgis_engine {
         CK(silu_mul_interleaved_launch(gu_buf.p, act.p, T, F, stream));
         ++n_launches;
       } else
-      gemm(norm_fused ? xm_resid : xm_xn, l.m_gu, xn.p, l.wgu, act.p, T, 2 * F, H, /*out_mode=*/2, &l.m_d, T, H, F,
-           /*ldy=*/F, nullptr, norm_fused ? &cons_gu : nullptr);
+      gemm(xm_xn, l.m_gu, xn.p, l.wgu, act.p, T, 2 * F, H, /*out_mode=*/2, /*ldy=*/F);
       bf16* down_out = ar_fused ? ar_buf(1) : tmp.p;
-      if (li + 1 < c.n_layers)
-        gemm(xm_act, l.m_d, act.p, l.wd, down_out, T, H, F, 0, &layers[li + 1].m_qkv, T, qkv_dim, H, 0, nullptr,
-             norm_fused ? &prod_mlp : nullptr);
-      else gemm(xm_act, l.m_d, act.p, l.wd, down_out, T, H, F, 0, R > 0 ? &m_lm : nullptr, R, Vl, H);
+      gemm(xm_act, l.m_d, act.p, l.wd, down_out, T, H, F);
       if (lora) {
         LoraGroup g{};
         g.n_mods = 1;
@@ -1360,7 +1305,7 @@ struct tgis_engine {
       lm_head_logits(R, 1);
       if (rank == 0) {
         scale_logits(R);
-        CK(sampler_launch(logits_ptr(), logits_bf16 ? 1 : 0, Vpad, V, ds<SampleRow>(off_rows), R, seen_bitmap.p, bitmap_words,
+        CK(sampler_launch(logits_ptr(), 1, Vpad, V, ds<SampleRow>(off_rows), R, seen_bitmap.p, bitmap_words,
                           samp_scratch.p, d_samp_out.p, stream, samp_complex & 1, num_sms,
                           (samp_complex & 2) ? allow_bitmap.p : nullptr));
         ++n_launches;
@@ -1390,7 +1335,7 @@ struct tgis_engine {
       // h += fc2 of the previous layer (its fp32 accumulators are still in y32), then LN1
       CK(opt_layernorm_launch(li == 0 ? nullptr : y32.p, li == 0 ? nullptr : layers[li - 1].b_fc2, resid.p, l.ln1, l.ln1_b,
                               xn.p, T, H, c.rms_eps, stream));
-      gemm(xm_xn, l.m_qkv, xn.p, l.wqkv, y32.p, T, qkv_dim, H, /*out_f32=*/1, &l.m_o, T, H, q_dim);
+      gemm(xm_xn, l.m_qkv, xn.p, l.wqkv, y32.p, T, qkv_dim, H, /*out_f32=*/1);
       bf16* kc = k_cache.p + (size_t)li * kv_layer_elems;
       bf16* vc = v_cache.p + (size_t)li * kv_layer_elems;
       // bias + rounding; q -> qkv buffer, k / v -> paged cache (no rotary embedding in between)
@@ -1400,17 +1345,15 @@ struct tgis_engine {
         const int max_splits = (max_dec_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
         CK(attn_decode_launch(qkv.p, qkv_dim, kc, vc, ds<DecItem>(items_off(S)), n_dec * max_splits, d_seqs,
                               ds<int32_t>(off_decids), n_dec, max_splits, part_o.p, part_ml.p, attn_out.p, q_dim, nq,
-                              nkv, attn_scale, num_sms, stream, attn_arrive.p));
-        n_launches += (max_splits > 1 && !attn_inkernel_merge) ? 2 : 1;
+                              nkv, attn_scale, num_sms, stream));
+        n_launches += max_splits > 1 ? 2 : 1;
       }
       if (n_tiles > 0) prefill_attention(kc, vc, attn_scale, n_tiles);
-      gemm(xm_attn, l.m_o, attn_out.p, l.wo, y32.p, T, H, q_dim, /*out_f32=*/1, &l.m_gu, T, F, H);
+      gemm(xm_attn, l.m_o, attn_out.p, l.wo, y32.p, T, H, q_dim, /*out_f32=*/1);
       CK(opt_layernorm_launch(y32.p, l.b_o, resid.p, l.ln2, l.ln2_b, xn.p, T, H, c.rms_eps, stream));
-      gemm(xm_xn, l.m_gu, xn.p, l.wgu, y32.p, T, F, H, /*out_f32=*/1, &l.m_d, T, H, F);
+      gemm(xm_xn, l.m_gu, xn.p, l.wgu, y32.p, T, F, H, /*out_f32=*/1);
       CK(opt_bias_act_launch(y32.p, F, l.b_fc1, act.p, F, T, F, /*relu=*/1, num_sms, stream));
-      // (the successor's first weight boxes are pulled into L2 by this launch's producer warp, as on the Llama path)
-      if (li + 1 < c.n_layers) gemm(xm_act, l.m_d, act.p, l.wd, y32.p, T, H, F, /*out_f32=*/1, &layers[li + 1].m_qkv, T, qkv_dim, H);
-      else gemm(xm_act, l.m_d, act.p, l.wd, y32.p, T, H, F, /*out_f32=*/1, R > 0 ? &m_lm : nullptr, R, Vl, H);
+      gemm(xm_act, l.m_d, act.p, l.wd, y32.p, T, H, F, /*out_f32=*/1);
       n_launches += 2;
     }
     // always run (even when no row is sampled this step): a prompt-logprob pass may read xn afterwards
@@ -1428,28 +1371,27 @@ struct tgis_engine {
   void lm_head_logits(int rows, int lg_idx) {
     const tgis_config& c = cfg;
     const int H = c.hidden, V = c.vocab;
-    const int lm_mode = logits_bf16 ? 0 : 1;
     if (tp == 1) {
-      gemm(xm_last, m_lm, last_hidden.p, lm_head, logits.p, rows, Vpad, H, lm_mode);
+      gemm(xm_last, m_lm, last_hidden.p, lm_head, logits.p, rows, Vpad, H);
     } else if (tp_fused_ar) {
       uint32_t* flags0 = reinterpret_cast<uint32_t*>(ar_peer[0] + lg_off + lg_logits_bytes());  // in rank 0's memory
       if (rank == 0) {
-        gemm(xm_last, m_lm, last_hidden.p, lm_head, logits_ptr(), rows, Vl, H, lm_mode, nullptr, 0, 0, 0, /*ldy=*/V);
+        gemm(xm_last, m_lm, last_hidden.p, lm_head, logits_ptr(), rows, Vl, H, 0, /*ldy=*/V);
         CK(logits_wait_launch(flags0, tp, ds<uint32_t>(off_epoch) + 2, (uint32_t)lg_idx, stream));
       } else {
-        gemm(xm_last, m_lm, last_hidden.p, lm_head, logits_shard.p, rows, Vl, H, lm_mode);
+        gemm(xm_last, m_lm, last_hidden.p, lm_head, logits_shard.p, rows, Vl, H);
         int* counter = reinterpret_cast<int*>(ar_mem + lg_off + lg_logits_bytes() + 128);  // local
-        CK(logits_push_launch(logits_shard.p, ar_peer[0] + lg_off, rows, (int)(Vl * lsz), (int)((size_t)V * lsz),
-                              (int)((size_t)rank * Vl * lsz), flags0 + rank, counter, ds<uint32_t>(off_epoch) + 2,
+        CK(logits_push_launch(logits_shard.p, ar_peer[0] + lg_off, rows, (int)(Vl * sizeof(bf16)), (int)((size_t)V * sizeof(bf16)),
+                              (int)((size_t)rank * Vl * sizeof(bf16)), flags0 + rank, counter, ds<uint32_t>(off_epoch) + 2,
                               (uint32_t)lg_idx, stream));
       }
       ++n_launches;
     } else {
-      gemm(xm_last, m_lm, last_hidden.p, lm_head, logits_shard.p, rows, Vl, H, lm_mode);
-      NK(nccl().AllGather(logits_shard.p, logits_gather.p, (size_t)rows * Vl * lsz, ncclInt8, comm, stream));
+      gemm(xm_last, m_lm, last_hidden.p, lm_head, logits_shard.p, rows, Vl, H);
+      NK(nccl().AllGather(logits_shard.p, logits_gather.p, (size_t)rows * Vl * sizeof(bf16), ncclInt8, comm, stream));
       if (rank == 0) {
         CK(launch_k(gather_relayout_kernel, dim3(num_sms * 4), dim3(256), 0, stream, (const uint4*)logits_gather.p,
-                    (uint4*)logits.p, rows, (int)(Vl * lsz / 16), tp));
+                    (uint4*)logits.p, rows, (int)(Vl * sizeof(bf16) / 16), tp));
         ++n_launches;
       }
     }
@@ -1458,7 +1400,7 @@ struct tgis_engine {
   // Granite's logits_scaling: bf16(logit * (1 / logits_scaling)) in place before the sampler reads the rows (rank 0)
   void scale_logits(int rows) {
     if (logit_scale == 1.f) return;
-    CK(logits_scale_launch(logits_ptr(), logits_bf16 ? 1 : 0, Vpad, cfg.vocab, rows, logit_scale, stream));
+    CK(logits_scale_launch(logits_ptr(), 1, Vpad, cfg.vocab, rows, logit_scale, stream));
     ++n_launches;
   }
 
@@ -1475,7 +1417,7 @@ struct tgis_engine {
     lm_head_logits(m, lg_idx);
     if (rank == 0) {
       scale_logits(m);
-      CK(sampler_launch(logits_ptr(), logits_bf16 ? 1 : 0, Vpad, V, ds<SampleRow>(off_rows), m, seen_bitmap.p, bitmap_words,
+      CK(sampler_launch(logits_ptr(), 1, Vpad, V, ds<SampleRow>(off_rows), m, seen_bitmap.p, bitmap_words,
                         samp_scratch.p, d_samp_out.p, stream, /*any_complex=*/0, num_sms));
       ++n_launches;
       CK(cudaMemcpyAsync(h_plp_out, d_samp_out.p, sizeof(SampleOut) * m, cudaMemcpyDeviceToHost, stream));
@@ -1484,10 +1426,6 @@ struct tgis_engine {
 
   // Wait until everything up to ev1 (the step's last operation on the stream) has executed.
   void wait_step_end() {
-    if (!sync_spin) {
-      CK(cudaStreamSynchronize(stream));
-      return;
-    }
     for (;;) {
       const cudaError_t q = cudaEventQuery(ev1);
       if (q == cudaSuccess) return;
@@ -1546,9 +1484,9 @@ struct tgis_engine {
       it = graphs.emplace(key, ge).first;
     }
     const double t_gl = debug_launch ? now_s() : 0.0;
-    if (graph_copy_outside) CK(cudaMemcpyAsync(d_stage.p, h_stage, h.copy_bytes, cudaMemcpyHostToDevice, stream));
+    CK(cudaMemcpyAsync(d_stage.p, h_stage, h.copy_bytes, cudaMemcpyHostToDevice, stream));
     CK(cudaGraphLaunch(it->second, stream));
-    if (graph_copy_outside && rank == 0 && h.R > 0)
+    if (rank == 0 && h.R > 0)
       CK(cudaMemcpyAsync(h_samp_out, d_samp_out.p, sizeof(SampleOut) * h.R, cudaMemcpyDeviceToHost, stream));
     if (debug_launch) graph_launch_host_s += now_s() - t_gl;
     n_launches += graph_nodes[key];
@@ -1692,7 +1630,7 @@ struct tgis_engine {
     const size_t copy_bytes = items_off(S) + sizeof(DecItem) * (1 + (size_t)n_dec * max_splits_step);
     const double t_ev0 = debug_launch ? now_s() : 0.0;
     CK(cudaEventRecord(ev0, stream));
-    const bool graphable = cfg.use_cuda_graphs && (tp == 1 || tp_graphs) && !profiling && n_tiles == 0 && n_dec == S && R == S;
+    const bool graphable = cfg.use_cuda_graphs && !profiling && n_tiles == 0 && n_dec == S && R == S;
     StepHeader hdr{T, n_dec, n_tiles, R, max_dec_kv, S, graphable ? 1 : 0, samp_complex, (uint64_t)copy_bytes, 0, 0, 1,
                    n_ctiles};
     if (tp > 1) {
@@ -1951,7 +1889,6 @@ struct tgis_engine {
 
   // one engine step; returns false when there was nothing to do
   bool step() {
-    if (debug_step_sleep_us > 0) usleep(debug_step_sleep_us);  // experiment: GPU idle time between steps
     if (debug_launch) t_step_begin = now_s();
     // ---- intake
     {
@@ -2263,8 +2200,6 @@ int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, fl
   e->res_mult = residual_multiplier;
   e->logit_scale = logit_scale;
   e->attn_scale = attention_multiplier > 0.f ? attention_multiplier : 1.0f / std::sqrt((float)e->model_head_dim);
-  // the TGIS_FUSE_NORM experiment folds the residual add into the GEMMs without the multiplier
-  if (residual_multiplier != 1.f) e->fuse_norm = false;
   return 0;
 }
 

@@ -36,27 +36,20 @@ constexpr int GEMM_BK = 64;   // k per stage (one 128-byte swizzle row of bf16)
 constexpr int EP_WARPS = 8;   // consumer warps: MMA + epilogue, two warpgroups
 constexpr int EP_THREADS = EP_WARPS * 32;
 constexpr int PRODUCER_WARP = EP_WARPS;
-constexpr int NORM_WARP0 = EP_WARPS + 1;
 constexpr int GEMM_THREADS = EP_THREADS + 32;
-constexpr int GEMM_THREADS_NORM = GEMM_THREADS + 64;  // + 2 activation-transform warps (fused RMSNorm consumer, GemmNorm::h)
 
-// NW = weight tiles (of GEMM_BN = 128 rows) per unit that share ONE activation tile: every unit re-reads its [BT x 64]
-// activation tile per k-block, and with NW = 2 that tile feeds two MMAs (two accumulators), halving the activation bytes
-// per weight byte.  An experiment (TGIS_GEMM_NW=2, see gemm_nw()): NW = 1 is what runs.
-//
-// LEAN = the decode instantiation (token tiles of at most GEMM_LEAN_MAX_T rows, NW = 1, no fused-norm warps, no push
-// variant of the cluster reduction): a GEMM_LEAN_STAGES-deep ring and at most 96 registers per thread (ptxas' cap for two
-// 288-thread CTAs), so TWO CTAs fit one SM (2 x (104 KB + 1 KB reserved) <= 228 KB of shared memory).  The grid still
+// LEAN = the decode instantiation (token tiles of at most GEMM_LEAN_MAX_T rows): a GEMM_LEAN_STAGES-deep ring and at
+// most 96 registers per thread (ptxas' cap for two 288-thread CTAs), so TWO CTAs fit one SM (2 x (104 KB + 1 KB
+// reserved) <= 228 KB of shared memory).  The grid still
 // holds at most one CTA per SM; the second slot is for the NEXT GEMM of the chain, whose CTAs become resident as soon as
 // this one triggers its dependents and fill their rings while this one drains (with one CTA per SM nothing of the next
 // launch could be resident until this one's CTA on that SM had exited).
 constexpr int GEMM_LEAN_MAX_T = 32;
 constexpr int GEMM_LEAN_STAGES = 5;
-template <int BT, int NW, bool LEAN = false>
+template <int BT, bool LEAN = false>
 struct GemmCfg {
-  static_assert(!LEAN || (BT <= GEMM_LEAN_MAX_T && NW == 1), "lean instantiation: decode token tiles, one weight tile");
-  static constexpr int W_TILE_BYTES = GEMM_BN * GEMM_BK * 2;
-  static constexpr int W_BYTES = NW * W_TILE_BYTES;
+  static_assert(!LEAN || BT <= GEMM_LEAN_MAX_T, "lean instantiation: decode token tiles");
+  static constexpr int W_BYTES = GEMM_BN * GEMM_BK * 2;
   static constexpr int X_BYTES = BT * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = W_BYTES + X_BYTES;
 #ifndef TGIS_GEMM_SMEM_KB
@@ -68,13 +61,9 @@ struct GemmCfg {
 #endif
   static constexpr int STAGES_CAP = LEAN ? GEMM_LEAN_STAGES : BT <= 64 ? TGIS_GEMM_DECODE_STAGES : 12;
   static constexpr int STAGES = STAGES_RAW > STAGES_CAP ? STAGES_CAP : STAGES_RAW;
-  static constexpr int PART_FLOATS = NW * BT * GEMM_BN;                  // fp32 partial of one unit
-  static constexpr int BAR_BYTES = 512;   // mbarriers (full, empty, ready, xfull), flag
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + BAR_BYTES + 256 /*rstd*/;
-  // fused-norm consumers append the norm weights (+ K * 2 bytes, K <= 8192)
-  static constexpr int SMEM_MAX =
-      LEAN ? SMEM_BYTES : (SMEM_BYTES + 16384) < 227 * 1024 ? (SMEM_BYTES + 16384) : 227 * 1024;
-  static constexpr int THREADS = !LEAN && BT <= GEMM_NORM_MAX_T ? GEMM_THREADS_NORM : GEMM_THREADS;  // launch bound
+  static constexpr int PART_FLOATS = BT * GEMM_BN;                       // fp32 partial of one unit
+  static constexpr int BAR_BYTES = 512;   // mbarriers (full, empty), flag
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + BAR_BYTES;
   static constexpr int MIN_BLOCKS = LEAN ? 2 : 1;
   static_assert(!LEAN || 2 * (SMEM_BYTES + 1024) <= 228 * 1024, "two lean CTAs must fit one SM's shared memory");
   static_assert(!LEAN || PART_FLOATS * 4 <= STAGES * STAGE_BYTES, "the cluster reduction parks a partial in the ring");
@@ -235,22 +224,17 @@ __device__ __forceinline__ void qkv_rope_store(const GemmRope& rope, int head, i
   }
 }
 
-// (the fused-norm warps only exist for token tiles of at most GEMM_NORM_MAX_T rows and not in the lean instantiation:
-// larger tiles get their registers, the lean one its second CTA per SM)
-template <int BT, int NW, bool LEAN>
-__global__ void __launch_bounds__(GemmCfg<BT, NW, LEAN>::THREADS, GemmCfg<BT, NW, LEAN>::MIN_BLOCKS)
+template <int BT, bool LEAN>
+__global__ void __launch_bounds__(GEMM_THREADS, GemmCfg<BT, LEAN>::MIN_BLOCKS)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap xmap,
                          void* __restrict__ Yv, int ldy, int T, int N, int K, float* __restrict__ ws,
-                         int* __restrict__ counters, int stream_weights, int out_f32,
-                         const __grid_constant__ CUtensorMap next_wmap, GemmNext nxt, int cluster_split,
-                         GemmRope rope, GemmNorm norm) {
+                         int* __restrict__ counters, int stream_weights, int out_f32, int cluster_split,
+                         GemmRope rope) {
   // output: bf16 (rounded once from the fp32 accumulator, = F.linear in model dtype) or raw fp32 (lm_head logits)
   __nv_bfloat16* __restrict__ Y = reinterpret_cast<__nv_bfloat16*>(Yv);
   float* __restrict__ Yf = reinterpret_cast<float*>(Yv);
-  using Cfg = GemmCfg<BT, NW, LEAN>;
-  constexpr bool NORM_ROLES = !LEAN && BT <= GEMM_NORM_MAX_T;  // fused RMSNorm consumer (warps 9..10) compiled in
+  using Cfg = GemmCfg<BT, LEAN>;
   constexpr int STAGES = Cfg::STAGES;
-  constexpr int BNW = GEMM_BN * NW;            // weight rows per unit
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_w = smem;
@@ -259,27 +243,17 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
   int* flag_smem = reinterpret_cast<int*>(bars + 2 * STAGES);
-  uint64_t* ready_bar = bars + 40;  // [STAGES <= 12] fused-norm consumer: token tile of the stage normalised in place
-  uint64_t* xfull_bar = bars + 52;  // [STAGES <= 12] fused-norm consumer: raw token tile landed (weights: full_bar)
-  float* rstd_smem = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES);  // [64]
-  uint8_t* wn_smem = smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES + 256;                      // [K] bf16 norm weights
-  // the token operand is RMSNorm(h): warps 9..10 rewrite each landed stage in place
-  const bool norm_in = NORM_ROLES && norm.h != nullptr;
 
   const int warp = threadIdx.x >> 5;
   STL_ENTER(2 | (N << 8));
   int* stl_slot_smem = flag_smem + 1;
   STL_SHARE(stl_slot_smem);  // read by the other warps after the set-up barrier
   if (threadIdx.x == 0) TL(0);  // kernel entry
-  const int n_tiles = (N + BNW - 1) / BNW;     // units along N
+  const int n_tiles = (N + GEMM_BN - 1) / GEMM_BN;
   const int t_tiles = (T + BT - 1) / BT;
   const int KB = (K + GEMM_BK - 1) / GEMM_BK;
   const int ncta = gridDim.x, cta = blockIdx.x;
   const GemmSched sched(n_tiles, t_tiles, KB, ncta, (stream_weights & 2) != 0);
-  // cluster mode, push variant: every CTA sends its partial rows straight into the OWNER's receive buffer (tokens
-  // t = r (mod s) belong to rank r), ONE cluster barrier, then each owner sums its own shared memory in rank order -- no
-  // remote read latency and no exit barrier (pull variant: park locally, barrier, read peers, barrier)
-  const bool cl_push = !LEAN && (stream_weights & 4) != 0;
   stream_weights &= 1;
   const long long total = sched.sk_total;  // stream-K region (== everything for decode-shaped launches)
 
@@ -289,69 +263,13 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], EP_WARPS);  // lane 0 of every consumer warp, once its MMAs on the stage retired
-      mbar_init(&ready_bar[i], 1);  // the transform warp that owns the stage's k-block (fused-norm consumer)
-      mbar_init(&xfull_bar[i], 1);
     }
     fence_barrier_init();
   }
   __syncthreads();
-  // push variant: peers write into this CTA's shared memory as soon as THEY are done -- every CTA of the cluster must be
-  // running before the first remote store (arrive now, wait right before pushing: free by then)
-  if (cl_push) asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
   griddep_launch();  // PDL: the next kernel may start its prologue now
   if (threadIdx.x == 0) TL(1);  // setup done (barriers)
   int cl_tile = -1, cl_tvalid = 0;  // cluster mode: the split tile this CTA contributed to (epilogue warps)
-
-  // ---- fused residual-stream RMSNorm (GemmNorm consumer side): xmap points at the residual stream h, so the producer
-  // warp's TMA stages the RAW [BT x 64] token tile (own barrier xfull_bar: it lands long before the weight tile).  A warp
-  // rewrites one landed stage IN PLACE as bf16(bf16(h * rstd) * w) -- 16-byte chunk c of row r sits at
-  // r * 128 + ((c ^ (r & 7)) << 4) under the 128-byte swizzle; lane -> chunk lane & 7, rows (lane >> 3) + 4 j -- and
-  // signals ready_bar, which the consumer warps wait for.  Warps 9 / 10 take the even / odd k-blocks; when the dependency
-  // resolves a whole ring of tiles lands at once, so the (then idle) first consumer warpgroup takes k-blocks 2..5 of that
-  // burst before it issues its first MMA.
-  constexpr int NJ = NORM_ROLES ? BT / 4 : 1;
-  const int norm_n_kb = (int)((total * (cta + 1)) / ncta - (total * cta) / ncta);  // decode-shaped: no whole-tile waves
-  const int norm_kb0 = (int)(((total * cta) / ncta) % KB);
-  const bool norm_helpers = norm_in && STAGES >= 6 && norm_n_kb >= 6;
-  auto norm_stage = [&](int i, const float (&rs)[NJ]) {
-    const int lane = lane_id();
-    const int c = lane & 7, r0 = lane >> 3;
-    const int stage = i % STAGES;
-    const uint32_t phase = (uint32_t)(i / STAGES) & 1u;
-    const int kb = (norm_kb0 + i) % KB;
-    uint32_t wb[4];
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];\n"
-                 : "=r"(wb[0]), "=r"(wb[1]), "=r"(wb[2]), "=r"(wb[3])
-                 : "r"(smem_u32(wn_smem) + (uint32_t)((kb * GEMM_BK + c * 8) * 2)));
-    mbar_wait(&xfull_bar[stage], phase);
-    const uint32_t st_base = smem_u32(smem_x) + (uint32_t)(stage * Cfg::X_BYTES);
-    uint32_t hb[NJ][4];
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int r = r0 + 4 * j;
-      asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];\n"
-                   : "=r"(hb[j][0]), "=r"(hb[j][1]), "=r"(hb[j][2]), "=r"(hb[j][3])
-                   : "r"(st_base + (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4))));
-    }
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int r = r0 + 4 * j;
-      uint32_t ob[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float h0 = __uint_as_float(hb[j][e] << 16), h1 = __uint_as_float(hb[j][e] & 0xffff0000u);
-        const float w0 = __uint_as_float(wb[e] << 16), w1 = __uint_as_float(wb[e] & 0xffff0000u);
-        const __nv_bfloat162 o2 = __floats2bfloat162_rn(bf16_round(h0 * rs[j]) * w0, bf16_round(h1 * rs[j]) * w1);
-        ob[e] = *reinterpret_cast<const uint32_t*>(&o2);
-      }
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};\n" ::"r"(st_base + (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4))),
-                   "r"(ob[0]), "r"(ob[1]), "r"(ob[2]), "r"(ob[3])
-                   : "memory");
-    }
-    fence_proxy_async();  // generic-proxy stores -> visible to the tensor core's async-proxy reads
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&ready_bar[stage]);
-  };
 
   if (warp == PRODUCER_WARP) {
     // ===================== TMA producer =====================
@@ -373,7 +291,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
         c.tile = tile;
         int n_tile, t_tile;
         tile_decode(sched, tile, n_tile, t_tile);
-        c.w_row = n_tile * BNW;
+        c.w_row = n_tile * GEMM_BN;
         c.x_row = t_tile * BT;
       };
       auto cur_init = [&](Cur& c) {
@@ -414,22 +332,17 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
         }
       };
       auto issue_w = [&](const Cur& c, int stage) {
-#pragma unroll
-        for (int h = 0; h < NW; ++h) {  // NW boxes of 128 rows (rows beyond N are zero-filled by TMA and still counted)
-          void* dst = smem_w + stage * Cfg::W_BYTES + h * Cfg::W_TILE_BYTES;
-          if (stream_weights) tma_load_2d_hint(&wmap, &full_bar[stage], dst, c.kb * GEMM_BK, c.w_row + h * GEMM_BN, pol_w);
-          else tma_load_2d(&wmap, &full_bar[stage], dst, c.kb * GEMM_BK, c.w_row + h * GEMM_BN);
-        }
+        // one box of 128 rows (rows beyond N are zero-filled by TMA and still counted)
+        void* dst = smem_w + stage * Cfg::W_BYTES;
+        if (stream_weights) tma_load_2d_hint(&wmap, &full_bar[stage], dst, c.kb * GEMM_BK, c.w_row, pol_w);
+        else tma_load_2d(&wmap, &full_bar[stage], dst, c.kb * GEMM_BK, c.w_row);
       };
       const int n_pre = n_kb < STAGES ? n_kb : STAGES;
       Cur wc, xc;
       cur_init(wc);
       xc = wc;
-      // fused-norm consumer: the (small, L2-resident) token tile gets its own barrier, so it is normalised while the
-      // stage's weight tile is still in flight and the rewrite adds nothing to the time a ring slot stays occupied
-      const uint32_t w_tx = norm_in ? (uint32_t)Cfg::W_BYTES : (uint32_t)Cfg::STAGE_BYTES;
       for (int i = 0; i < n_pre; ++i) {
-        mbar_arrive_expect_tx(&full_bar[i], w_tx);
+        mbar_arrive_expect_tx(&full_bar[i], Cfg::STAGE_BYTES);
         issue_w(wc, i);
         cur_next(wc);
       }
@@ -442,16 +355,11 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
       for (int i = 0; i < n_kb; ++i) {
         if (i >= n_pre) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], w_tx);
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
           issue_w(wc, stage);
           cur_next(wc);
         }
-        uint64_t* x_bar = &full_bar[stage];
-        if (norm_in) {
-          x_bar = &xfull_bar[stage];
-          mbar_arrive_expect_tx(x_bar, Cfg::X_BYTES);
-        }
-        tma_load_2d_hint(&xmap, x_bar, smem_x + stage * Cfg::X_BYTES, xc.kb * GEMM_BK, xc.x_row, pol_x);
+        tma_load_2d_hint(&xmap, &full_bar[stage], smem_x + stage * Cfg::X_BYTES, xc.kb * GEMM_BK, xc.x_row, pol_x);
         cur_next(xc);
         if (++stage == STAGES) {
           stage = 0;
@@ -460,46 +368,21 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
       }
       TL(4);  // last TMA issued
       STL_EXTRA(*stl_slot_smem, 1);
-      // Cross-kernel weight prefetch: HBM goes idle while this kernel drains its pipeline, reduces split tiles and
-      // exits, and the next GEMM of the layer stack needs ~10 us before its own loads are in flight.  So the boxes
-      // that the next GEMM's CTAs will read FIRST are pulled into the 50 MB L2 now (TMA prefetch, no smem, no
-      // completion tracking): next CTA c2 starts at k-block (total2 * c2 / grid2) of its (tile, k-block) space.
-      if (nxt.kb_prefetch > 0) {
-        const long long total2 = (long long)nxt.n_tiles * nxt.KB;
-        for (int c2 = cta; c2 < nxt.grid; c2 += ncta) {
-          const long long b2 = (total2 * c2) / nxt.grid, e2 = (total2 * (c2 + 1)) / nxt.grid;
-          const int n2 = (int)((e2 - b2) < nxt.kb_prefetch ? (e2 - b2) : nxt.kb_prefetch);
-          int tile2 = (int)(b2 / nxt.KB), kb2 = (int)(b2 % nxt.KB);
-          for (int i = 0; i < n2; ++i) {
-            for (int h = 0; h < NW; ++h) tma_prefetch_2d(&next_wmap, kb2 * GEMM_BK, tile2 * BNW + h * GEMM_BN);
-            if (++kb2 == nxt.KB) { kb2 = 0; ++tile2; }
-          }
-        }
-      }
     }
   } else if (warp < EP_WARPS) {
     // ===================== consumers: wgmma on weight rows 64 wg .. 64 wg + 63, epilogue from registers ==========
     const int wg = warp >> 2;
     const int lane = lane_id();
     const int ep_tid = threadIdx.x;
-    // accumulator fragment (ptx.cuh wgmma_m64k16): d[h][4 j + 2 hh + e] holds weight row frag_row + 8 hh, token
+    // accumulator fragment (ptx.cuh wgmma_m64k16): d[4 j + 2 hh + e] holds weight row frag_row + 8 hh, token
     // 8 j + frag_col + e
     const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     const int frag_col = 2 * (lane & 3);
-    if constexpr (NORM_ROLES) {
-      if (norm_helpers && warp < 4) {  // start-up burst of the fused-norm consumer: k-blocks 2..5
-        asm volatile("bar.sync 2, 192;\n" ::: "memory");  // rstd is in shared memory
-        float rs[NJ];
-#pragma unroll
-        for (int j = 0; j < NJ; ++j) rs[j] = rstd_smem[(lane >> 3) + 4 * j];
-        norm_stage(warp + 2, rs);  // warps 0..3
-      }
-    }
     UnitIter it(sched, cta);
     int tile, kb0, kb1, slot;
     int stage = 0;
     uint32_t phase = 0;
-    float d[NW][BT / 2];
+    float d[BT / 2];
     while (it.next(tile, kb0, kb1, slot)) {
       int n_tile, t_tile;
       tile_decode(sched, tile, n_tile, t_tile);
@@ -509,31 +392,21 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
       int prev_stage = 0;
       // (the first MMA of a unit overwrites d; zeroing it here ends the previous unit's live range for the compiler)
 #pragma unroll
-      for (int h = 0; h < NW; ++h)
-#pragma unroll
-        for (int i = 0; i < BT / 2; ++i) d[h][i] = 0.f;
+      for (int i = 0; i < BT / 2; ++i) d[i] = 0.f;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        if (norm_in) mbar_wait(&ready_bar[stage], phase);  // the token tile has been normalised in place
         if (ep_tid == 0 && kb == kb0) STL_EXTRA(*stl_slot_smem, 0);
         const uint64_t b_desc = make_smem_desc_sw128(smem_u32(smem_x + stage * Cfg::X_BYTES));
-#pragma unroll
-        for (int h = 0; h < NW; ++h) wgmma_fence_acc(d[h]);
+        wgmma_fence_acc(d);
         wgmma_fence();
+        const uint64_t a_desc = make_smem_desc_sw128(smem_u32(smem_w + stage * Cfg::W_BYTES + wg * (64 * GEMM_BK * 2)));
 #pragma unroll
-        for (int h = 0; h < NW; ++h) {
-          const uint64_t a_desc = make_smem_desc_sw128(
-              smem_u32(smem_w + stage * Cfg::W_BYTES + h * Cfg::W_TILE_BYTES + wg * (64 * GEMM_BK * 2)));
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) {
-            // advance 16 bf16 = 32 B inside the 128-B swizzle atom: +2 in 16-byte units on the start address
-            wgmma_m64k16<BT>(d[h], a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2),
-                             (kb > kb0 || k > 0) ? 1u : 0u);
-          }
+        for (int k = 0; k < GEMM_BK / 16; ++k) {
+          // advance 16 bf16 = 32 B inside the 128-B swizzle atom: +2 in 16-byte units on the start address
+          wgmma_m64k16<BT>(d, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), (kb > kb0 || k > 0) ? 1u : 0u);
         }
         wgmma_commit();
-#pragma unroll
-        for (int h = 0; h < NW; ++h) wgmma_fence_acc(d[h]);
+        wgmma_fence_acc(d);
         // the previous k-block's MMAs have retired: its stage goes back to the producer
         wgmma_wait<1>();
         if (kb > kb0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
@@ -544,50 +417,34 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
         }
       }
       wgmma_wait<0>();
-#pragma unroll
-      for (int h = 0; h < NW; ++h) wgmma_fence_acc(d[h]);
+      wgmma_fence_acc(d);
       if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-      if (cl_push) asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");  // all peers are running
-      // pull variant: the partial goes into the ring, which the other warpgroup may still be reading
-      if (partial && cluster_split > 0 && !cl_push) asm volatile("bar.sync 1, %0;\n" ::"n"(EP_THREADS) : "memory");
+      // cluster mode: the partial goes into the ring, which the other warpgroup may still be reading
+      if (partial && cluster_split > 0) asm volatile("bar.sync 1, %0;\n" ::"n"(EP_THREADS) : "memory");
       if (ep_tid == 0) TL(5);  // accumulator ready (all MMAs of the unit retired)
-      if (ep_tid == 0 && !norm_in) STL_EXTRA(*stl_slot_smem, 2);
+      if (ep_tid == 0) STL_EXTRA(*stl_slot_smem, 2);
       float* my_ws = ws + (size_t)(cta * 2 + slot) * Cfg::PART_FLOATS;
-      const int crank_e = cl_push ? (int)cluster_ctarank() : 0;
-      const int tpo = cl_push ? (BT + cluster_split - 1) / cluster_split : 0;
 #pragma unroll
-      for (int h = 0; h < NW; ++h) {  // the unit's NW accumulators = weight tiles n_tile * NW + h
-#pragma unroll
-        for (int i = 0; i < BT / 2; ++i) {
-          const int row = frag_row + 8 * ((i >> 1) & 1);  // weight row within the tile
-          const int c = 8 * (i >> 2) + frag_col + (i & 1);  // token within the token tile
-          const int n = (n_tile * NW + h) * GEMM_BN + row;
-          const float v = d[h][i];
-          if (!partial) {
-            if (out_f32 == 2) {
-              // fused SwiGLU: weight rows are interleaved (2j = gate_j, 2j+1 = up_j); the partner row sits in lane ^ 4,
-              // even rows produce act[t, n/2]
-              const float other = __shfl_xor_sync(0xffffffffu, v, 4);
-              if ((row & 1) == 0 && n < N && c < t_valid) Y[(size_t)(t_base + c) * ldy + (n >> 1)] = swiglu_bf16(v, other);
-            } else if (n < N && c < t_valid) {
-              const size_t o = (size_t)(t_base + c) * ldy + n;
-              if (out_f32) Yf[o] = v;
-              else Y[o] = __float2bfloat16_rn(v);
-            }
-          } else if (c < t_valid) {
-            // split tile: fp32 partial [token][128 rows] to the global workspace, or (cluster mode) to shared memory
-            if (cl_push) {
-              // receive buffer of owner c % s (behind the ring, never aliased with in-flight stages -- the owner may
-              // still be in its main loop): [source rank][local token index c / s][128 rows]
-              const uint32_t ra = dsmem_addr(
-                  smem_u32(wn_smem) + (uint32_t)(((crank_e * tpo + c / cluster_split) * GEMM_BN + row) * 4),
-                  (uint32_t)(c % cluster_split));
-              asm volatile("st.shared::cluster.f32 [%0], %1;\n" ::"r"(ra), "f"(v) : "memory");
-            } else {
-              float* dst = (cluster_split > 0 ? reinterpret_cast<float*>(smem) : my_ws) + h * (BT * GEMM_BN);
-              dst[(size_t)c * GEMM_BN + row] = v;
-            }
+      for (int i = 0; i < BT / 2; ++i) {
+        const int row = frag_row + 8 * ((i >> 1) & 1);  // weight row within the tile
+        const int c = 8 * (i >> 2) + frag_col + (i & 1);  // token within the token tile
+        const int n = n_tile * GEMM_BN + row;
+        const float v = d[i];
+        if (!partial) {
+          if (out_f32 == 2) {
+            // fused SwiGLU: weight rows are interleaved (2j = gate_j, 2j+1 = up_j); the partner row sits in lane ^ 4,
+            // even rows produce act[t, n/2]
+            const float other = __shfl_xor_sync(0xffffffffu, v, 4);
+            if ((row & 1) == 0 && n < N && c < t_valid) Y[(size_t)(t_base + c) * ldy + (n >> 1)] = swiglu_bf16(v, other);
+          } else if (n < N && c < t_valid) {
+            const size_t o = (size_t)(t_base + c) * ldy + n;
+            if (out_f32) Yf[o] = v;
+            else Y[o] = __float2bfloat16_rn(v);
           }
+        } else if (c < t_valid) {
+          // split tile: fp32 partial [token][128 rows] to the global workspace, or (cluster mode) to shared memory
+          float* dst = cluster_split > 0 ? reinterpret_cast<float*>(smem) : my_ws;
+          dst[(size_t)c * GEMM_BN + row] = v;
         }
       }
       if (ep_tid == 0) TL(6);  // partial/direct stores issued
@@ -618,10 +475,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
           constexpr int FIX_C = LEAN ? 2 : 3, FIX_T = LEAN ? 2 : 8;
           const int r4 = (ep_tid & 31) * 4;   // first of this thread's 4 rows
           const int tq = ep_tid >> 5;         // token phase 0..EP_WARPS-1
-#pragma unroll 1
-          for (int h = 0; h < NW; ++h) {
-          const int nt = n_tile * NW + h;     // weight tile (= head of the qkv projection)
-          const int n4 = nt * GEMM_BN + r4;
+          const int n4 = n_tile * GEMM_BN + r4;
           for (int tb = tq; tb < t_valid; tb += EP_WARPS * FIX_T) {
             float4 acc[FIX_T];
 #pragma unroll
@@ -634,7 +488,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
                 const bool cv = c <= c_last;
                 const long long cb = cv ? (total * c) / ncta : 0;
                 const int cslot = ((int)(cb / KB) == tile - sched.sk_tile0) ? 0 : 1;
-                const float* p = ws + (size_t)((cv ? c : c_first) * 2 + cslot) * Cfg::PART_FLOATS + h * (BT * GEMM_BN) + r4;
+                const float* p = ws + (size_t)((cv ? c : c_first) * 2 + cslot) * Cfg::PART_FLOATS + r4;
 #pragma unroll
                 for (int j = 0; j < FIX_T; ++j) {
                   const int t = tb + EP_WARPS * j;
@@ -656,7 +510,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
                 const size_t o = (size_t)(t_base + t) * ldy + n4;
                 const float av[4] = {acc[j].x, acc[j].y, acc[j].z, acc[j].w};
                 if (rope.positions != nullptr) {  // qkv projection: RoPE + KV scatter (warp-uniform t and tile)
-                  qkv_rope_store(rope, nt, t_base + t, r4, av, Y + o);
+                  qkv_rope_store(rope, n_tile, t_base + t, r4, av, Y + o);
                 } else if (out_f32 == 2) {  // fused SwiGLU: rows (n4, n4+1) and (n4+2, n4+3) are (gate, up) pairs
                   __nv_bfloat16* yo = Y + (size_t)(t_base + t) * ldy + (n4 >> 1);
                   if (n4 + 1 < N) yo[0] = swiglu_bf16(av[0], av[1]);
@@ -681,66 +535,17 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
               }
             }
           }
-          }
           if (ep_tid == 0) counters[tile] = 0;
           if (ep_tid == 0) TL(8);  // ordered reduction done (last arriver only)
         }
         asm volatile("bar.sync 1, %0;\n" ::"n"(EP_THREADS) : "memory");  // flag_smem reuse safety
       }
     }
-  } else if (norm_in) {
-    // ===================== activation transform: fused residual-stream RMSNorm (warps 9..10) ====================
-    // k-blocks alternate between the two warps; consumer warps 0..3 take k-blocks 2..5 of the start-up burst (see
-    // norm_stage above).  rstd first: lane p fetches partial sum p of every row of this warp's half of the token tile
-    // (all loads independent: one L2 round trip), a fixed shuffle tree adds them (deterministic).
-    if constexpr (NORM_ROLES) {
-      const int tw = warp - NORM_WARP0;            // 0 / 1
-      const int tid = threadIdx.x - GEMM_THREADS;  // 0..63
-      const int lane = lane_id();
-      // the norm weights are static: all of them into shared memory before the dependency wait
-      for (int i = tid; i < K / 8; i += 64)
-        reinterpret_cast<uint4*>(wn_smem)[i] = __ldg(reinterpret_cast<const uint4*>(norm.w_norm) + i);
-      griddep_wait();  // the partial sums (and h, through the producer warp's TMA) come from the preceding GEMM
-      if (tid == 0) STL_EXTRA(*stl_slot_smem, 2);  // (timeline builds: fused consumers report this instead of acc-ready)
-      constexpr int RW = BT / 2;
-      const int row0 = tw * RW, np = norm.n_parts;
-      const bool ok0 = lane < np, ok1 = lane + 32 < np;
-      float v[RW];
-#pragma unroll
-      for (int r = 0; r < RW; ++r) {
-        const int row = row0 + r;
-        const float* pp = norm.sumsq_in + (size_t)(row < T ? row : 0) * np;
-        const float a0 = __ldcg(pp + (ok0 ? lane : 0)), a1 = __ldcg(pp + (ok1 ? lane + 32 : 0));
-        v[r] = (ok0 ? a0 : 0.f) + (ok1 ? a1 : 0.f);
-      }
-      // level by level over ALL rows (RW independent shuffles in flight per level), then lane r finishes row r
-#pragma unroll
-      for (int sh = 16; sh > 0; sh >>= 1) {
-#pragma unroll
-        for (int r = 0; r < RW; ++r) v[r] += __shfl_xor_sync(0xffffffffu, v[r], sh);
-      }
-      float mine = 0.f;
-#pragma unroll
-      for (int r = 0; r < RW; ++r) mine = lane == r ? v[r] : mine;
-      if (lane < RW) rstd_smem[row0 + lane] = row0 + lane < T ? rsqrtf(mine / (float)K + norm.eps) : 0.f;
-      if (norm_helpers) asm volatile("bar.sync 2, 192;\n" ::: "memory");
-      else asm volatile("bar.sync 2, 64;\n" ::: "memory");
-      if (tid == 0) STL_EXTRA(*stl_slot_smem, 3);
-      float rs[NJ];
-#pragma unroll
-      for (int j = 0; j < NJ; ++j) rs[j] = rstd_smem[(lane >> 3) + 4 * j];
-      int i = tw;
-      if (i < norm_n_kb) norm_stage(i, rs);
-      i += norm_helpers ? 6 : 2;
-      for (; i < norm_n_kb; i += 2) norm_stage(i, rs);
-    }
   }
 
   if (cluster_split > 0) {
     // ---- on-chip split-K reduction across the cluster (all threads take part in the cluster barriers)
-    // (push variant: the consumer warps consumed the start-up phase before their remote stores, the others do it here)
-    if (cl_push && warp >= EP_WARPS) asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-    cluster_sync_all();  // every CTA's partial is in its (pull) / its owner's (push) shared memory
+    cluster_sync_all();  // every CTA's partial is in its shared memory
     if (warp < EP_WARPS && cl_tile >= 0) {
       const int ep_tid = threadIdx.x;
       const int crank = (int)cluster_ctarank();
@@ -748,36 +553,18 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
       const int tq = ep_tid >> 5;         // token phase 0..EP_WARPS-1
       const uint32_t stg = smem_u32(smem);
       constexpr int FIX_T = LEAN ? 2 : 4;  // (lean: a CTA owns at most 16 tokens of its 32-token tile at split >= 2)
-#pragma unroll 1
-      for (int h = 0; h < NW; ++h) {
-      const int nt = cl_tile * NW + h;    // weight tile (= head of the qkv projection)
-      const int n4 = nt * GEMM_BN + r4;
-      const uint32_t hoff = (uint32_t)(h * BT * GEMM_BN * 4);
+      const int n4 = cl_tile * GEMM_BN + r4;
       // tokens of this CTA: t = crank + split * i; thread takes i = tq (mod EP_WARPS)
       for (int i0 = tq; crank + cluster_split * i0 < cl_tvalid; i0 += EP_WARPS * FIX_T) {
         float4 acc[FIX_T];
 #pragma unroll
         for (int j = 0; j < FIX_T; ++j) acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-        uint2 resv[FIX_T];  // fused residual add: this thread's residual values, in flight during the DSMEM reads
-        if (!LEAN && norm.sumsq_out != nullptr) {
-#pragma unroll
-          for (int j = 0; j < FIX_T; ++j) {
-            const int t = crank + cluster_split * (i0 + EP_WARPS * j);
-            resv[j] = t < cl_tvalid ? __ldcg(reinterpret_cast<const uint2*>(norm.residual + (size_t)t * ldy + n4))
-                                    : make_uint2(0u, 0u);
-          }
-        }
         for (int c = 0; c < cluster_split; ++c) {  // contributor rank order = k order: deterministic
-          const uint32_t peer = dsmem_addr(stg, (uint32_t)c) + hoff;
-          const int tpo = (BT + cluster_split - 1) / cluster_split;
+          const uint32_t peer = dsmem_addr(stg, (uint32_t)c);
           float4 v[FIX_T];
 #pragma unroll
           for (int j = 0; j < FIX_T; ++j) {
             const int t = crank + cluster_split * (i0 + EP_WARPS * j);
-            if (cl_push)  // own receive buffer: [source rank c][local token index][128 rows]
-              v[j] = t < cl_tvalid ? *reinterpret_cast<const float4*>(wn_smem + (size_t)(((c * tpo + i0 + EP_WARPS * j) * GEMM_BN + r4) * 4))
-                                   : make_float4(0.f, 0.f, 0.f, 0.f);
-            else
             v[j] = t < cl_tvalid ? ld_dsmem_f4(peer + (uint32_t)((t * GEMM_BN + r4) * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
           }
 #pragma unroll
@@ -791,27 +578,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
           if (t < cl_tvalid) {
             const size_t o = (size_t)t * ldy + n4;
             const float av[4] = {acc[j].x, acc[j].y, acc[j].z, acc[j].w};
-            if (!LEAN && norm.sumsq_out != nullptr) {
-              // h = bf16(bf16(y) + residual) (fused_add_rms_norm's add), back into the residual stream, + this tile's
-              // share of sum(h^2) for the consumer's rstd; t and the tile are warp-uniform
-              const float rr[4] = {__uint_as_float(resv[j].x << 16), __uint_as_float(resv[j].x & 0xffff0000u),
-                                   __uint_as_float(resv[j].y << 16), __uint_as_float(resv[j].y & 0xffff0000u)};
-              float hh[4], ssq = 0.f;
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                hh[e] = bf16_round(bf16_round(av[e]) + rr[e]);
-                ssq += hh[e] * hh[e];
-              }
-              __nv_bfloat162 lo = __floats2bfloat162_rn(hh[0], hh[1]), hi = __floats2bfloat162_rn(hh[2], hh[3]);
-              uint2 pk;
-              pk.x = *reinterpret_cast<uint32_t*>(&lo);
-              pk.y = *reinterpret_cast<uint32_t*>(&hi);
-              *reinterpret_cast<uint2*>(norm.residual + o) = pk;
-#pragma unroll
-              for (int sh = 16; sh > 0; sh >>= 1) ssq += __shfl_xor_sync(0xffffffffu, ssq, sh);
-              if (lane_id() == 0) norm.sumsq_out[(size_t)t * (N / GEMM_BN) + nt] = ssq;
-            } else if (rope.positions != nullptr) {
-              qkv_rope_store(rope, nt, t, r4, av, Y + o);
+            if (rope.positions != nullptr) {
+              qkv_rope_store(rope, cl_tile, t, r4, av, Y + o);
             } else if (out_f32 == 2) {
               __nv_bfloat16* yo = Y + (size_t)t * ldy + (n4 >> 1);
               if (n4 + 1 < N) yo[0] = swiglu_bf16(av[0], av[1]);
@@ -836,9 +604,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
           }
         }
       }
-      }
     }
-    if (!cl_push) cluster_sync_all();  // nobody exits while a peer may still read its shared memory
+    cluster_sync_all();  // nobody exits while a peer may still read its shared memory
   }
   if (threadIdx.x == 0) TL(9);  // all roles done
   STL_EXIT();
@@ -892,44 +659,20 @@ int gemm_pick_bt(int T) {
   return 256;
 }
 
-// Weight tiles per unit (GemmCfg).  1 everywhere by default.  TGIS_GEMM_NW=2 makes decode-shaped launches share one
-// activation tile between two weight tiles (half the activation re-reads per weight byte): an experiment, not the
-// default -- halving the tile count doubles the partial size of every split-K reduction and leaves 5 ring stages instead
-// of 8.  Token tiles of at most 128 rows only: two accumulators of 256 tokens do not fit a thread's registers.
-int gemm_nw(int T) {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TGIS_GEMM_NW");
-    v = (e && e[0] == '2') ? 2 : 1;
-  }
-  return T <= 128 ? v : 1;
-}
-static int gemm_bn(int T) { return GEMM_BN * gemm_nw(T); }
-
-static bool gemm_cluster_enabled() {  // TGIS_GEMM_CLUSTER=0: always reduce split tiles through global memory
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TGIS_GEMM_CLUSTER");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-template <int BT, int NW, bool LEAN>
+template <int BT, bool LEAN>
 __global__ void gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap, const __grid_constant__ CUtensorMap, void*, int,
-                                         int, int, int, float*, int*, int, int, const __grid_constant__ CUtensorMap,
-                                         GemmNext, int, GemmRope, GemmNorm);
+                                         int, int, int, float*, int*, int, int, int, GemmRope);
 
 // Per-instantiation function attributes, set once (retried until they succeed): the dynamic shared memory limit, and for
 // the lean instantiation the full 228 KB shared-memory carveout its two CTAs per SM need.
-template <int BT, int NW, bool LEAN>
+template <int BT, bool LEAN>
 static cudaError_t gemm_set_attrs() {
   static bool done = false;
   if (done) return cudaSuccess;
-  cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BT, NW, LEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       GemmCfg<BT, NW, LEAN>::SMEM_MAX);
+  cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BT, LEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       GemmCfg<BT, LEAN>::SMEM_BYTES);
   if (e == cudaSuccess && LEAN)
-    e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BT, NW, LEAN>, cudaFuncAttributePreferredSharedMemoryCarveout,
+    e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BT, LEAN>, cudaFuncAttributePreferredSharedMemoryCarveout,
                              (int)cudaSharedmemCarveoutMaxShared);
   done = e == cudaSuccess;
   return e;
@@ -944,7 +687,7 @@ static int gemm_max_clusters(int s, int num_sms) {
   static int cache[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   if (s < 2 || s > 8) return num_sms / (s > 0 ? s : 1);
   if (cache[s] == 0) {
-    using Cfg = GemmCfg<32, 1>;
+    using Cfg = GemmCfg<32>;
     cudaLaunchConfig_t qc{};
     qc.gridDim = dim3(s * (num_sms / s));
     qc.blockDim = dim3(GEMM_THREADS);
@@ -957,8 +700,8 @@ static int gemm_max_clusters(int s, int num_sms) {
     qc.attrs = qa;
     qc.numAttrs = 1;
     int n = 0;
-    if (gemm_set_attrs<32, 1, false>() == cudaSuccess &&
-        cudaOccupancyMaxActiveClusters(&n, gemm_bf16_wgmma_kernel<32, 1, false>, &qc) == cudaSuccess && n > 0) {
+    if (gemm_set_attrs<32, false>() == cudaSuccess &&
+        cudaOccupancyMaxActiveClusters(&n, gemm_bf16_wgmma_kernel<32, false>, &qc) == cudaSuccess && n > 0) {
       cache[s] = n;
     } else {
       cudaGetLastError();
@@ -967,21 +710,13 @@ static int gemm_max_clusters(int s, int num_sms) {
   }
   return cache[s];
 }
-static bool gemm_fit_clusters() {  // TGIS_GEMM_FIT_CLUSTERS=0: round-1 policy (largest split, cluster mode only if it fits)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TGIS_GEMM_FIT_CLUSTERS");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
 
 size_t gemm_workspace_bytes(int num_sms) { return (size_t)num_sms * 2 * 2 * 256 * GEMM_BN * sizeof(float); }
 
 // Grid size of a launch (pure function of the shape: the NEXT kernel's grid must be known one launch ahead)
 int gemm_grid_size(int T, int N, int K, int num_sms) {
-  const int BT = gemm_pick_bt(T), BN = gemm_bn(T);
-  const int n_tiles = (N + BN - 1) / BN, t_tiles = (T + BT - 1) / BT, KB = (K + GEMM_BK - 1) / GEMM_BK;
+  const int BT = gemm_pick_bt(T);
+  const int n_tiles = (N + GEMM_BN - 1) / GEMM_BN, t_tiles = (T + BT - 1) / BT, KB = (K + GEMM_BK - 1) / GEMM_BK;
   long long total = (long long)n_tiles * t_tiles * KB;
   // do not cut finer than 4 k-blocks per CTA: tiny problems use fewer CTAs
   long long max_ctas = (total + 3) / 4;
@@ -1002,7 +737,7 @@ int gemm_grid_size(int T, int N, int K, int num_sms) {
     // Prefer a split whose clusters are all co-resident (qkv of the 8B model: 48 tiles x 3 CTAs -- only 45 clusters of 3
     // fit, so round 1 reduced it through global memory; 48 clusters of 2 fit): the on-chip reduction spreads the fused
     // RoPE + KV-scatter epilogue over the cluster's CTAs, which is what lets it replace rope_kvwrite_kernel above 32 tokens
-    if (gemm_fit_clusters() && gemm_cluster_enabled() && t_tiles == 1)
+    if (t_tiles == 1)
       while (split > 2 && tiles > gemm_max_clusters(split, num_sms)) --split;
     grid = (int)(tiles * split);
   }
@@ -1015,8 +750,8 @@ int gemm_grid_size(int T, int N, int K, int num_sms) {
 
 // Even-split launches (every tile cut into `split` k-ranges owned by `split` consecutive CTAs): the factor, or 0.
 int gemm_even_split(int T, int N, int K, int num_sms) {
-  const int BT = gemm_pick_bt(T), BN = gemm_bn(T);
-  const int n_tiles = (N + BN - 1) / BN, t_tiles = (T + BT - 1) / BT, KB = (K + GEMM_BK - 1) / GEMM_BK;
+  const int BT = gemm_pick_bt(T);
+  const int n_tiles = (N + GEMM_BN - 1) / GEMM_BN, t_tiles = (T + BT - 1) / BT, KB = (K + GEMM_BK - 1) / GEMM_BK;
   const long long tiles = (long long)n_tiles * t_tiles;
   if (t_tiles != 1 || tiles > num_sms / 2) return 0;
   const int grid = gemm_grid_size(T, N, K, num_sms);
@@ -1027,32 +762,21 @@ int gemm_even_split(int T, int N, int K, int num_sms) {
   return (split >= 2 && KB >= split) ? split : 0;
 }
 
-GemmNext gemm_next_desc(int T_next, int N_next, int K_next, int num_sms, int kb_prefetch) {
-  GemmNext n{};
-  const int BT = gemm_pick_bt(T_next);
-  if ((T_next + BT - 1) / BT != 1) return n;  // only decode-shaped successors (one token tile) are prefetched
-  n.n_tiles = (N_next + gemm_bn(T_next) - 1) / gemm_bn(T_next);
-  n.KB = (K_next + GEMM_BK - 1) / GEMM_BK;
-  n.grid = gemm_grid_size(T_next, N_next, K_next, num_sms);
-  n.kb_prefetch = kb_prefetch;
-  return n;
-}
-
 // cluster mode: on-chip split-K reduction when every tile is split evenly over <= 8 consecutive CTAs, the fp32 partial
-// fits the drained ring, and all clusters can be co-resident (checked once per (BT, NW, split, grid)).  Returns the
-// split or 0.
-template <int BT, int NW>
+// fits the drained ring, and all clusters can be co-resident (checked once per (BT, split, grid)).  Returns the split
+// or 0.
+template <int BT>
 static int cluster_split_bt(int T, int N, int K, int num_sms) {
-  using Cfg = GemmCfg<BT, NW>;
+  using Cfg = GemmCfg<BT>;
   static int cluster_ok[9][160];  // [split][grid / split]: 0 unknown, 1 yes, -1 no
-  int split = gemm_cluster_enabled() ? gemm_even_split(T, N, K, num_sms) : 0;
+  int split = gemm_even_split(T, N, K, num_sms);
   if (split > 8 || (size_t)Cfg::PART_FLOATS * sizeof(float) > (size_t)Cfg::STAGES * Cfg::STAGE_BYTES) split = 0;
   if (split == 0) return 0;
   const int grid = gemm_grid_size(T, N, K, num_sms);
   const int nc = grid / split;
   if (nc >= 160) return 0;
   if (cluster_ok[split][nc] == 0) {
-    gemm_set_attrs<BT, NW, false>();
+    gemm_set_attrs<BT, false>();
     cudaLaunchConfig_t qc{};
     qc.gridDim = dim3(split * (num_sms / split));
     qc.blockDim = dim3(GEMM_THREADS);
@@ -1065,130 +789,86 @@ static int cluster_split_bt(int T, int N, int K, int num_sms) {
     qc.attrs = qa;
     qc.numAttrs = 1;
     int n_clusters = 0;
-    const cudaError_t qe = cudaOccupancyMaxActiveClusters(&n_clusters, gemm_bf16_wgmma_kernel<BT, NW, false>, &qc);
+    const cudaError_t qe = cudaOccupancyMaxActiveClusters(&n_clusters, gemm_bf16_wgmma_kernel<BT, false>, &qc);
     // All clusters of the launch must be co-resident: a GPC only hosts floor(SMs / split) of them, and one cluster left
     // over for a second wave doubles the launch time.
     cluster_ok[split][nc] = (qe == cudaSuccess && n_clusters >= nc) ? 1 : -1;
     if (getenv("TGIS_GEMM_DEBUG"))
-      fprintf(stderr, "[gemm] BT=%d NW=%d split=%d: %d clusters fit, grid %d -> cluster mode %s\n", BT, NW, split,
-              n_clusters, grid, cluster_ok[split][nc] == 1 ? "on" : "off");
+      fprintf(stderr, "[gemm] BT=%d split=%d: %d clusters fit, grid %d -> cluster mode %s\n", BT, split, n_clusters, grid,
+              cluster_ok[split][nc] == 1 ? "on" : "off");
     if (qe != cudaSuccess) cudaGetLastError();
   }
   return cluster_ok[split][nc] == 1 ? split : 0;
-}
-
-template <int BT>
-static int cluster_split_nw(int T, int N, int K, int num_sms) {
-  return gemm_nw(T) == 2 ? cluster_split_bt<BT, 2>(T, N, K, num_sms) : cluster_split_bt<BT, 1>(T, N, K, num_sms);
 }
 
 // The split factor gemm_bf16_launch will run this shape with in cluster mode (0: global-memory fix-up) -- callers that
 // want the fused RoPE epilogue ask first.
 int gemm_cluster_split(int T, int N, int K, int num_sms) {
   switch (gemm_pick_bt(T)) {
-    case 16: return cluster_split_nw<16>(T, N, K, num_sms);
-    case 32: return cluster_split_nw<32>(T, N, K, num_sms);
-    case 64: return cluster_split_nw<64>(T, N, K, num_sms);
-    case 128: return cluster_split_nw<128>(T, N, K, num_sms);
-    default: return cluster_split_nw<256>(T, N, K, num_sms);
+    case 16: return cluster_split_bt<16>(T, N, K, num_sms);
+    case 32: return cluster_split_bt<32>(T, N, K, num_sms);
+    case 64: return cluster_split_bt<64>(T, N, K, num_sms);
+    case 128: return cluster_split_bt<128>(T, N, K, num_sms);
+    default: return cluster_split_bt<256>(T, N, K, num_sms);
   }
 }
 
-template <int BT, int NW>
+template <int BT>
 static cudaError_t launch_bt(const CUtensorMap& wmap, const CUtensorMap& xmap, void* Y, int ldy, int T, int N, int K,
                              float* ws, int* counters, int num_sms, int out_f32, cudaStream_t stream,
-                             const CUtensorMap& next_wmap, const GemmNext& nxt, const GemmRope& rope, const GemmNorm& norm,
-                             bool lean) {
-  using Cfg = GemmCfg<BT, NW>;
+                             const GemmRope& rope, bool lean) {
   const int t_tiles = (T + BT - 1) / BT;
   const int grid = gemm_grid_size(T, N, K, num_sms);
-  // bit 0: weights are read once (evict-first); bit 1: stream-K share before the whole tiles (GemmSched::sk_first;
-  // TGIS_GEMM_SK_FIRST=0: pure stream-K as in round 1).  The fused-norm consumer's transform warps assume the pure cut.
+  // bit 0: weights are read once (evict-first); bit 1: stream-K share before the whole tiles (GemmSched::sk_first).
   // Token tiles above 64 rows keep the pure cut: there the whole tile's direct epilogue (128+ tokens per row) is a
   // longer tail than the fix-up it replaces.
-  static int sk_first_env = -1;
-  if (sk_first_env < 0) {
-    const char* e = getenv("TGIS_GEMM_SK_FIRST");
-    sk_first_env = (e && e[0] == '0') ? 0 : 1;
-  }
-  int stream_weights = (t_tiles == 1) ? (1 | ((sk_first_env && norm.h == nullptr && BT <= 64) ? 2 : 0)) : 0;
-  const int split = cluster_split_bt<BT, NW>(T, N, K, num_sms);
-  // bit 2: push variant of the cluster reduction (receive buffer of (BT + 8) x 128 floats behind the ring; token tiles of
-  // at most 32 rows, where it fits next to the full ring).  TGIS_GEMM_CLUSTER_PUSH=1 enables it (default: pull variant).
-  static int push_env = -1;
-  if (push_env < 0) {
-    const char* e = getenv("TGIS_GEMM_CLUSTER_PUSH");
-    push_env = (e && e[0] == '1') ? 1 : 0;
-  }
-  const bool push = push_env && split > 0 && BT <= 32 && NW == 1 && norm.h == nullptr;
-  if (push) stream_weights |= 4;
+  const int stream_weights = (t_tiles == 1) ? (1 | (BT <= 64 ? 2 : 0)) : 0;
+  const int split = cluster_split_bt<BT>(T, N, K, num_sms);
   // the fused RoPE epilogue lives in the two split-tile reductions (cluster and global fix-up): every tile must be split
   if (rope.positions != nullptr && (gemm_even_split(T, N, K, num_sms) < 2 || out_f32 != 0 ||
                                     N != (rope.n_q + 2 * rope.n_kv) * HEAD_DIM))
     return cudaErrorInvalidValue;
-  // fused residual add / RMSNorm (GemmNorm): the producer side lives in the cluster reduction only, the consumer side in
-  // decode-shaped launches with a token tile of at most 64 rows
-  if (norm.sumsq_out != nullptr && (split == 0 || out_f32 != 0 || rope.positions != nullptr || N % GEMM_BN != 0 ||
-                                    norm.residual == nullptr || ldy != N))
-    return cudaErrorInvalidValue;
-  const size_t smem_bytes = (size_t)Cfg::SMEM_BYTES + (norm.h != nullptr ? (size_t)K * 2 : 0) +
-                            (push ? (size_t)(BT + 8) * GEMM_BN * 4 : 0);
-  if (norm.h != nullptr && (t_tiles != 1 || BT > GEMM_NORM_MAX_T || K % GEMM_BK != 0 || NW != 1 || norm.n_parts <= 0 || norm.n_parts > GEMM_NORM_MAX_PARTS ||
-                            smem_bytes > (size_t)Cfg::SMEM_MAX))
-    return cudaErrorInvalidValue;
-  const int threads = norm.h != nullptr ? GEMM_THREADS_NORM : GEMM_THREADS;
-  // decode token tiles without the fused-norm roles or the push receive buffer run lean (GemmCfg): same tiles, split
-  // points and reduction order, a shorter ring and room for the next launch's CTA on every SM
-  auto kernel = gemm_bf16_wgmma_kernel<BT, NW, false>;
-  size_t smem = smem_bytes;
-  cudaError_t e = gemm_set_attrs<BT, NW, false>();
-  if constexpr (BT <= GEMM_LEAN_MAX_T && NW == 1) {
-    if (lean && norm.h == nullptr && norm.sumsq_out == nullptr && !push) {
-      kernel = gemm_bf16_wgmma_kernel<BT, NW, true>;
-      smem = GemmCfg<BT, NW, true>::SMEM_BYTES;
-      e = gemm_set_attrs<BT, NW, true>();
+  // decode token tiles run lean (GemmCfg): same tiles, split points and reduction order, a shorter ring and room for the
+  // next launch's CTA on every SM
+  auto kernel = gemm_bf16_wgmma_kernel<BT, false>;
+  size_t smem = GemmCfg<BT>::SMEM_BYTES;
+  cudaError_t e = gemm_set_attrs<BT, false>();
+  if constexpr (BT <= GEMM_LEAN_MAX_T) {
+    if (lean) {
+      kernel = gemm_bf16_wgmma_kernel<BT, true>;
+      smem = GemmCfg<BT, true>::SMEM_BYTES;
+      e = gemm_set_attrs<BT, true>();
     }
   }
   if (e != cudaSuccess) return e;
   if (split > 0)
-    return launch_k_cluster(kernel, dim3(grid), dim3(threads), smem, stream, split, wmap, xmap, Y, ldy, T, N, K, ws,
-                            counters, stream_weights, out_f32, next_wmap, nxt, split, rope, norm);
-  return launch_k(kernel, dim3(grid), dim3(threads), smem, stream, wmap, xmap, Y, ldy, T, N, K, ws, counters,
-                  stream_weights, out_f32, next_wmap, nxt, 0, rope, norm);
+    return launch_k_cluster(kernel, dim3(grid), dim3(GEMM_THREADS), smem, stream, split, wmap, xmap, Y, ldy, T, N, K, ws,
+                            counters, stream_weights, out_f32, split, rope);
+  return launch_k(kernel, dim3(grid), dim3(GEMM_THREADS), smem, stream, wmap, xmap, Y, ldy, T, N, K, ws, counters,
+                  stream_weights, out_f32, 0, rope);
 }
 
 // xmap must have been built with box_rows == gemm_pick_bt(T)
 cudaError_t gemm_bf16_launch(const CUtensorMap& wmap, const CUtensorMap& xmap, void* Y, int ldy, int T, int N, int K,
                              float* ws, int* counters, int num_sms, cudaStream_t stream, int out_f32,
-                             const CUtensorMap* next_wmap, const GemmNext* next, const GemmRope* rope, const GemmNorm* norm,
-                             bool lean) {
+                             const GemmRope* rope, bool lean) {
   GemmRope rp{};
   if (rope) rp = *rope;
-  GemmNorm nr{};
-  if (norm) nr = *norm;
-  GemmNext nx{};
-  if (next && next_wmap) nx = *next;
-  const CUtensorMap& nm = (next && next_wmap) ? *next_wmap : wmap;
-  const int nw = gemm_nw(T);
-#define TGIS_GEMM_CASE(B)                                                                                              \
-  return nw == 2 ? launch_bt<B, 2>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, nm, nx, rp, nr, lean) \
-                 : launch_bt<B, 1>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, nm, nx, rp, nr, lean)
   switch (gemm_pick_bt(T)) {
-    case 16: TGIS_GEMM_CASE(16);
-    case 32: TGIS_GEMM_CASE(32);
-    case 64: TGIS_GEMM_CASE(64);
-    case 128: TGIS_GEMM_CASE(128);
-    default: TGIS_GEMM_CASE(256);
+    case 16: return launch_bt<16>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, rp, lean);
+    case 32: return launch_bt<32>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, rp, lean);
+    case 64: return launch_bt<64>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, rp, lean);
+    case 128: return launch_bt<128>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, rp, lean);
+    default: return launch_bt<256>(wmap, xmap, Y, ldy, T, N, K, ws, counters, num_sms, out_f32, stream, rp, lean);
   }
-#undef TGIS_GEMM_CASE
 }
 
 template <int BT, bool LEAN>
 static int blocks_per_sm_bt() {
-  if (gemm_set_attrs<BT, 1, LEAN>() != cudaSuccess) return -1;
+  if (gemm_set_attrs<BT, LEAN>() != cudaSuccess) return -1;
   int n = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, gemm_bf16_wgmma_kernel<BT, 1, LEAN>, GEMM_THREADS,
-                                                    GemmCfg<BT, 1, LEAN>::SMEM_BYTES) != cudaSuccess)
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, gemm_bf16_wgmma_kernel<BT, LEAN>, GEMM_THREADS,
+                                                    GemmCfg<BT, LEAN>::SMEM_BYTES) != cudaSuccess)
     return -1;
   return n;
 }

@@ -13,7 +13,6 @@ namespace tgis {
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                       uint32_t box_rows, uint32_t box_cols);
 int gemm_pick_bt(int T);
-int gemm_nw(int T);  // weight tiles (128 rows each) per unit sharing one activation tile: 2 for decode-shaped launches
 size_t gemm_workspace_bytes(int num_sms);
 int gemm_timeline_read(unsigned long long* out64);  // debug builds (-DTGIS_GEMM_TIMELINE) only
 // -DTGIS_STEP_TIMELINE builds: point every translation unit's kernels at the timeline buffer (ptx.cuh); else -2
@@ -21,14 +20,8 @@ int gemm_set_step_timeline(unsigned long long* buf);
 int elementwise_set_step_timeline(unsigned long long* buf);
 int attention_set_step_timeline(unsigned long long* buf);
 int sampler_set_step_timeline(unsigned long long* buf);
-// Decode-shaped successor of a GEMM launch: lets the running kernel pull the first `kb_prefetch` weight boxes of every
-// CTA of the NEXT GEMM into L2 while its own tail drains (kb_prefetch == 0: off).
-struct GemmNext {
-  int n_tiles, KB, grid, kb_prefetch;
-};
 int gemm_grid_size(int T, int N, int K, int num_sms);
 int gemm_even_split(int T, int N, int K, int num_sms);  // every tile cut over this many consecutive CTAs, or 0
-GemmNext gemm_next_desc(int T_next, int N_next, int K_next, int num_sms, int kb_prefetch);
 // Y: bf16 [T, ldy] (out_f32 = 0), fp32 [T, ldy] (out_f32 = 1, lm_head logits), or out_f32 = 2: fused SwiGLU — W rows are
 // interleaved (gate_j, up_j) pairs and Y is bf16 [T, ldy >= N/2] = bf16(bf16(silu(gate)) * up)
 // Optional fused epilogue of the qkv projection (cluster mode only, gemm_cluster_split() > 0): RoPE on the q / k heads
@@ -41,31 +34,10 @@ struct GemmRope {
   __nv_bfloat16* v_cache;
   int32_t n_q, n_kv;
 };
-// Optional fusion of the layer stack's  residual add + RMSNorm  (vllm layernorm.py fused_add_rms_norm; same rounding
-// points as add_rmsnorm_launch) into the two GEMMs either side of it, decode-shaped launches only (one token tile,
-// T <= 64):
-//  * producer (o / down projection, cluster mode required): the split-tile reduction does not write Y; it computes
-//    h = bf16(bf16(acc) + residual), stores h back to `residual` [T, N] and the tile's sum of h^2 to
-//    sumsq_out[t * (N / 128) + tile]  (N % 128 == 0);
-//  * consumer (qkv / gate_up projection): the activation operand is not loaded by TMA; two extra warps build
-//    bf16(bf16(h * rstd) * w_norm) straight into the swizzled shared-memory stage, rstd[t] from the n_parts partial sums
-//    added in tile order (deterministic).  K % 64 == 0.
-struct GemmNorm {
-  __nv_bfloat16* residual;       // producer: in/out [T, N]; nullptr = off
-  float* sumsq_out;              // producer: [T][N / 128]
-  const __nv_bfloat16* h;        // consumer: [T, K]; nullptr = off
-  const float* sumsq_in;         // consumer: [T][n_parts]
-  const __nv_bfloat16* w_norm;   // consumer: [K]
-  int32_t n_parts;
-  float eps;
-};
-constexpr int GEMM_NORM_MAX_T = 64;
-constexpr int GEMM_NORM_MAX_PARTS = 64;  // hidden <= 8192
 int gemm_cluster_split(int T, int N, int K, int num_sms);
 cudaError_t gemm_bf16_launch(const CUtensorMap& wmap, const CUtensorMap& xmap, void* Y, int ldy, int T, int N, int K,
                              float* ws, int* counters, int num_sms, cudaStream_t stream, int out_f32 = 0,
-                             const CUtensorMap* next_wmap = nullptr, const GemmNext* next = nullptr,
-                             const GemmRope* rope = nullptr, const GemmNorm* norm = nullptr, bool lean = true);
+                             const GemmRope* rope = nullptr, bool lean = true);
 // CTAs per SM of the instantiation a T-token launch runs (the lean decode one when `lean` and T <= 32; gemm_wgmma.cu),
 // or -1 when the occupancy query fails
 int gemm_blocks_per_sm(int T, bool lean);
@@ -230,9 +202,7 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
                                const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits, float* part_o,
                                float* part_ml, __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                               int num_sms, cudaStream_t stream, int* arrive = nullptr);
-// arrive: [n_seqs * n_kv] ints, zero before the first launch (re-armed by the kernel): with it, the split merge runs inside
-// the streaming kernel (last-arriving warp per (sequence, kv head)) and attn_merge_kernel is not launched.
+                               int num_sms, cudaStream_t stream);
 // Prefill / chunked prefill (q_len >= 1), causal over the paged cache.
 cudaError_t attn_prefill_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
                                 const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,

@@ -108,7 +108,7 @@ int tgis_k_gemm(const void* x_dev, const void* w_dev, void* y_dev, int32_t T, in
     KCK(cudaEventRecord(e0, st));
     for (int i = 0; i < iters; ++i)
       KCK(gemm_bf16_launch(wm, xm, y_dev, out_f32 == 2 ? N / 2 : N, T, N, K, ws.p, ctr.p, sms, st, out_f32, nullptr,
-                           nullptr, nullptr, nullptr, /*lean=*/impl != 2));
+                           /*lean=*/impl != 2));
     KCK(cudaEventRecord(e1, st));
     KCK(cudaStreamSynchronize(st));
   }
@@ -208,72 +208,8 @@ int tgis_k_gemm_rope(const void* x_dev, const void* w_dev, void* y_dev, int32_t 
   KCK(pos.upload(positions_host, T));
   KCK(sm.upload(slot_mapping_host, T));
   const GemmRope rp{pos.p, sm.p, (const bf16*)cos_sin_dev, (bf16*)k_cache_dev, (bf16*)v_cache_dev, n_q, n_kv};
-  KCK(gemm_bf16_launch(wm, xm, y_dev, N, T, N, K, ws.p, ctr.p, sms, 0, 0, nullptr, nullptr, &rp));
+  KCK(gemm_bf16_launch(wm, xm, y_dev, N, T, N, K, ws.p, ctr.p, sms, 0, 0, &rp));
   KCK(cudaDeviceSynchronize());
-  return 0;
-}
-
-// Layer-stack slice  a -> [GEMM W1] -> (+ residual, RMSNorm w_norm) -> [GEMM W2 (out_mode2: 0 bf16, 2 fused SwiGLU)] -> y2
-// run either as three launches (fused = 0: gemm, add_rmsnorm_launch, gemm) or as two with the add + norm folded into the
-// two GEMMs (fused = 1, GemmNorm).  residual [T, H] is updated in place either way.  Returns 1 when the launch plan cannot
-// fuse this shape (nothing computed).  iters > 1 times the chain (residual keeps accumulating: timing only).
-int tgis_k_gemm_norm_chain(const void* a_dev, int32_t a_rows_alloc, const void* w1_dev, void* residual_dev,
-                           const void* w_norm_dev, const void* w2_dev, void* y2_dev, int32_t T, int32_t K1, int32_t H,
-                           int32_t N2, float eps, int32_t out_mode2, int32_t fused, int32_t iters, float* us_out) {
-  const int sms = test_num_sms();
-  const int bt = gemm_pick_bt(T);
-  if (fused && (T > GEMM_NORM_MAX_T || gemm_cluster_split(T, H, K1, sms) == 0 || H % 128 != 0)) return 1;
-  if (a_rows_alloc < bt) return kfail("a must have at least one TMA box of rows allocated");
-  Tmp<bf16> y1, xn;
-  Tmp<float> ssq, ws;
-  Tmp<int> ctr;
-  const int rows = T > bt ? T : bt;
-  KCK(y1.alloc((size_t)rows * H));
-  KCK(xn.alloc((size_t)rows * H));
-  KCK(cudaMemset(xn.p, 0, (size_t)rows * H * sizeof(bf16)));
-  KCK(ssq.alloc((size_t)rows * (H / 128 + 1)));
-  KCK(ws.alloc(gemm_workspace_bytes(sms) / sizeof(float)));
-  KCK(ctr.alloc(1 << 16));
-  KCK(cudaMemset(ctr.p, 0, sizeof(int) << 16));
-  CUtensorMap wm1, am, wm2, xm;
-  if (make_tmap_bf16_2d(&wm1, w1_dev, H, K1, K1, 128, 64) != 0) return kfail("w1 tensor map failed");
-  if (make_tmap_bf16_2d(&am, a_dev, a_rows_alloc, K1, K1, bt, 64) != 0) return kfail("a tensor map failed");
-  if (make_tmap_bf16_2d(&wm2, w2_dev, N2, H, H, 128, 64) != 0) return kfail("w2 tensor map failed");
-  // the fused consumer stages the raw residual stream by TMA and normalises it in shared memory
-  if (make_tmap_bf16_2d(&xm, fused ? residual_dev : (void*)xn.p, fused ? a_rows_alloc : rows, H, H, bt, 64) != 0)
-    return kfail("xn tensor map failed");
-  const int ldy2 = out_mode2 == 2 ? N2 / 2 : N2;
-  cudaEvent_t e0, e1;
-  KCK(cudaEventCreate(&e0));
-  KCK(cudaEventCreate(&e1));
-  if (iters < 1) iters = 1;
-  KCK(cudaEventRecord(e0, 0));
-  for (int i = 0; i < iters; ++i) {
-    if (fused) {
-      GemmNorm prod{};
-      prod.residual = (bf16*)residual_dev;
-      prod.sumsq_out = ssq.p;
-      KCK(gemm_bf16_launch(wm1, am, y1.p, H, T, H, K1, ws.p, ctr.p, sms, 0, 0, nullptr, nullptr, nullptr, &prod));
-      GemmNorm cons{};
-      cons.h = (const bf16*)residual_dev;
-      cons.sumsq_in = ssq.p;
-      cons.w_norm = (const bf16*)w_norm_dev;
-      cons.n_parts = H / 128;
-      cons.eps = eps;
-      KCK(gemm_bf16_launch(wm2, xm, y2_dev, ldy2, T, N2, H, ws.p, ctr.p, sms, 0, out_mode2, nullptr, nullptr, nullptr, &cons));
-    } else {
-      KCK(gemm_bf16_launch(wm1, am, y1.p, H, T, H, K1, ws.p, ctr.p, sms, 0, 0));
-      KCK(add_rmsnorm_launch(y1.p, (bf16*)residual_dev, (const bf16*)w_norm_dev, xn.p, T, H, eps, 0));
-      KCK(gemm_bf16_launch(wm2, xm, y2_dev, ldy2, T, N2, H, ws.p, ctr.p, sms, 0, out_mode2));
-    }
-  }
-  KCK(cudaEventRecord(e1, 0));
-  KCK(cudaDeviceSynchronize());
-  float ms = 0.f;
-  KCK(cudaEventElapsedTime(&ms, e0, e1));
-  if (us_out) *us_out = ms * 1000.f / iters;
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
   return 0;
 }
 
@@ -287,7 +223,6 @@ struct AttnCall {
   Tmp<int32_t> dec, tseq, tq0, bt;
   Tmp<float> po, pml;
   Tmp<DecItem> items;
-  Tmp<int> arrive;  // arrival counters of the in-kernel split merge (the launcher ignores them when that path is off)
 
   // split_mode: 0 every prefill tile on the existing kernel, 1 every one on the split-context kernel, 2 the engine's
   // selection (prefill_split_pick); split-context tiles are listed last, as in the engine's step
@@ -332,8 +267,6 @@ struct AttnCall {
     std::vector<DecItem> h_items(1 + nd * max_splits);
     decode_items_build(h_items.data(), h_seqs.data(), h_dec.data(), n_dec, block_table_host, bt_stride);
     KCK(items.upload(h_items.data(), h_items.size()));
-    KCK(arrive.alloc(nd * n_kv));
-    KCK(cudaMemset(arrive.p, 0, sizeof(int) * nd * n_kv));
     return 0;
   }
   // decode (+ split merge), then prefill, then split-context prefill: the engine's order
@@ -343,7 +276,7 @@ struct AttnCall {
     if (decode)
       KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, items.p,
                              n_dec * max_splits, seqs.p, dec.p, n_dec, max_splits, po.p, pml.p, (bf16*)out_dev, out_ld,
-                             n_q, n_kv, scale, test_num_sms(), st, arrive.p));
+                             n_q, n_kv, scale, test_num_sms(), st));
     const int n_std = n_tiles - n_ctiles;
     KCK(attn_prefill_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, seqs.p,
                             tseq.p, tq0.p, n_std, bt.p, bt_stride, (bf16*)out_dev, out_ld, n_q, n_kv, scale, st));
@@ -443,7 +376,7 @@ int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, 
   cudaError_t e;
   if (writer == 1) {
     const GemmRope rp{pos.p, sm.p, (const bf16*)cos_sin_dev, (bf16*)k_cache_dev, (bf16*)v_cache_dev, n_q, n_kv};
-    e = gemm_bf16_launch(wm, xm, qkv_dev, N, T, N, K, ws.p, ctr.p, sms, st, 0, nullptr, nullptr, &rp);
+    e = gemm_bf16_launch(wm, xm, qkv_dev, N, T, N, K, ws.p, ctr.p, sms, st, 0, &rp);
   } else {
     e = rope_kvwrite_launch((bf16*)qkv_dev, pos.p, sm.p, (const bf16*)cos_sin_dev, (bf16*)k_cache_dev,
                             (bf16*)v_cache_dev, T, n_q, n_kv, st);
@@ -486,9 +419,6 @@ int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const v
   Tmp<DecItem> d_items;
   KCK(d_items.upload(items.data(), items.size()));
   const int num_sms = test_num_sms();
-  Tmp<int> arrive;
-  KCK(arrive.alloc((size_t)n_seqs * n_kv));
-  KCK(cudaMemset(arrive.p, 0, sizeof(int) * (size_t)n_seqs * n_kv));
   cudaEvent_t e0, e1;
   KCK(cudaEventCreate(&e0));
   KCK(cudaEventCreate(&e1));
@@ -499,7 +429,7 @@ int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const v
     const char* vc = (const char*)v_cache_dev + (size_t)l * layer_stride_bytes;
     KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)kc, (const bf16*)vc, d_items.p,
                            n_seqs * max_splits, d_seqs.p, nullptr, n_seqs, max_splits, po.p, pml.p, (bf16*)out_dev,
-                           out_ld, n_q, n_kv, scale, num_sms, 0, arrive.p));
+                           out_ld, n_q, n_kv, scale, num_sms, 0));
   }
   KCK(cudaEventRecord(e1, 0));
   KCK(cudaDeviceSynchronize());
@@ -528,9 +458,6 @@ int tgis_k_gemm_blocks_per_sm(int32_t T, int32_t lean, int32_t* out) {
   *out = gemm_blocks_per_sm(T, lean != 0);
   return *out > 0 ? 0 : kfail("occupancy query failed");
 }
-
-// weight rows per GEMM unit (128 x the number of weight tiles that share one activation tile) for a T-token launch
-int tgis_k_gemm_unit_rows(int32_t T) { return 128 * gemm_nw(T); }
 
 // Host-only: the decode work-item list the scheduler builds for a step (no GPU needed).  seqs_host as in
 // tgis_k_attention (all decode sequences); items_out: (1 + capacity) x 8 int32 records; returns the entry count or -1.
