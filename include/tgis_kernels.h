@@ -83,6 +83,20 @@ int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, 
 /* host-only: GEMM launch plan for a shape: token tile (16..256), grid, even-split factor (0: stream-K + global fix-up) */
 int tgis_k_gemm_plan(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* bt_out, int32_t* grid_out,
                      int32_t* even_split_out);
+/* host-only: the GEMM's work schedule for a shape, from the code the kernel runs.
+ * info_out[12]: bt, grid, even-split factor, cluster split (0 without a device), weight tiles, token tiles, k-blocks per
+ *   tile, whole-tile waves, CTAs taking one more whole tile, sk_first, first stream-K tile, stream-K units.
+ * units_out: unit_cap x {cta, tile, kb0, kb1, slot}, each CTA's units in the order it runs them (tile = linear tile index;
+ *   k-blocks [kb0, kb1); slot = the workspace slot of a partial unit).
+ * splits_out: split_cap x {tile, first contributor, CTAs owning units in the tile, arrivals the fix-up waits for}, one per
+ *   split tile in tile order.  reads_out: read_cap x {tile, cta, slot}, the partials the fix-up sums, in summation order. */
+int tgis_k_gemm_schedule(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* info_out, int32_t* units_out,
+                         int32_t unit_cap, int32_t* n_units_out, int32_t* splits_out, int32_t split_cap,
+                         int32_t* n_splits_out, int32_t* reads_out, int32_t read_cap, int32_t* n_reads_out);
+/* GEMMs back to back on one stream as the engine's step launches them (PDL, the lean decode instantiation, one workspace
+ * and one counter array zeroed once).  desc_host: n x {T, N, K, ldx, x_rows_alloc, ldy, out_f32 (0 bf16, 1 fp32,
+ * 2 SwiGLU)}; ptrs_host: n x {x_dev, w_dev, y_dev}.  *counters_left_out = counters not back at 0 at the end. */
+int tgis_k_gemm_chain(int32_t n, const int32_t* desc_host, const uint64_t* ptrs_host, int32_t* counters_left_out);
 /* CTAs per SM of the GEMM instantiation a T-token launch runs (lean = 0: the one-CTA-per-SM instantiation) */
 int tgis_k_gemm_blocks_per_sm(int32_t T, int32_t lean, int32_t* out);
 /* host-only: the decode work-item list of a step (csrc/kernels.h DecItem: q_row, kv_len, seq | split << 16, 0,

@@ -94,11 +94,12 @@ def test_decode_work_items_host_logic():
 
 
 def test_gemm_launch_plan_host_logic_with_128_row_units():
-    """Pure host arithmetic of the GEMM launcher (gemm_wgmma.cu): for the decode shapes of the 8B and 70B/TP8 layer
-    stacks the plan must (a) never use more CTAs than SMs (the stream-K fix-up and the chain kernel rely on co-residency),
-    (b) in even-split mode give every CTA a k-range inside ONE tile (the cluster epilogue reduces exactly one unit per
-    CTA), and (c) cover the (tile, k-block) space exactly once.  132 SMs = H100 SXM; 148 keeps a second SM count in play
-    (the split factors of qkv / o / down differ between the two)."""
+    """tgis_k_gemm_plan for the decode shapes (T <= 256, one token tile) of the 8B and 70B/TP8 layer stacks: (a) never
+    more CTAs than SMs, and (b) in even-split mode, contiguous cuts of the tile-major (tile, k-block) space into `grid`
+    ranges put every CTA's range inside ONE tile, cta // split (the cluster epilogue reduces exactly one unit per CTA).
+    This restates the cut of decode-shaped launches only (no whole-tile waves, no sk_first); the schedule the kernel
+    runs, in every regime and at prefill sizes, is checked in tests/test_gemm_schedule_cpu.py.  132 SMs = H100 SXM; 148
+    keeps a second SM count in play (the split factors of qkv / o / down differ between the two)."""
     lib = _lib.load_library()
     shapes = [(6144, 4096), (4096, 4096), (28672, 4096), (4096, 14336), (128256, 4096),      # Llama-3-8B
               (1280, 8192), (8192, 1024), (7168, 8192), (8192, 3584)]                        # 70B / TP8 shards

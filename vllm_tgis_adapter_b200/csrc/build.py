@@ -17,7 +17,7 @@ LIB_DIR = PKG / "lib"
 OBJ_DIR = CSRC / "build"
 LIB_PATH = LIB_DIR / "libtgis_engine.so"
 SOURCES = ["gemm_wgmma.cu", "gemm_ref.cu", "elementwise.cu", "attention.cu", "sampler.cu", "lora.cu", "opt.cu", "engine.cu", "test_api.cu"]
-HEADERS = ["ptx.cuh", "launch.cuh", "kernels.h", "../../include/tgis_engine.h", "../../include/tgis_kernels.h"]
+HEADERS = ["ptx.cuh", "launch.cuh", "gemm_sched.cuh", "kernels.h", "../../include/tgis_engine.h", "../../include/tgis_kernels.h"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     *ARCH,

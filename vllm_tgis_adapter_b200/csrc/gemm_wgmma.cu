@@ -23,6 +23,7 @@
 //    global-memory fix-up: bit-identical) and writes the final rows.
 #include <string.h>
 
+#include "gemm_sched.cuh"
 #include "kernels.h"
 #include "launch.cuh"
 #include "ptx.cuh"
@@ -68,89 +69,6 @@ struct GemmCfg {
   static_assert(!LEAN || 2 * (SMEM_BYTES + 1024) <= 228 * 1024, "two lean CTAs must fit one SM's shared memory");
   static_assert(!LEAN || PART_FLOATS * 4 <= STAGES * STAGE_BYTES, "the cluster reduction parks a partial in the ring");
 };
-
-// Prefill-shaped launches (more than one token tile): "data-parallel waves + stream-K tail".  Linear tile index i
-// (see tile_decode) -> the first dp_waves * ncta tiles are whole tiles dealt round-robin, wave w = tiles
-// [w * ncta, (w+1) * ncta): at any moment the ncta CTAs work on ONE compact 8 x (ncta / 8) rectangle of (weight tile, token
-// tile) pairs, so both operands of a wave stay in L2 (with contiguous per-CTA ranges the CTAs drift apart, the working
-// set is every weight tile + every activation tile, far more than L2 holds).  The remaining < ncta tiles are cut
-// stream-K style.  Decode-shaped launches have dp_waves = 0.
-//
-// Decode-shaped launches with at least one tile per CTA (gate_up: 224 tiles, lm_head: 1002) use the same two
-// regions in the OPPOSITE order ("sk_first"): every CTA first works through its < 1 tile share of the stream-K region --
-// the shared tiles, whose last-arriver fix-up (atomic + L2 round trip + ordered sum) then runs in the epilogue warps
-// UNDER the main loop of the following whole tile -- and ends on a whole tile with a direct epilogue.  With the pure
-// stream-K cut most CTAs END on a shared tile piece, and the fix-ups (4-6.5 us at 32 tokens, growing with T) are the
-// launch's tail.  Same tiles, same split points inside a shared tile's k-range order, same rank-ordered sums.
-struct GemmSched {
-  int n_tiles, t_tiles, KB, ncta;
-  int dp_waves;        // whole-tile waves
-  int sk_tile0;        // first tile of the stream-K region
-  long long sk_total;  // (tile, k-block) units in the stream-K region
-  bool sk_first;       // stream-K region before the whole-tile waves
-  __device__ GemmSched(int n_tiles_, int t_tiles_, int KB_, int ncta_, bool sk_first_)
-      : n_tiles(n_tiles_), t_tiles(t_tiles_), KB(KB_), ncta(ncta_) {
-    const int tiles = n_tiles * t_tiles;
-    sk_first = sk_first_ && t_tiles == 1 && tiles >= ncta;
-    dp_waves = (t_tiles > 1 || sk_first) ? tiles / ncta : 0;
-    sk_tile0 = dp_waves * ncta;
-    sk_total = (long long)(tiles - sk_tile0) * KB;
-  }
-};
-// linear tile index -> (weight tile, token tile).  One token tile: identity.  Otherwise blocks of 8 weight tiles, token
-// tile next, weight tile fastest: ncta consecutive indices = 8 weight tiles x ncta / 8 token tiles.
-__device__ __forceinline__ void tile_decode(const GemmSched& sc, int tile, int& n_tile, int& t_tile) {
-  if (sc.t_tiles == 1) {
-    n_tile = tile;
-    t_tile = 0;
-    return;
-  }
-  constexpr int NB = 8;
-  const int full = NB * sc.t_tiles;
-  const int nb = tile / full, rem = tile - nb * full;
-  const int nb_n = min(NB, sc.n_tiles - nb * NB);
-  t_tile = rem / nb_n;
-  n_tile = nb * NB + rem - t_tile * nb_n;
-}
-
-struct UnitIter {
-  // whole tiles wave * ncta + cta for wave < dp_waves, then the contiguous range [pos, end) of the stream-K region's
-  // (tile, kblock) space owned by this CTA
-  long long pos, end;
-  int kb_per_tile, wave, dp_waves, cta, ncta, sk_tile0;
-  bool first, sk_first;
-  __device__ UnitIter(const GemmSched& sc, int cta_)
-      : kb_per_tile(sc.KB), wave(0), dp_waves(sc.dp_waves), cta(cta_), ncta(sc.ncta), sk_tile0(sc.sk_tile0), first(true),
-        sk_first(sc.sk_first) {
-    pos = (sc.sk_total * cta_) / sc.ncta;
-    end = (sc.sk_total * (cta_ + 1)) / sc.ncta;
-  }
-  __device__ bool next(int& tile, int& kb0, int& kb1, int& slot) {
-    if (wave < dp_waves && (!sk_first || pos >= end)) {
-      tile = wave * ncta + cta;
-      kb0 = 0;
-      kb1 = kb_per_tile;
-      slot = 0;
-      ++wave;
-      return true;
-    }
-    if (pos >= end) return false;
-    tile = sk_tile0 + (int)(pos / kb_per_tile);
-    kb0 = (int)(pos % kb_per_tile);
-    long long rem = end - pos;
-    int room = kb_per_tile - kb0;
-    int take = rem < room ? (int)rem : room;
-    kb1 = kb0 + take;
-    slot = first ? 0 : 1;
-    first = false;
-    pos += take;
-    return true;
-  }
-};
-
-__device__ __forceinline__ int unit_owner(long long p, long long total, int ncta) {
-  return (int)(((p + 1) * ncta - 1) / total);
-}
 
 #ifdef TGIS_GEMM_TIMELINE
 __device__ unsigned long long g_gemm_timeline[4][16];
@@ -255,7 +173,6 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
   const int ncta = gridDim.x, cta = blockIdx.x;
   const GemmSched sched(n_tiles, t_tiles, KB, ncta, (stream_weights & 2) != 0);
   stream_weights &= 1;
-  const long long total = sched.sk_total;  // stream-K region (== everything for decode-shaped launches)
 
   if (warp == PRODUCER_WARP && elect_one()) {
     tma_prefetch_desc(&wmap);
@@ -273,64 +190,32 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
 
   if (warp == PRODUCER_WARP) {
     // ===================== TMA producer =====================
-    // The CTA's k-blocks are one contiguous range [begin, end) of the global (tile, k-block) space.  Weights are
-    // static, so the first STAGES weight tiles are requested BEFORE the grid-dependency wait: under PDL this
-    // overlaps the previous kernel's tail (and the small kernel in between) with useful HBM traffic.
+    // The CTA's k-blocks, unit by unit in the consumers' order (UnitIter).  Weights are static, so the first STAGES
+    // weight tiles are requested BEFORE the grid-dependency wait: under PDL this overlaps the previous kernel's tail (and
+    // the small kernel in between) with useful HBM traffic.
     if (elect_one()) {
       const uint64_t pol_w = policy_evict_first();
       const uint64_t pol_x = policy_evict_last();
-      const long long begin = (total * cta) / ncta, end = (total * (cta + 1)) / ncta;
-      const int n_kb = sched.dp_waves * KB + (int)(end - begin);
-      // (tile, kb) cursors advanced incrementally: no divisions on the per-k-block issue path.  A cursor walks the
-      // CTA's whole tiles (wave order) and then its stream-K range; rows are re-derived only when the tile changes.
+      // (tile, kb) cursors: rows are re-derived once per unit, the per-k-block issue path only increments
       struct Cur {
-        int wave, tile, kb, w_row, x_row;
-        int sk_left;  // sk_first: k-blocks left in the stream-K share (then the whole-tile waves)
+        UnitIter it;
+        int kb, kb1, w_row, x_row;
       };
-      auto cur_set_tile = [&](Cur& c, int tile) {
-        c.tile = tile;
+      auto cur_unit = [&](Cur& c) {
+        int tile, slot;
+        if (!c.it.next(tile, c.kb, c.kb1, slot)) return;
         int n_tile, t_tile;
         tile_decode(sched, tile, n_tile, t_tile);
         c.w_row = n_tile * GEMM_BN;
         c.x_row = t_tile * BT;
       };
-      auto cur_init = [&](Cur& c) {
-        c.wave = 0;
-        c.sk_left = sched.sk_first ? (int)(end - begin) : 0;
-        if (sched.dp_waves > 0 && c.sk_left == 0) {
-          c.kb = 0;
-          cur_set_tile(c, cta);
-        } else {
-          c.kb = (int)(begin % KB);
-          cur_set_tile(c, sched.sk_tile0 + (int)(begin / KB));
-        }
-      };
       auto cur_next = [&](Cur& c) {
-        if (c.sk_left > 0) {  // sk_first: inside the stream-K share
-          if (--c.sk_left == 0) {  // -> first whole tile
-            c.kb = 0;
-            if (sched.dp_waves > 0) cur_set_tile(c, cta);
-            return;
-          }
-          if (++c.kb == KB) {
-            c.kb = 0;
-            cur_set_tile(c, c.tile + 1);
-          }
-          return;
-        }
-        if (++c.kb < KB) return;
-        c.kb = 0;
-        if (c.wave < sched.dp_waves) {
-          if (++c.wave < sched.dp_waves) {
-            cur_set_tile(c, c.wave * ncta + cta);
-          } else {  // into the stream-K tail
-            c.kb = (int)(begin % KB);
-            cur_set_tile(c, sched.sk_tile0 + (int)(begin / KB));
-          }
-        } else {
-          cur_set_tile(c, c.tile + 1);
-        }
+        if (++c.kb == c.kb1) cur_unit(c);
       };
+      Cur wc{UnitIter(sched, cta), 0, 0, 0, 0};
+      const int n_kb = (int)wc.it.kblocks();
+      cur_unit(wc);
+      Cur xc = wc;
       auto issue_w = [&](const Cur& c, int stage) {
         // one box of 128 rows (rows beyond N are zero-filled by TMA and still counted)
         void* dst = smem_w + stage * Cfg::W_BYTES;
@@ -338,9 +223,6 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
         else tma_load_2d(&wmap, &full_bar[stage], dst, c.kb * GEMM_BK, c.w_row);
       };
       const int n_pre = n_kb < STAGES ? n_kb : STAGES;
-      Cur wc, xc;
-      cur_init(wc);
-      xc = wc;
       for (int i = 0; i < n_pre; ++i) {
         mbar_arrive_expect_tx(&full_bar[i], Cfg::STAGE_BYTES);
         issue_w(wc, i);
@@ -455,9 +337,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
         // stream-K fix-up: last arriver reduces all partials of this tile in CTA order (deterministic)
         // publish: CTA-wide barrier, then ONE acq_rel atomic (cumulative over the barrier) instead of membar.gl
         asm volatile("bar.sync 1, %0;\n" ::"n"(EP_THREADS) : "memory");
-        const long long p0 = (long long)(tile - sched.sk_tile0) * KB;  // position inside the stream-K region
-        const int c_first = unit_owner(p0, total, ncta);
-        const int c_last = unit_owner(p0 + KB - 1, total, ncta);
+        int c_first, c_last;
+        sched.split_owners(tile, c_first, c_last);
         if (ep_tid == 0) {
           int old;
           asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], 1;\n" : "=r"(old) : "l"(counters + tile) : "memory");
@@ -486,9 +367,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_co
               for (int ci = 0; ci < FIX_C; ++ci) {
                 const int c = c0g + ci;
                 const bool cv = c <= c_last;
-                const long long cb = cv ? (total * c) / ncta : 0;
-                const int cslot = ((int)(cb / KB) == tile - sched.sk_tile0) ? 0 : 1;
-                const float* p = ws + (size_t)((cv ? c : c_first) * 2 + cslot) * Cfg::PART_FLOATS + r4;
+                const int cr = cv ? c : c_first;
+                const float* p = ws + (size_t)(cr * 2 + sched.partial_slot(cr, tile)) * Cfg::PART_FLOATS + r4;
 #pragma unroll
                 for (int j = 0; j < FIX_T; ++j) {
                   const int t = tb + EP_WARPS * j;
@@ -685,7 +565,8 @@ static cudaError_t gemm_set_attrs() {
 // per SM, and the split factor (hence the split points and the numerics) must not depend on which instantiation runs.
 static int gemm_max_clusters(int s, int num_sms) {
   static int cache[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-  if (s < 2 || s > 8) return num_sms / (s > 0 ? s : 1);
+  static bool no_device = false;  // host-only callers vary num_sms between calls: nothing is cached then
+  if (s < 2 || s > 8 || no_device) return num_sms / (s > 0 ? s : 1);
   if (cache[s] == 0) {
     using Cfg = GemmCfg<32>;
     cudaLaunchConfig_t qc{};
@@ -705,7 +586,8 @@ static int gemm_max_clusters(int s, int num_sms) {
       cache[s] = n;
     } else {
       cudaGetLastError();
-      cache[s] = num_sms / s;
+      no_device = true;
+      return num_sms / s;
     }
   }
   return cache[s];
@@ -813,16 +695,26 @@ int gemm_cluster_split(int T, int N, int K, int num_sms) {
   }
 }
 
+// bit 0: weights are read once (evict-first); bit 1: stream-K share before the whole tiles (GemmSched::sk_first).
+// Token tiles above 64 rows keep the pure cut: there the whole tile's direct epilogue (128+ tokens per row) is a
+// longer tail than the fix-up it replaces.
+int gemm_stream_flags(int T) {
+  const int BT = gemm_pick_bt(T);
+  return T <= BT ? (1 | (BT <= 64 ? 2 : 0)) : 0;
+}
+
+GemmSched gemm_schedule(int T, int N, int K, int num_sms) {
+  const int BT = gemm_pick_bt(T);
+  return GemmSched((N + GEMM_BN - 1) / GEMM_BN, (T + BT - 1) / BT, (K + GEMM_BK - 1) / GEMM_BK,
+                   gemm_grid_size(T, N, K, num_sms), (gemm_stream_flags(T) & 2) != 0);
+}
+
 template <int BT>
 static cudaError_t launch_bt(const CUtensorMap& wmap, const CUtensorMap& xmap, void* Y, int ldy, int T, int N, int K,
                              float* ws, int* counters, int num_sms, int out_f32, cudaStream_t stream,
                              const GemmRope& rope, bool lean) {
-  const int t_tiles = (T + BT - 1) / BT;
   const int grid = gemm_grid_size(T, N, K, num_sms);
-  // bit 0: weights are read once (evict-first); bit 1: stream-K share before the whole tiles (GemmSched::sk_first).
-  // Token tiles above 64 rows keep the pure cut: there the whole tile's direct epilogue (128+ tokens per row) is a
-  // longer tail than the fix-up it replaces.
-  const int stream_weights = (t_tiles == 1) ? (1 | (BT <= 64 ? 2 : 0)) : 0;
+  const int stream_weights = gemm_stream_flags(T);
   const int split = cluster_split_bt<BT>(T, N, K, num_sms);
   // the fused RoPE epilogue lives in the two split-tile reductions (cluster and global fix-up): every tile must be split
   if (rope.positions != nullptr && (gemm_even_split(T, N, K, num_sms) < 2 || out_f32 != 0 ||

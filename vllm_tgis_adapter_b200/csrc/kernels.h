@@ -22,6 +22,9 @@ int attention_set_step_timeline(unsigned long long* buf);
 int sampler_set_step_timeline(unsigned long long* buf);
 int gemm_grid_size(int T, int N, int K, int num_sms);
 int gemm_even_split(int T, int N, int K, int num_sms);  // every tile cut over this many consecutive CTAs, or 0
+int gemm_stream_flags(int T);  // the kernel's stream_weights argument: bit 0 evict-first weights, bit 1 sk_first
+struct GemmSched;              // gemm_sched.cuh
+GemmSched gemm_schedule(int T, int N, int K, int num_sms);  // the work schedule gemm_bf16_launch runs
 // Y: bf16 [T, ldy] (out_f32 = 0), fp32 [T, ldy] (out_f32 = 1, lm_head logits), or out_f32 = 2: fused SwiGLU — W rows are
 // interleaved (gate_j, up_j) pairs and Y is bf16 [T, ldy >= N/2] = bf16(bf16(silu(gate)) * up)
 // Optional fused epilogue of the qkv projection (cluster mode only, gemm_cluster_split() > 0): RoPE on the q / k heads

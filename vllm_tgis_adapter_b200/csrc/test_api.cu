@@ -5,6 +5,7 @@
 #include <vector>
 
 #include "../../include/tgis_kernels.h"
+#include "gemm_sched.cuh"
 #include "kernels.h"
 
 using namespace tgis;
@@ -449,6 +450,97 @@ int tgis_k_gemm_plan(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* 
   *bt_out = gemm_pick_bt(T);
   *grid_out = gemm_grid_size(T, N, K, num_sms);
   *even_split_out = gemm_even_split(T, N, K, num_sms);
+  return 0;
+}
+
+// Host-only: the GEMM's work schedule for a shape, listed from the code the kernel runs (gemm_sched.cuh).  No GPU needed
+// (without one, the cluster split reads 0 and the even-split factor assumes every cluster fits).
+int tgis_k_gemm_schedule(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* info_out, int32_t* units_out,
+                         int32_t unit_cap, int32_t* n_units_out, int32_t* splits_out, int32_t split_cap,
+                         int32_t* n_splits_out, int32_t* reads_out, int32_t read_cap, int32_t* n_reads_out) {
+  if (T <= 0 || N <= 0 || K <= 0 || num_sms <= 0) return kfail("bad shape");
+  const GemmSched sc = gemm_schedule(T, N, K, num_sms);
+  if (sc.sk_total > INT32_MAX) return kfail("stream-K region too large to list");
+  const int32_t info[12] = {gemm_pick_bt(T), sc.ncta, gemm_even_split(T, N, K, num_sms),
+                            gemm_cluster_split(T, N, K, num_sms), sc.n_tiles, sc.t_tiles, sc.KB, sc.dp_waves,
+                            sc.dp_extra, sc.sk_first ? 1 : 0, sc.sk_tile0, (int32_t)sc.sk_total};
+  memcpy(info_out, info, sizeof(info));
+  const int tiles = sc.n_tiles * sc.t_tiles;
+  std::vector<int> last_owner(tiles, -1), owners(tiles, 0);
+  std::vector<char> split(tiles, 0);
+  int nu = 0;
+  for (int c = 0; c < sc.ncta; ++c) {
+    UnitIter it(sc, c);
+    int tile, kb0, kb1, slot;
+    while (it.next(tile, kb0, kb1, slot)) {
+      if (nu >= unit_cap) return kfail("unit_cap too small");
+      const int32_t u[5] = {c, tile, kb0, kb1, slot};
+      memcpy(units_out + 5 * nu++, u, sizeof(u));
+      if (tile < 0 || tile >= tiles) continue;  // (listed; the caller checks the range)
+      if (last_owner[tile] != c) ++owners[tile];
+      last_owner[tile] = c;
+      if (kb0 > 0 || kb1 < sc.KB) split[tile] = 1;
+    }
+  }
+  *n_units_out = nu;
+  int ns = 0, nr = 0;
+  for (int tile = 0; tile < tiles; ++tile) {
+    if (!split[tile]) continue;
+    int c_first, c_last;
+    sc.split_owners(tile, c_first, c_last);
+    if (ns >= split_cap) return kfail("split_cap too small");
+    const int32_t s[4] = {tile, c_first, owners[tile], c_last - c_first + 1};
+    memcpy(splits_out + 4 * ns++, s, sizeof(s));
+    for (int c = c_first; c <= c_last; ++c) {
+      if (nr >= read_cap) return kfail("read_cap too small");
+      const int32_t r[3] = {tile, c, sc.partial_slot(c, tile)};
+      memcpy(reads_out + 3 * nr++, r, sizeof(r));
+    }
+  }
+  *n_splits_out = ns;
+  *n_reads_out = nr;
+  return 0;
+}
+
+// GEMMs launched back to back on one stream the way the engine's step launches them: PDL, the lean decode
+// instantiation, ONE workspace and ONE counter array zeroed once before the first launch, no synchronisation in
+// between.  desc_host: n x 7 {T, N, K, ldx, x_rows_alloc, ldy, out_f32}; ptrs_host: n x 3 device addresses {x, w, y}.
+// *counters_left_out = the number of counters not back at 0 after the last GEMM.
+int tgis_k_gemm_chain(int32_t n, const int32_t* desc_host, const uint64_t* ptrs_host, int32_t* counters_left_out) {
+  const int sms = test_num_sms();
+  constexpr int N_COUNTERS = 1 << 16;  // as the engine allocates them
+  std::vector<CUtensorMap> wm(n), xm(n);
+  for (int i = 0; i < n; ++i) {
+    const int32_t* d = desc_host + 7 * i;
+    const int T = d[0], N = d[1], K = d[2], ldx = d[3], x_rows = d[4];
+    if (T <= 0 || N <= 0 || K <= 0 || x_rows < gemm_pick_bt(T)) return kfail("bad shape or too few x rows allocated");
+    if (make_tmap_bf16_2d(&wm[i], (const void*)ptrs_host[3 * i + 1], N, K, K, 128, 64) != 0)
+      return kfail("weight tensor map failed");
+    if (make_tmap_bf16_2d(&xm[i], (const void*)ptrs_host[3 * i], x_rows, K, ldx, gemm_pick_bt(T), 64) != 0)
+      return kfail("activation tensor map failed");
+  }
+  Tmp<float> ws;
+  Tmp<int> ctr;
+  KCK(ws.alloc(gemm_workspace_bytes(sms) / sizeof(float)));
+  KCK(ctr.alloc(N_COUNTERS));
+  KCK(cudaMemset(ctr.p, 0, sizeof(int) * N_COUNTERS));
+  KCK(cudaDeviceSynchronize());
+  cudaStream_t st;
+  KCK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  cudaError_t e = cudaSuccess;
+  for (int i = 0; i < n && e == cudaSuccess; ++i) {
+    const int32_t* d = desc_host + 7 * i;
+    e = gemm_bf16_launch(wm[i], xm[i], (void*)ptrs_host[3 * i + 2], d[5], d[0], d[1], d[2], ws.p, ctr.p, sms, st, d[6]);
+  }
+  const cudaError_t es = cudaStreamSynchronize(st);
+  cudaStreamDestroy(st);
+  if (e != cudaSuccess) return kfail(std::string("gemm_bf16_launch: ") + cudaGetErrorString(e));
+  if (es != cudaSuccess) return kfail(std::string("cudaStreamSynchronize: ") + cudaGetErrorString(es));
+  std::vector<int> h(N_COUNTERS);
+  KCK(cudaMemcpy(h.data(), ctr.p, sizeof(int) * N_COUNTERS, cudaMemcpyDeviceToHost));
+  int left = 0;
+  for (int v : h) left += v != 0;
+  *counters_left_out = left;
   return 0;
 }
 

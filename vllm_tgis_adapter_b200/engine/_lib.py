@@ -76,7 +76,7 @@ ENGINE_SYMBOLS = [
 ]
 KERNEL_SYMBOLS = [
     "tgis_k_last_error", "tgis_k_gemm_timeline", "tgis_k_step_timeline_enable", "tgis_k_step_timeline_read", "tgis_k_gemm", "tgis_k_rmsnorm", "tgis_k_rmsnorm_mult", "tgis_k_embed", "tgis_k_opt_layernorm", "tgis_k_opt_bias_act", "tgis_k_opt_embed", "tgis_k_silu_mul", "tgis_k_rope_kv", "tgis_k_gemm_rope", "tgis_k_attention", "tgis_k_attention_split", "tgis_k_attention_split_bench", "tgis_k_rope_attention",
-    "tgis_k_attention_bench", "tgis_k_decode_items", "tgis_k_gemm_plan", "tgis_k_gemm_blocks_per_sm",
+    "tgis_k_attention_bench", "tgis_k_decode_items", "tgis_k_gemm_plan", "tgis_k_gemm_schedule", "tgis_k_gemm_chain", "tgis_k_gemm_blocks_per_sm",
     "tgis_k_sampler", "tgis_k_sampler_ex", "tgis_k_sampler_masked", "tgis_k_sampler_scaled", "tgis_k_lora", "tgis_k_lora_bench", "tgis_k_silu_mul_interleaved", "tgis_k_sizeof_sample_row", "tgis_k_sizeof_sample_out", "tgis_k_kv_block",
 ]
 
@@ -131,6 +131,9 @@ def load_library() -> C.CDLL:
     lib.tgis_engine_destroy.restype = None
     lib.tgis_engine_run_until_idle.argtypes = [vp]
     lib.tgis_k_gemm.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(f32), i32]
+    lib.tgis_k_gemm_schedule.argtypes = [i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), i32, C.POINTER(i32), C.POINTER(i32), i32, C.POINTER(i32),
+                                         C.POINTER(i32), i32, C.POINTER(i32)]
+    lib.tgis_k_gemm_chain.argtypes = [i32, C.POINTER(i32), C.POINTER(C.c_uint64), C.POINTER(i32)]
     lib.tgis_k_rmsnorm.argtypes = [vp, vp, vp, vp, i32, i32, f32]
     lib.tgis_k_rmsnorm_mult.argtypes = [vp, vp, vp, vp, i32, i32, f32, f32]
     lib.tgis_k_embed.argtypes = [vp, vp, vp, i32, i32, i32, f32]
