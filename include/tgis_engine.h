@@ -64,7 +64,8 @@ typedef struct tgis_config {
   int32_t hidden;
   int32_t n_q_heads;
   int32_t n_kv_heads;
-  int32_t head_dim; /* 128; OPT: 64 or 128 */
+  int32_t head_dim; /* 128 or 64 (LLAMA 64: native 64-dim KV tiles, tp_size 1, max_loras 0, no Granite scalars; OPT 64:
+                       zero-padded to the 128-dim tiles) */
   int32_t ffn;
   int32_t vocab;              /* any size when tp_size == 1 (the lm_head is padded to a multiple of 8 internally) */
   float rope_theta;
@@ -206,9 +207,15 @@ int tgis_engine_load_weight(tgis_engine* e, const char* name, const void* ptr, i
  *   residual_multiplier   r = bf16(r + bf16(x * m)) after o_proj and after down_proj; tp_size must be 1 unless m == 1
  *   attention_multiplier  the softmax scale (0: 1 / sqrt(head_dim))
  *   logit_scale           1 / logits_scaling: the sampler sees bf16(logit * s)
- * The defaults 1, 1, 0, 1 are the Llama stack, bit for bit. */
+ * The defaults 1, 1, 0, 1 are the Llama stack, bit for bit.  An engine created with head_dim 64 accepts only the
+ * defaults (Granite with 64-dim heads is not supported yet). */
 int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, float residual_multiplier,
                                   float attention_multiplier, float logit_scale);
+/* Scaled rotary embeddings (config.json rope_scaling / rope_parameters, e.g. rope_type llama3): the host computes the
+ * scaled table and loads it as the weight "tgis.rope_cos_sin" ([max_model_len][head_dim] = cos | sin).  After this call
+ * tgis_engine_start fails unless that table was loaded, instead of serving the built-in unscaled one.  Valid only between
+ * tgis_engine_create and tgis_engine_start, TGIS_ARCH_LLAMA only. */
+int tgis_engine_require_rope_table(tgis_engine* e);
 /* Automatic prefix caching (vLLM's enable_prefix_caching; default off here, on in vLLM).  Valid only between
  * tgis_engine_create and tgis_engine_start.  A full 32-token KV block that a completed step wrote is keyed by (its
  * parent's key, its 32 token ids, LoRA slot + the slot's generation, bumped by every clear / weight load of the slot);

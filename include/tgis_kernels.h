@@ -80,6 +80,23 @@ int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, 
                           const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, const int32_t* seqs_host,
                           int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride,
                           void* out_dev, int32_t n_q, int32_t n_kv, float scale);
+/* The same hooks for either head geometry: head_dim 128 (the calls above) or 64, where qkv rows are (n_q + 2 n_kv) * 64,
+ * cos_sin rows cos(32) | sin(32), a K tile is [8 chunks][32 tok][8] and a V tile [32 tok][8 chunks ^ (tok & 7)][8] (4 KiB
+ * each), for group sizes n_q / n_kv in {1, 2, 4, 8}.  tgis_k_attention_hd = tgis_k_attention_split_hd with mode 0. */
+int tgis_k_rope_kv_hd(int32_t head_dim, void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
+                      const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q,
+                      int32_t n_kv);
+int tgis_k_attention_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                        const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
+                        int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale);
+int tgis_k_attention_split_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                              const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                              int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
+                              int32_t mode);
+int tgis_k_attention_bench_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                              const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                              int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
+                              int32_t n_layers, int64_t layer_stride_bytes, int32_t iters, float* us_out);
 /* host-only: GEMM launch plan for a shape: token tile (16..256), grid, even-split factor (0: stream-K + global fix-up) */
 int tgis_k_gemm_plan(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* bt_out, int32_t* grid_out,
                      int32_t* even_split_out);

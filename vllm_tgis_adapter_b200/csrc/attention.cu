@@ -1,5 +1,7 @@
 // Paged-KV attention for the TGIS hot path (SURVEY.md §2.2 K6/K7; reference call site: grpc_server.py:222 ->
-// vllm v1/attention/backends/flashinfer.py:1665,1803).  Causal, GQA, head_dim 128, bf16 in / fp32 softmax.
+// vllm v1/attention/backends/flashinfer.py:1665,1803).  Causal, GQA, bf16 in / fp32 softmax.  The head dimension D is a
+// template parameter of every kernel here: 128 (the figures quoted in the comments) or 64, where a K / V tile is 4 KiB of
+// 8 chunks, every MMA loop over the head dimension is half as long and a decode warp's ring holds twice as many tiles.
 //
 // HBM layout of the cache (ours to choose; see kernels.h): per (block, kv_head) one contiguous 8 KiB K tile stored
 // "8-dim chunk major" [16][32 tok][8] and one 8 KiB V tile [32 tok][16 chunks ^ (tok&7)][8].  Both tiles are fetched
@@ -27,7 +29,7 @@ namespace tgis {
 TGIS_STL_DEFINE(attention)
 
 constexpr int DEC_TOK = DECODE_SPLIT;        // tokens per split (8 KV blocks streamed through a 4-stage ring)
-constexpr int TILE_BYTES = KV_BLOCK * HEAD_DIM * 2;  // 8192
+template <int D> constexpr int TILE_BYTES = KV_BLOCK * D * 2;  // 8192 (D = 64: 4096)
 static_assert(DEC_TOK == DECODE_SPLIT, "split size mismatch");
 
 __device__ __forceinline__ float warp_max(float v) {
@@ -95,26 +97,30 @@ constexpr int DEC_THREADS = DEC_WARPS * 32;
 #ifndef TGIS_DEC_MINB
 #define TGIS_DEC_MINB 2  // CTAs per SM (register cap); shared memory must agree: MINB * 4 * (RING * 8 + 2) KiB <= 227
 #endif
-constexpr int DEC_RING = TGIS_DEC_RING;
-constexpr int DEC_Q_BYTES = 8 * HEAD_DIM * 2;                           // up to 8 heads
-constexpr int DEC_WARP_SMEM = DEC_RING * TILE_BYTES + DEC_Q_BYTES;      // 26 KiB
-constexpr int DEC_SMEM = DEC_WARPS * DEC_WARP_SMEM + DEC_WARPS * 4 * 8; // + 4 mbarriers per warp
+// D = 64: twice the tiles of half the size, so a warp keeps the same 24 KiB in flight in the same shared-memory budget
+template <int D> constexpr int DEC_RING = TGIS_DEC_RING * (128 / D);
+template <int D> constexpr int DEC_Q_BYTES = 8 * D * 2;                                          // up to 8 heads
+template <int D> constexpr int DEC_WARP_SMEM = DEC_RING<D> * TILE_BYTES<D> + DEC_Q_BYTES<D>;     // 26 KiB (D = 64: 25)
+// + one mbarrier per ring buffer and one for Q, per warp
+template <int D> constexpr int DEC_SMEM = DEC_WARPS * DEC_WARP_SMEM<D> + DEC_WARPS * (DEC_RING<D> + 1) * 8;
 
-template <int G>
+template <int D, int G>
 __global__ void __launch_bounds__(DEC_THREADS, TGIS_DEC_MINB)
 attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv_bfloat16* __restrict__ k_cache,
                    const __nv_bfloat16* __restrict__ v_cache, const DecItem* __restrict__ items,
                    int max_splits, float* __restrict__ part_o, float* __restrict__ part_ml,
                    __nv_bfloat16* __restrict__ out, int out_ld, int n_kv, float scale, int prefetch_old) {
   static_assert(G <= 8, "query heads of a group are rows 0..7 of the MMA tile");
+  constexpr int DEC_RING = tgis::DEC_RING<D>, DEC_WARP_SMEM = tgis::DEC_WARP_SMEM<D>;
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint8_t* ring = smem + warp * DEC_WARP_SMEM;
-  uint8_t* q_s = ring + DEC_RING * TILE_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + DEC_WARPS * DEC_WARP_SMEM) + warp * 4;  // [3] tiles, [3] = Q
-  uint64_t* q_bar = full + 3;
+  uint8_t* q_s = ring + DEC_RING * TILE_BYTES<D>;
+  // [DEC_RING] tiles, [DEC_RING] = Q
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + DEC_WARPS * DEC_WARP_SMEM) + warp * (DEC_RING + 1);
+  uint64_t* q_bar = full + DEC_RING;
   if (lane == 0) {
-    for (int i = 0; i < 4; ++i) mbar_init(&full[i], 1);
+    for (int i = 0; i <= DEC_RING; ++i) mbar_init(&full[i], 1);
     fence_barrier_init();
   }
   __syncwarp();
@@ -153,9 +159,9 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
     if (i_f >= n_flat) return;
     if (lane == 0) {
       const __nv_bfloat16* src =
-          (i_kv ? v_cache : k_cache) + ((size_t)pick(i_blks, i_jb) * n_kv + i_kvh) * (KV_BLOCK * HEAD_DIM);
-      mbar_arrive_expect_tx(&full[i_buf], TILE_BYTES);
-      bulk_load_1d_hint(ring + i_buf * TILE_BYTES, src, TILE_BYTES, &full[i_buf], kv_policy);  // read once per step
+          (i_kv ? v_cache : k_cache) + ((size_t)pick(i_blks, i_jb) * n_kv + i_kvh) * (KV_BLOCK * D);
+      mbar_arrive_expect_tx(&full[i_buf], TILE_BYTES<D>);
+      bulk_load_1d_hint(ring + i_buf * TILE_BYTES<D>, src, TILE_BYTES<D>, &full[i_buf], kv_policy);  // read once per step
     }
     i_buf = i_buf == DEC_RING - 1 ? 0 : i_buf + 1;
     if (i_kv == 0) {
@@ -179,8 +185,8 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
   };
   auto issue_q = [&](const int4& it, int kvh) {
     if (lane == 0) {
-      mbar_arrive_expect_tx(q_bar, G * HEAD_DIM * 2);
-      bulk_load_1d(q_s, qkv + (size_t)it.x * qkv_ld + (size_t)kvh * G * HEAD_DIM, G * HEAD_DIM * 2, q_bar);
+      mbar_arrive_expect_tx(q_bar, G * D * 2);
+      bulk_load_1d(q_s, qkv + (size_t)it.x * qkv_ld + (size_t)kvh * G * D, G * D * 2, q_bar);
     }
   };
 
@@ -220,29 +226,29 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
     // ---- Q^T as B fragments: n = head (lane/4), 8 k-steps of 16 dims; heads >= G are zero columns
     mbar_wait(q_bar, q_ph);
     q_ph ^= 1;
-    uint32_t qb[8][2];
+    uint32_t qb[D / 16][2];
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      const uint8_t* qp = q_s + (hr * HEAD_DIM + ks * 16 + t4 * 2) * 2;
+    for (int ks = 0; ks < D / 16; ++ks) {
+      const uint8_t* qp = q_s + (hr * D + ks * 16 + t4 * 2) * 2;
       qb[ks][0] = hr < G ? *reinterpret_cast<const uint32_t*>(qp) : 0u;
       qb[ks][1] = hr < G ? *reinterpret_cast<const uint32_t*>(qp + 16) : 0u;
     }
     // this thread's accumulators: heads 2*t4 + {0,1} (e & 1), dims md*16 + hr + {0,8} (e >> 1)
-    float ot[8][4];
+    float ot[D / 16][4];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) ot[i][0] = ot[i][1] = ot[i][2] = ot[i][3] = 0.f;
+    for (int i = 0; i < D / 16; ++i) ot[i][0] = ot[i][1] = ot[i][2] = ot[i][3] = 0.f;
     float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};  // l_r: this thread's share (reduced at the end)
 
     for (int jb = 0; jb < n_blk; ++jb) {
       // ---- S^T = K Q^T : 2 m-tiles (16 tokens) x 8 k-steps (16 dims = chunks 2ks, 2ks+1); ldmatrix.x4 = one A
       // fragment: matrices (tok lo, chunk 2ks), (tok hi, chunk 2ks), (tok lo, chunk 2ks+1), (tok hi, chunk 2ks+1)
       mbar_wait(&full[c_buf], c_ph);
-      const uint32_t k_base = ring_base + c_buf * TILE_BYTES;
+      const uint32_t k_base = ring_base + c_buf * TILE_BYTES<D>;
       float st[2][4];
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt) st[mt][0] = st[mt][1] = st[mt][2] = st[mt][3] = 0.f;
 #pragma unroll
-      for (int ks = 0; ks < 8; ++ks) {
+      for (int ks = 0; ks < D / 16; ++ks) {
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) {
           uint32_t ka[4];
@@ -295,7 +301,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
         bl[mt][1] = movmatrix_trans(pack_bf16x2(p[2] - bf16_round(p[2]), p[3] - bf16_round(p[3])));
       }
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
+      for (int i = 0; i < D / 16; ++i) {
         ot[i][0] *= corr[0];
         ot[i][1] *= corr[1];
         ot[i][2] *= corr[0];
@@ -305,16 +311,16 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
       // ldmatrix.trans: matrices (tok lo, chunk 2md), (tok lo, chunk 2md+1), (tok hi, chunk 2md), (tok hi, chunk 2md+1).
       // Slots >= valid carry p = 0 (cache slots hold finite values).
       mbar_wait(&full[c_buf], c_ph);
-      const uint32_t v_base = ring_base + c_buf * TILE_BYTES;
+      const uint32_t v_base = ring_base + c_buf * TILE_BYTES<D>;
 #pragma unroll
       for (int kk = 0; kk < 2; ++kk) {
         const int tok = kk * 16 + (mi >> 1) * 8 + ri;
 #pragma unroll
-        for (int md = 0; md < 8; md += 2) {
+        for (int md = 0; md < D / 16; md += 2) {
           uint32_t va[2][4];
 #pragma unroll
           for (int u = 0; u < 2; ++u)
-            ldmatrix_x4_trans(va[u], v_base + tok * (HEAD_DIM * 2) + (((2 * (md + u) + (mi & 1)) ^ (tok & 7)) * 16));
+            ldmatrix_x4_trans(va[u], v_base + tok * (D * 2) + (((2 * (md + u) + (mi & 1)) ^ (tok & 7)) * 16));
           mma_bf16_16816(ot[md], va[0], bh[kk][0], bh[kk][1]);
           mma_bf16_16816(ot[md + 1], va[1], bh[kk][0], bh[kk][1]);
           mma_bf16_16816(ot[md], va[0], bl[kk][0], bl[kk][1]);
@@ -334,25 +340,25 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
 
     // ---- item epilogue
     if (n_splits == 1) {
-      __nv_bfloat16* o_dst = out + (size_t)c_it.x * out_ld + (size_t)(kvh * G + 2 * t4) * HEAD_DIM + hr;
+      __nv_bfloat16* o_dst = out + (size_t)c_it.x * out_ld + (size_t)(kvh * G + 2 * t4) * D + hr;
       const float inv[2] = {1.f / l_r[0], 1.f / l_r[1]};
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         if (2 * t4 + (e & 1) < G) {
 #pragma unroll
-          for (int md = 0; md < 8; ++md)
-            o_dst[(e & 1) * HEAD_DIM + md * 16 + (e >> 1) * 8] = __float2bfloat16_rn(ot[md][e] * inv[e & 1]);
+          for (int md = 0; md < D / 16; ++md)
+            o_dst[(e & 1) * D + md * 16 + (e >> 1) * 8] = __float2bfloat16_rn(ot[md][e] * inv[e & 1]);
         }
       }
     } else {
       // store the partial (m in the exp2 domain); attn_merge_kernel combines the splits in split order
       const size_t pbase = (size_t)(seq * n_kv + kvh) * max_splits;
-      float* po = part_o + ((pbase + split) * G + 2 * t4) * HEAD_DIM + hr;
+      float* po = part_o + ((pbase + split) * G + 2 * t4) * D + hr;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         if (2 * t4 + (e & 1) < G) {
 #pragma unroll
-          for (int md = 0; md < 8; ++md) po[(e & 1) * HEAD_DIM + md * 16 + (e >> 1) * 8] = ot[md][e];
+          for (int md = 0; md < D / 16; ++md) po[(e & 1) * D + md * 16 + (e >> 1) * 8] = ot[md][e];
         }
       }
       if (hr == 0) {
@@ -369,8 +375,8 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
 
 // Split merge: one CTA per (decode sequence, kv head) with more than one split, thread = dim.  Reads the partials in
 // split order (deterministic), writes the normalised bf16 rows.
-template <int G>
-__global__ void __launch_bounds__(HEAD_DIM)
+template <int D, int G>
+__global__ void __launch_bounds__(D)
 attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ seq_ids, int max_splits,
                   const float* __restrict__ part_o, const float* __restrict__ part_ml,
                   __nv_bfloat16* __restrict__ out, int out_ld, int n_kv) {
@@ -391,7 +397,7 @@ attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ 
   for (int c0 = 0; c0 < n_splits; c0 += 64) {
     const int nc = min(64, n_splits - c0);
     __syncthreads();
-    for (int i = d; i < nc * G * 2; i += HEAD_DIM) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
+    for (int i = d; i < nc * G * 2; i += D) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
     __syncthreads();
     for (int sp = 0; sp < nc; ++sp)
 #pragma unroll
@@ -403,7 +409,7 @@ attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ 
     const int nc = min(64, n_splits - c0);
     if (n_splits > 64) {
       __syncthreads();
-      for (int i = d; i < nc * G * 2; i += HEAD_DIM) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
+      for (int i = d; i < nc * G * 2; i += D) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
       __syncthreads();
     }
     for (int sp0 = 0; sp0 < nc; sp0 += SPB) {
@@ -412,7 +418,7 @@ attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ 
       for (int j = 0; j < SPB; ++j)
 #pragma unroll
         for (int g = 0; g < G; ++g)
-          ov[j][g] = (sp0 + j < nc) ? __ldcg(&part_o[((pbase + c0 + sp0 + j) * G + g) * HEAD_DIM + d]) : 0.f;
+          ov[j][g] = (sp0 + j < nc) ? __ldcg(&part_o[((pbase + c0 + sp0 + j) * G + g) * D + d]) : 0.f;
 #pragma unroll
       for (int j = 0; j < SPB; ++j) {
         if (sp0 + j < nc) {
@@ -426,13 +432,13 @@ attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ 
       }
     }
   }
-  __nv_bfloat16* o_dst = out + (size_t)sq.q_start * out_ld + (size_t)kvh * G * HEAD_DIM;
+  __nv_bfloat16* o_dst = out + (size_t)sq.q_start * out_ld + (size_t)kvh * G * D;
 #pragma unroll
-  for (int g = 0; g < G; ++g) o_dst[g * HEAD_DIM + d] = __float2bfloat16_rn(o_f[g] / l_f[g]);
+  for (int g = 0; g < G; ++g) o_dst[g * D + d] = __float2bfloat16_rn(o_f[g] / l_f[g]);
   STL_EXIT();
 }
 
-template <int G>
+template <int D, int G>
 static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
                                    const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                    const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits,
@@ -441,7 +447,7 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
   static bool attr = false;
   if (!attr) {
     cudaError_t e =
-        cudaFuncSetAttribute(attn_decode_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, DEC_SMEM);
+        cudaFuncSetAttribute(attn_decode_kernel<D, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, DEC_SMEM<D>);
     if (e != cudaSuccess) return e;
     attr = true;
   }
@@ -449,10 +455,10 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
   const int grid = (int)std::min<long long>((long long)TGIS_DEC_MINB * num_sms, (max_flat + DEC_WARPS - 1) / DEC_WARPS);
   const char* env_pre = getenv("TGIS_ATTN_PREFETCH");  // 0: no cache reads before the grid-dependency wait
   const int prefetch_old = (env_pre && env_pre[0] == '0') ? 0 : 1;
-  cudaError_t e = launch_k(attn_decode_kernel<G>, dim3(grid), dim3(DEC_THREADS), DEC_SMEM, stream, qkv, qkv_ld,
+  cudaError_t e = launch_k(attn_decode_kernel<D, G>, dim3(grid), dim3(DEC_THREADS), DEC_SMEM<D>, stream, qkv, qkv_ld,
                            k_cache, v_cache, items, max_splits, part_o, part_ml, out, out_ld, n_kv, scale, prefetch_old);
   if (e != cudaSuccess || max_splits <= 1) return e;
-  return launch_k(attn_merge_kernel<G>, dim3(n_seqs, n_kv), dim3(HEAD_DIM), 0, stream, seqs, seq_ids, max_splits,
+  return launch_k(attn_merge_kernel<D, G>, dim3(n_seqs, n_kv), dim3(D), 0, stream, seqs, seq_ids, max_splits,
                   (const float*)part_o, (const float*)part_ml, out, out_ld, n_kv);
 }
 
@@ -460,29 +466,38 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
                                const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits, float* part_o,
                                float* part_ml, __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                               int num_sms, cudaStream_t stream) {
+                               int num_sms, cudaStream_t stream, int head_dim) {
   if (max_entries <= 0 || n_seqs <= 0) return cudaSuccess;
   if (n_q % n_kv != 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
-#define TGIS_DEC(GG)                                                                                               \
-  case GG:                                                                                                         \
-    return decode_launch_g<GG>(qkv, qkv_ld, k_cache, v_cache, items, max_entries, seqs, seq_ids, n_seqs, max_splits, \
-                               part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream)
-  switch (G) {
-    TGIS_DEC(1);
-    TGIS_DEC(2);
-    TGIS_DEC(3);
-    TGIS_DEC(4);
-    TGIS_DEC(8);
-    default: return cudaErrorInvalidValue;
+#define TGIS_DEC(DD, GG)                                                                                      \
+  case GG:                                                                                                    \
+    return decode_launch_g<DD, GG>(qkv, qkv_ld, k_cache, v_cache, items, max_entries, seqs, seq_ids, n_seqs, \
+                                   max_splits, part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream)
+  if (head_dim == 128) {
+    switch (G) {
+      TGIS_DEC(128, 1);
+      TGIS_DEC(128, 2);
+      TGIS_DEC(128, 3);
+      TGIS_DEC(128, 4);
+      TGIS_DEC(128, 8);
+    }
+  } else if (head_dim == 64) {
+    switch (G) {
+      TGIS_DEC(64, 1);
+      TGIS_DEC(64, 2);
+      TGIS_DEC(64, 4);
+      TGIS_DEC(64, 8);
+    }
   }
 #undef TGIS_DEC
+  return cudaErrorInvalidValue;
 }
 
 // ================================================================================================ prefill
 constexpr int PF_QROWS = 16;  // query tokens per tile
 static_assert(PF_QROWS % PF_CLUSTER == 0, "every CTA of a split cluster merges the same number of rows");
-constexpr int PF_SPLIT_SMEM_MAX = PF_QROWS * HEAD_DIM * 4 * 8;  // G = 8: the fp32 partial O of 8 heads x 16 rows
+template <int D> constexpr int PF_SPLIT_SMEM_MAX = PF_QROWS * D * 4 * 8;  // G = 8: the fp32 partial O of 8 heads x 16 rows
 
 // grid (n_tiles, n_kv) / SPLIT: (n_tiles * PF_CLUSTER, n_kv) in clusters of PF_CLUSTER; blockDim = 32 * G (warp = query
 // head inside the GQA group).
@@ -492,14 +507,14 @@ constexpr int PF_SPLIT_SMEM_MAX = PF_QROWS * HEAD_DIM * 4 * 8;  // G = 8: the fp
 // more), and after a cluster barrier merges the partials of rows [r * 16 / PF_CLUSTER, ...) from every rank through
 // distributed shared memory, in rank order, in fp32.  No global workspace and no atomics: the same bits on every run,
 // and the split points depend only on the tile's own block range.
-template <bool SPLIT>
+template <int D, bool SPLIT>
 __global__ void __launch_bounds__(256)
 attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv_bfloat16* __restrict__ k_cache,
                     const __nv_bfloat16* __restrict__ v_cache, const AttnSeq* __restrict__ seqs,
                     const int32_t* __restrict__ tile_seq, const int32_t* __restrict__ tile_q0,
                     const int32_t* __restrict__ block_table, int bt_stride, __nv_bfloat16* __restrict__ out,
                     int out_ld, int n_kv, int G, float scale) {
-  __shared__ __align__(128) uint8_t kv_static[SPLIT ? 16 : 2 * 2 * TILE_BYTES];  // 2 stages x (K | V)
+  __shared__ __align__(128) uint8_t kv_static[SPLIT ? 16 : 2 * 2 * TILE_BYTES<D>];  // 2 stages x (K | V)
   extern __shared__ __align__(128) uint8_t kv_dyn[];
   uint8_t* kv_s = SPLIT ? kv_dyn : kv_static;
   __shared__ uint64_t bars[2];
@@ -529,10 +544,10 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   const int32_t* bt = block_table + (size_t)sq.block_row * bt_stride;
   auto issue = [&](int j) {
     const int st = (j - jb0) & 1;
-    const size_t tl = ((size_t)bt[j] * n_kv + kvh) * (KV_BLOCK * HEAD_DIM);
-    mbar_arrive_expect_tx(&bars[st], 2 * TILE_BYTES);
-    bulk_load_1d(kv_s + st * 2 * TILE_BYTES, k_cache + tl, TILE_BYTES, &bars[st]);
-    bulk_load_1d(kv_s + st * 2 * TILE_BYTES + TILE_BYTES, v_cache + tl, TILE_BYTES, &bars[st]);
+    const size_t tl = ((size_t)bt[j] * n_kv + kvh) * (KV_BLOCK * D);
+    mbar_arrive_expect_tx(&bars[st], 2 * TILE_BYTES<D>);
+    bulk_load_1d(kv_s + st * 2 * TILE_BYTES<D>, k_cache + tl, TILE_BYTES<D>, &bars[st]);
+    bulk_load_1d(kv_s + st * 2 * TILE_BYTES<D> + TILE_BYTES<D>, v_cache + tl, TILE_BYTES<D>, &bars[st]);
   };
   if (threadIdx.x == 0) {
     if (jb1 > jb0) issue(jb0);
@@ -540,22 +555,22 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   }
 
   // Q fragments (A operand), rows g and g+8 of the tile; rows past n_rows are clamped (results discarded)
-  uint32_t qa[8][4];
+  uint32_t qa[D / 16][4];
   {
     const int r0 = min(g, n_rows - 1), r1 = min(g + 8, n_rows - 1);
-    const __nv_bfloat16* q_r0 = qkv + (size_t)(sq.q_start + q0 + r0) * qkv_ld + (size_t)head * HEAD_DIM;
-    const __nv_bfloat16* q_r1 = qkv + (size_t)(sq.q_start + q0 + r1) * qkv_ld + (size_t)head * HEAD_DIM;
+    const __nv_bfloat16* q_r0 = qkv + (size_t)(sq.q_start + q0 + r0) * qkv_ld + (size_t)head * D;
+    const __nv_bfloat16* q_r1 = qkv + (size_t)(sq.q_start + q0 + r1) * qkv_ld + (size_t)head * D;
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
+    for (int ks = 0; ks < D / 16; ++ks) {
       qa[ks][0] = *reinterpret_cast<const uint32_t*>(q_r0 + ks * 16 + t * 2);
       qa[ks][1] = *reinterpret_cast<const uint32_t*>(q_r1 + ks * 16 + t * 2);
       qa[ks][2] = *reinterpret_cast<const uint32_t*>(q_r0 + ks * 16 + 8 + t * 2);
       qa[ks][3] = *reinterpret_cast<const uint32_t*>(q_r1 + ks * 16 + 8 + t * 2);
     }
   }
-  float o[16][4];
+  float o[D / 8][4];
 #pragma unroll
-  for (int i = 0; i < 16; ++i)
+  for (int i = 0; i < D / 8; ++i)
 #pragma unroll
     for (int e = 0; e < 4; ++e) o[i][e] = 0.f;
   float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};
@@ -565,15 +580,15 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   for (int j = jb0; j < jb1; ++j) {
     const int st = (j - jb0) & 1;
     mbar_wait(&bars[st], ((j - jb0) >> 1) & 1);
-    const uint8_t* k_t = kv_s + st * 2 * TILE_BYTES;
-    const uint8_t* v_t = k_t + TILE_BYTES;
+    const uint8_t* k_t = kv_s + st * 2 * TILE_BYTES<D>;
+    const uint8_t* v_t = k_t + TILE_BYTES<D>;
     // ---- S = Q K^T : 4 n-tiles (8 tokens each) x 8 k-steps
     float s[4][4];
 #pragma unroll
     for (int nt = 0; nt < 4; ++nt) {
       s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
 #pragma unroll
-      for (int ks = 0; ks < 8; ++ks) {
+      for (int ks = 0; ks < D / 16; ++ks) {
         const int tok = nt * 8 + g;
         const uint32_t b0 = *reinterpret_cast<const uint32_t*>(k_t + ((2 * ks) * KV_BLOCK + tok) * 16 + t * 4);
         const uint32_t b1 = *reinterpret_cast<const uint32_t*>(k_t + ((2 * ks + 1) * KV_BLOCK + tok) * 16 + t * 4);
@@ -602,7 +617,7 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
       l_r[r] *= corr[r];
     }
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
+    for (int i = 0; i < D / 8; ++i) {
       o[i][0] *= corr[0]; o[i][1] *= corr[0]; o[i][2] *= corr[1]; o[i][3] *= corr[1];
     }
     // P is fed to the tensor cores as bf16 hi + bf16 lo (two MMAs): ~16 mantissa bits instead of 8, so the result
@@ -629,13 +644,13 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
 #pragma unroll
     for (int kk = 0; kk < 2; ++kk) {
 #pragma unroll
-      for (int nd = 0; nd < 16; nd += 2) {
+      for (int nd = 0; nd < D / 8; nd += 2) {
         // lane -> (matrix = lane/8, row = lane%8): matrices (tok lo, nd), (tok hi, nd), (tok lo, nd+1), (tok hi, nd+1)
         const int mi = lane >> 3, ri = lane & 7;
         const int tok = kk * 16 + (mi & 1) * 8 + ri;
         const int chunk = nd + (mi >> 1);
         uint32_t vb[4];
-        ldmatrix_x4_trans(vb, v_base + tok * (HEAD_DIM * 2) + ((chunk ^ (tok & 7)) * 16));
+        ldmatrix_x4_trans(vb, v_base + tok * (D * 2) + ((chunk ^ (tok & 7)) * 16));
         mma_bf16_16816(o[nd], pa[kk], vb[0], vb[1]);
         mma_bf16_16816(o[nd + 1], pa[kk], vb[2], vb[3]);
         mma_bf16_16816(o[nd], pl[kk], vb[0], vb[1]);
@@ -659,17 +674,17 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int row = g + r * 8;
-      float* dst = po + (size_t)(warp * PF_QROWS + row) * HEAD_DIM + t * 2;
+      float* dst = po + (size_t)(warp * PF_QROWS + row) * D + t * 2;
 #pragma unroll
-      for (int nd = 0; nd < 16; ++nd)
+      for (int nd = 0; nd < D / 8; ++nd)
         *reinterpret_cast<float2*>(dst + nd * 8) = make_float2(o[nd][r * 2], o[nd][r * 2 + 1]);
       if (t == 0) ml_s[warp * PF_QROWS + row] = make_float4(m_r[r], l_r[r], 0.f, 0.f);
     }
     cluster_sync_all();
-    // merge: this CTA writes rows crank * RPC .. + RPC of every head; 16 threads per (head, row), 8 dims each
-    constexpr int RPC = PF_QROWS / PF_CLUSTER;
+    // merge: this CTA writes rows crank * RPC .. + RPC of every head; 16 threads per (head, row), D / 16 dims each
+    constexpr int RPC = PF_QROWS / PF_CLUSTER, DPT = D / 16;
     const int pr = threadIdx.x >> 4;
-    const int hd = pr / RPC, row = crank * RPC + pr % RPC, d0 = (threadIdx.x & 15) * 8;
+    const int hd = pr / RPC, row = crank * RPC + pr % RPC, d0 = (threadIdx.x & 15) * DPT;
     const int idx = hd * PF_QROWS + row;
     float2 mlk[PF_CLUSTER];
     float m_f = -INFINITY;
@@ -679,28 +694,38 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
       mlk[k] = make_float2(v.x, v.y);
       m_f = fmaxf(m_f, v.x);
     }
-    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float acc[DPT];
+#pragma unroll
+    for (int i = 0; i < DPT; ++i) acc[i] = 0.f;
     float l_f = 0.f;
-    const uint32_t po_addr = smem_u32(po + (size_t)idx * HEAD_DIM + d0);
+    const uint32_t po_addr = smem_u32(po + (size_t)idx * D + d0);
 #pragma unroll
     for (int k = 0; k < PF_CLUSTER; ++k) {
       const float fs = (mlk[k].x == -INFINITY) ? 0.f : exp2f(mlk[k].x - m_f);
-      const float4 a = ld_dsmem_f4(dsmem_addr(po_addr, k));
-      const float4 b = ld_dsmem_f4(dsmem_addr(po_addr + 16, k));
+      float4 a[DPT / 4];
+#pragma unroll
+      for (int i = 0; i < DPT / 4; ++i) a[i] = ld_dsmem_f4(dsmem_addr(po_addr + 16 * i, k));
       l_f += mlk[k].y * fs;
-      acc[0] += a.x * fs; acc[1] += a.y * fs; acc[2] += a.z * fs; acc[3] += a.w * fs;
-      acc[4] += b.x * fs; acc[5] += b.y * fs; acc[6] += b.z * fs; acc[7] += b.w * fs;
+#pragma unroll
+      for (int i = 0; i < DPT / 4; ++i) {
+        acc[4 * i] += a[i].x * fs; acc[4 * i + 1] += a[i].y * fs; acc[4 * i + 2] += a[i].z * fs; acc[4 * i + 3] += a[i].w * fs;
+      }
     }
     cluster_sync_all();  // no CTA leaves while a peer may still read its shared memory
     if (row < n_rows) {
       const float inv = 1.f / l_f;
-      __nv_bfloat16* dst = out + (size_t)(sq.q_start + q0 + row) * out_ld + (size_t)(kvh * G + hd) * HEAD_DIM + d0;
-      uint4 pk;
-      pk.x = pack_bf16x2(acc[0] * inv, acc[1] * inv);
-      pk.y = pack_bf16x2(acc[2] * inv, acc[3] * inv);
-      pk.z = pack_bf16x2(acc[4] * inv, acc[5] * inv);
-      pk.w = pack_bf16x2(acc[6] * inv, acc[7] * inv);
-      *reinterpret_cast<uint4*>(dst) = pk;
+      __nv_bfloat16* dst = out + (size_t)(sq.q_start + q0 + row) * out_ld + (size_t)(kvh * G + hd) * D + d0;
+      if constexpr (D == 128) {
+        uint4 pk;
+        pk.x = pack_bf16x2(acc[0] * inv, acc[1] * inv);
+        pk.y = pack_bf16x2(acc[2] * inv, acc[3] * inv);
+        pk.z = pack_bf16x2(acc[4] * inv, acc[5] * inv);
+        pk.w = pack_bf16x2(acc[6] * inv, acc[7] * inv);
+        *reinterpret_cast<uint4*>(dst) = pk;
+      } else {
+        *reinterpret_cast<uint2*>(dst) =
+            make_uint2(pack_bf16x2(acc[0] * inv, acc[1] * inv), pack_bf16x2(acc[2] * inv, acc[3] * inv));
+      }
     }
     return;
   }
@@ -709,9 +734,9 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
     const int row = g + r * 8;
     if (row < n_rows) {
       const float inv = 1.f / l_r[r];
-      __nv_bfloat16* dst = out + (size_t)(sq.q_start + q0 + row) * out_ld + (size_t)head * HEAD_DIM;
+      __nv_bfloat16* dst = out + (size_t)(sq.q_start + q0 + row) * out_ld + (size_t)head * D;
 #pragma unroll
-      for (int nd = 0; nd < 16; ++nd)
+      for (int nd = 0; nd < D / 8; ++nd)
         *reinterpret_cast<uint32_t*>(dst + nd * 8 + t * 2) = pack_bf16x2(o[nd][r * 2] * inv, o[nd][r * 2 + 1] * inv);
     }
   }
@@ -720,25 +745,26 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
 cudaError_t attn_prefill_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
                                 const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                 const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
-                                __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale, cudaStream_t stream) {
+                                __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale, cudaStream_t stream,
+                                int head_dim) {
   if (n_tiles <= 0) return cudaSuccess;
   if (n_q % n_kv != 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
-  if (G > 8) return cudaErrorInvalidValue;
+  if (G > 8 || (head_dim != 128 && head_dim != 64)) return cudaErrorInvalidValue;
   dim3 grid(n_tiles, n_kv);
-  return launch_k(attn_prefill_kernel<false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
+  if (head_dim == 64)
+    return launch_k(attn_prefill_kernel<64, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
+                    tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale);
+  return launch_k(attn_prefill_kernel<128, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
                   tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale);
 }
 
-cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
-                                      const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
-                                      const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
-                                      __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                                      cudaStream_t stream) {
-  if (n_tiles <= 0) return cudaSuccess;
-  if (n_q % n_kv != 0) return cudaErrorInvalidValue;
-  const int G = n_q / n_kv;
-  if (G > 8) return cudaErrorInvalidValue;
+template <int D>
+static cudaError_t prefill_split_launch_d(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
+                                          const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
+                                          const int32_t* tile_q0, int n_tiles, const int32_t* block_table,
+                                          int bt_stride, __nv_bfloat16* out, int out_ld, int n_kv, int G, float scale,
+                                          cudaStream_t stream) {
   // the shared-memory opt-in is per device: one bit per device ordinal, set once (racing setters set the same value)
   static std::atomic<uint64_t> attr_set{0};
   int dev = 0;
@@ -746,15 +772,34 @@ cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, cons
   if (e != cudaSuccess) return e;
   const uint64_t bit = dev < 64 ? 1ull << dev : 0ull;
   if (!(attr_set.load(std::memory_order_acquire) & bit)) {
-    e = cudaFuncSetAttribute(attn_prefill_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PF_SPLIT_SMEM_MAX);
+    e = cudaFuncSetAttribute(attn_prefill_kernel<D, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             PF_SPLIT_SMEM_MAX<D>);
     if (e != cudaSuccess) return e;
     attr_set.fetch_or(bit, std::memory_order_release);
   }
-  const int smem = std::max(2 * 2 * TILE_BYTES, G * PF_QROWS * HEAD_DIM * 4);
+  const int smem = std::max(2 * 2 * TILE_BYTES<D>, G * PF_QROWS * D * 4);
   dim3 grid(n_tiles * PF_CLUSTER, n_kv);
-  return launch_k_cluster(attn_prefill_kernel<true>, grid, dim3(32 * G), (size_t)smem, stream, PF_CLUSTER, qkv, qkv_ld,
-                          k_cache, v_cache, seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G,
-                          scale);
+  return launch_k_cluster(attn_prefill_kernel<D, true>, grid, dim3(32 * G), (size_t)smem, stream, PF_CLUSTER, qkv,
+                          qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv,
+                          G, scale);
+}
+
+cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
+                                      const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
+                                      const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
+                                      __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
+                                      cudaStream_t stream, int head_dim) {
+  if (n_tiles <= 0) return cudaSuccess;
+  if (n_q % n_kv != 0) return cudaErrorInvalidValue;
+  const int G = n_q / n_kv;
+  if (G > 8) return cudaErrorInvalidValue;
+  if (head_dim == 128)
+    return prefill_split_launch_d<128>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
+                                       bt_stride, out, out_ld, n_kv, G, scale, stream);
+  if (head_dim == 64)
+    return prefill_split_launch_d<64>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
+                                      bt_stride, out, out_ld, n_kv, G, scale, stream);
+  return cudaErrorInvalidValue;
 }
 
 }  // namespace tgis

@@ -629,6 +629,8 @@ cudaError_t silu_mul_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, in
 // grid = (T, ceil(heads/16)); 128 threads = 16 heads x 8 threads; a thread owns 8 consecutive rotary pairs
 // (i..i+7, i+64..i+71): every global access is a 16-byte vector, and 8 consecutive dims are exactly one chunk of the
 // K / V cache layouts, so the scatter is one 16-byte store per half.
+// D = 64: 32 heads x 4 threads, pairs (i..i+7, i+32..i+39), 8 chunks per K / V row.
+template <int D>
 __global__ void __launch_bounds__(128)
 rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ positions,
                     const int32_t* __restrict__ slot_mapping, const __nv_bfloat16* __restrict__ cos_sin,
@@ -636,18 +638,19 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
   griddep_launch();
   griddep_wait();
   const int t = blockIdx.x;
-  const int head = blockIdx.y * 16 + (threadIdx.x >> 3);
-  const int c = threadIdx.x & 7;  // chunk of 8 pairs: dims [8c, 8c+8) and [64+8c, 64+8c+8)
+  constexpr int CH = D / 16;      // chunks per half of a head = threads per head
+  const int head = blockIdx.y * (128 / CH) + threadIdx.x / CH;
+  const int c = threadIdx.x % CH;  // chunk of 8 pairs: dims [8c, 8c+8) and [D/2+8c, D/2+8c+8)
   const int n_heads = n_q + 2 * n_kv;
   if (head >= n_heads) return;
-  __nv_bfloat16* h = qkv + ((size_t)t * n_heads + head) * HEAD_DIM;
+  __nv_bfloat16* h = qkv + ((size_t)t * n_heads + head) * D;
   const int slot = slot_mapping[t];
   BF8 lo = reinterpret_cast<const BF8*>(h)[c];
-  BF8 hi = reinterpret_cast<const BF8*>(h)[8 + c];
+  BF8 hi = reinterpret_cast<const BF8*>(h)[CH + c];
   if (head < n_q + n_kv) {
     const int pos = positions[t];
-    const BF8 cs = reinterpret_cast<const BF8*>(cos_sin + (size_t)pos * HEAD_DIM)[c];
-    const BF8 sn = reinterpret_cast<const BF8*>(cos_sin + (size_t)pos * HEAD_DIM + 64)[c];
+    const BF8 cs = reinterpret_cast<const BF8*>(cos_sin + (size_t)pos * D)[c];
+    const BF8 sn = reinterpret_cast<const BF8*>(cos_sin + (size_t)pos * D + D / 2)[c];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       const float x1 = __bfloat162float(lo.v[e]), x2 = __bfloat162float(hi.v[e]);
@@ -656,31 +659,35 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
       hi.v[e] = __float2bfloat16_rn(bf16_round(x2 * cc) + bf16_round(x1 * ss));
     }
     reinterpret_cast<BF8*>(h)[c] = lo;
-    reinterpret_cast<BF8*>(h)[8 + c] = hi;
+    reinterpret_cast<BF8*>(h)[CH + c] = hi;
     if (head >= n_q && slot >= 0) {
       const int kvh = head - n_q;
       const int blk = slot / KV_BLOCK, off = slot % KV_BLOCK;
-      BF8* kb = reinterpret_cast<BF8*>(k_cache + ((size_t)blk * n_kv + kvh) * (KV_BLOCK * HEAD_DIM));
+      BF8* kb = reinterpret_cast<BF8*>(k_cache + ((size_t)blk * n_kv + kvh) * (KV_BLOCK * D));
       kb[c * KV_BLOCK + off] = lo;        // K layout: [chunk = d/8][token][8]
-      kb[(8 + c) * KV_BLOCK + off] = hi;
+      kb[(CH + c) * KV_BLOCK + off] = hi;
     }
   } else if (slot >= 0) {
     const int kvh = head - n_q - n_kv;
     const int blk = slot / KV_BLOCK, off = slot % KV_BLOCK;
-    BF8* vb = reinterpret_cast<BF8*>(v_cache + ((size_t)blk * n_kv + kvh) * (KV_BLOCK * HEAD_DIM) + (size_t)off * HEAD_DIM);
+    BF8* vb = reinterpret_cast<BF8*>(v_cache + ((size_t)blk * n_kv + kvh) * (KV_BLOCK * D) + (size_t)off * D);
     vb[c ^ (off & 7)] = lo;               // V layout: [token][16-byte chunk ^ (token & 7)][8]
-    vb[(8 + c) ^ (off & 7)] = hi;
+    vb[(CH + c) ^ (off & 7)] = hi;
   }
 }
 
 cudaError_t rope_kvwrite_launch(__nv_bfloat16* qkv, const int32_t* positions, const int32_t* slot_mapping,
                                 const __nv_bfloat16* cos_sin, __nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int T,
-                                int n_q, int n_kv, cudaStream_t stream) {
+                                int n_q, int n_kv, cudaStream_t stream, int head_dim) {
   if (T <= 0) return cudaSuccess;
   const int n_heads = n_q + 2 * n_kv;
+  if (head_dim == 64)
+    return launch_k(rope_kvwrite_kernel<64>, dim3(T, (n_heads + 31) / 32), dim3(128), 0, stream, qkv, positions,
+                    slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv);
+  if (head_dim != 128) return cudaErrorInvalidValue;
   dim3 grid(T, (n_heads + 15) / 16);
-  return launch_k(rope_kvwrite_kernel, grid, dim3(128), 0, stream, qkv, positions, slot_mapping, cos_sin, k_cache, v_cache,
-                  n_q, n_kv);
+  return launch_k(rope_kvwrite_kernel<128>, grid, dim3(128), 0, stream, qkv, positions, slot_mapping, cos_sin, k_cache,
+                  v_cache, n_q, n_kv);
 }
 
 }  // namespace tgis

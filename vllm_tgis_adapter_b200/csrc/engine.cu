@@ -252,11 +252,14 @@ struct tgis_engine {
   DevBuf<bf16> w_arena;
   bf16 *embed = nullptr, *lm_head = nullptr, *final_norm = nullptr, *cos_sin = nullptr;
   bool lm_head_loaded = false, cos_sin_loaded = false;
+  bool rope_table_required = false;  // scaled RoPE: default_rope_table() is not this model's table
   // OPT (opt.cu): learned positions [max_model_len + 2, hidden], final LayerNorm bias; model head dim (64 or 128: every
   // head is zero-padded to the 128-dim attention tiles at load time); fp32 GEMM accumulators of the biased projections
   bool opt = false;
   bf16 *pos_embed = nullptr, *final_norm_b = nullptr;
-  int pos_rows = 0, model_head_dim = HEAD_DIM;
+  // model_head_dim: the checkpoint's head size (the softmax scale); kv_head_dim: the head size of the qkv rows, the rotary
+  // table and the KV tiles, i.e. of the kernels that run.  They differ for OPT only (64-dim heads zero-padded to 128).
+  int pos_rows = 0, model_head_dim = HEAD_DIM, kv_head_dim = HEAD_DIM;
   float attn_scale = 0.f;
   // Granite's scalars (tgis_engine_set_model_scalars; 1 = the Llama stack): embedding and residual multipliers, and the
   // scale of the bf16 logits the sampler sees (1 / logits_scaling)
@@ -470,11 +473,12 @@ struct tgis_engine {
     Vl = c.vocab / tp;
     Vpad = (c.vocab + 7) / 8 * 8;  // == vocab under tensor parallelism (tgis_engine_create)
     opt = c.arch == TGIS_ARCH_OPT;
-    model_head_dim = opt ? c.head_dim : HEAD_DIM;
+    model_head_dim = c.head_dim;
+    kv_head_dim = opt ? HEAD_DIM : c.head_dim;
     attn_scale = 1.0f / std::sqrt((float)model_head_dim);  // zero-padded head dims add nothing to q . k
     pos_rows = opt ? c.max_model_len + 2 : 0;
-    q_dim = nq * HEAD_DIM;
-    qkv_dim = (nq + 2 * nkv) * HEAD_DIM;
+    q_dim = nq * kv_head_dim;
+    qkv_dim = (nq + 2 * nkv) * kv_head_dim;
     bt_stride = (c.max_model_len + KV_BLOCK - 1) / KV_BLOCK;
     max_splits_cap = (c.max_model_len + DECODE_SPLIT - 1) / DECODE_SPLIT;
     bitmap_words = (c.vocab + 31) / 32;
@@ -501,7 +505,7 @@ struct tgis_engine {
     const size_t per_layer = (size_t)qkv_dim * H + H * q_dim + 2 * F * H + H * F + 2 * H;
     const size_t opt_extra = opt ? (size_t)pos_rows * H + H + L * ((size_t)qkv_dim + 4 * H + F) + 64 * (6 * L + 4) : 0;
     const size_t Vp = Vpad;
-    const size_t total = Vp * H /*embed*/ + Vp * H /*lm_head*/ + H /*norm*/ + (size_t)c.max_model_len * HEAD_DIM +
+    const size_t total = Vp * H /*embed*/ + Vp * H /*lm_head*/ + H /*norm*/ + (size_t)c.max_model_len * kv_head_dim +
                          L * per_layer + 64 * (6 * L + 8) + opt_extra;
     w_arena.alloc(total);
     if (opt) w_arena.zero();  // the padded head dims of q/k/v rows, out_proj columns and their biases stay zero
@@ -518,7 +522,7 @@ struct tgis_engine {
       CK(cudaMemset(lm_head + V * H, 0, (Vp - V) * H * sizeof(bf16)));
     }
     final_norm = take(H);
-    cos_sin = take((size_t)c.max_model_len * HEAD_DIM);
+    cos_sin = take((size_t)c.max_model_len * kv_head_dim);
     layers.resize(L);
     for (auto& l : layers) {
       l.wqkv = take((size_t)qkv_dim * H);
@@ -556,7 +560,7 @@ struct tgis_engine {
     if (c.max_loras > 0) {
       max_loras = c.max_loras;
       lora_R = c.max_lora_rank;
-      const size_t R = lora_R, Sl = max_loras, kvd = (size_t)nkv * HEAD_DIM;
+      const size_t R = lora_R, Sl = max_loras, kvd = (size_t)nkv * kv_head_dim;
       const size_t per_layer = Sl * (R * H + q_dim * R + 2 * (R * H + kvd * R) + R * q_dim + H * R + 2 * R * H +
                                      (size_t)2 * F * 2 * R + R * F + H * R);
       lora_arena.alloc(per_layer * L);
@@ -590,7 +594,7 @@ struct tgis_engine {
     gemm_counters.alloc(1 << 16);
     gemm_counters.zero();
     const int G = c.n_q_heads / c.n_kv_heads;
-    part_o.alloc((size_t)S_max * nkv * max_splits_cap * G * HEAD_DIM);
+    part_o.alloc((size_t)S_max * nkv * max_splits_cap * G * kv_head_dim);
     part_ml.alloc((size_t)S_max * nkv * max_splits_cap * G * 2);
     samp_scratch.alloc((size_t)S_max * V);
     seen_bitmap.alloc((size_t)S_max * bitmap_words);
@@ -656,7 +660,7 @@ struct tgis_engine {
     }
 
     // ---- KV cache
-    const size_t block_elems = (size_t)nkv * KV_BLOCK * HEAD_DIM;  // per layer, per K or V (this rank's kv heads)
+    const size_t block_elems = (size_t)nkv * KV_BLOCK * kv_head_dim;  // per layer, per K or V (this rank's kv heads)
     size_t kv_bytes = c.kv_cache_bytes;
     if (kv_bytes == 0) {
       size_t free_b = 0, total_b = 0;
@@ -874,14 +878,14 @@ struct tgis_engine {
 
   void default_rope_table() {
     // HF LlamaRotaryEmbedding: inv_freq fp32, freqs = pos * inv_freq (fp32), cos/sin fp32 -> model dtype.
-    const int half = HEAD_DIM / 2;
-    std::vector<bf16> tab((size_t)cfg.max_model_len * HEAD_DIM);
+    const int hd = kv_head_dim, half = hd / 2;
+    std::vector<bf16> tab((size_t)cfg.max_model_len * hd);
     for (int pos = 0; pos < cfg.max_model_len; ++pos)
       for (int i = 0; i < half; ++i) {
-        const float inv = (float)(1.0 / std::pow((double)cfg.rope_theta, (double)(2 * i) / HEAD_DIM));
+        const float inv = (float)(1.0 / std::pow((double)cfg.rope_theta, (double)(2 * i) / hd));
         const float f = (float)pos * inv;
-        tab[(size_t)pos * HEAD_DIM + i] = __float2bfloat16_rn((float)std::cos((double)f));
-        tab[(size_t)pos * HEAD_DIM + half + i] = __float2bfloat16_rn((float)std::sin((double)f));
+        tab[(size_t)pos * hd + i] = __float2bfloat16_rn((float)std::cos((double)f));
+        tab[(size_t)pos * hd + half + i] = __float2bfloat16_rn((float)std::sin((double)f));
       }
     CK(cudaMemcpy(cos_sin, tab.data(), tab.size() * sizeof(bf16), cudaMemcpyHostToDevice));
   }
@@ -974,7 +978,7 @@ struct tgis_engine {
     if (name == "model.embed_tokens.weight") full(embed, V, H);
     else if (name == "lm_head.weight") { rows_shard(lm_head, V, H, Vl); lm_head_loaded = true; }
     else if (name == "model.norm.weight") full(final_norm, H, 1);
-    else if (name == "tgis.rope_cos_sin") { full(cos_sin, c.max_model_len, HEAD_DIM); cos_sin_loaded = true; }
+    else if (name == "tgis.rope_cos_sin") { full(cos_sin, c.max_model_len, kv_head_dim); cos_sin_loaded = true; }
     else if (name.rfind("model.layers.", 0) == 0) {
       const size_t dot = name.find('.', 13);
       if (dot == std::string::npos) return fail("bad weight name " + name);
@@ -982,11 +986,11 @@ struct tgis_engine {
       if (li < 0 || li >= c.n_layers) return fail("layer index out of range in " + name);
       LayerW& l = layers[li];
       const std::string sub = name.substr(dot + 1);
-      const int64_t kvd = (int64_t)nkv * HEAD_DIM;  // local
-      if (sub == "self_attn.q_proj.weight") rows_shard(l.wqkv, (int64_t)c.n_q_heads * HEAD_DIM, H, q_dim);
-      else if (sub == "self_attn.k_proj.weight") rows_shard(l.wqkv + (size_t)q_dim * H, (int64_t)c.n_kv_heads * HEAD_DIM, H, kvd);
-      else if (sub == "self_attn.v_proj.weight") rows_shard(l.wqkv + (size_t)(q_dim + kvd) * H, (int64_t)c.n_kv_heads * HEAD_DIM, H, kvd);
-      else if (sub == "self_attn.o_proj.weight") cols_shard(l.wo, H, (int64_t)c.n_q_heads * HEAD_DIM, q_dim);
+      const int64_t kvd = (int64_t)nkv * kv_head_dim;  // local
+      if (sub == "self_attn.q_proj.weight") rows_shard(l.wqkv, (int64_t)c.n_q_heads * kv_head_dim, H, q_dim);
+      else if (sub == "self_attn.k_proj.weight") rows_shard(l.wqkv + (size_t)q_dim * H, (int64_t)c.n_kv_heads * kv_head_dim, H, kvd);
+      else if (sub == "self_attn.v_proj.weight") rows_shard(l.wqkv + (size_t)(q_dim + kvd) * H, (int64_t)c.n_kv_heads * kv_head_dim, H, kvd);
+      else if (sub == "self_attn.o_proj.weight") cols_shard(l.wo, H, (int64_t)c.n_q_heads * kv_head_dim, q_dim);
       // gate / up rows are INTERLEAVED in wgu (row 2j = gate_j, row 2j+1 = up_j) so the GEMM epilogue can fuse SwiGLU
       else if (sub == "mlp.gate_proj.weight") { rows_shard(l.wgu, F, H, Fl); interleave = 1; }
       else if (sub == "mlp.up_proj.weight") { rows_shard(l.wgu + H, F, H, Fl); interleave = 1; }
@@ -1022,7 +1026,7 @@ struct tgis_engine {
   }
   template <class Fn>
   void lora_for_each(int32_t slot, Fn fn) {
-    const size_t R = lora_R, H = cfg.hidden, F = Fl, kvd = (size_t)nkv * HEAD_DIM, s = (size_t)(slot - 1);
+    const size_t R = lora_R, H = cfg.hidden, F = Fl, kvd = (size_t)nkv * kv_head_dim, s = (size_t)(slot - 1);
     for (auto& ll : lora_layers) {
       fn(ll.A_q + s * R * H, R * H);              fn(ll.B_q + s * q_dim * R, (size_t)q_dim * R);
       fn(ll.A_k + s * R * H, R * H);              fn(ll.B_k + s * kvd * R, kvd * R);
@@ -1054,7 +1058,7 @@ struct tgis_engine {
     const std::string mod = rest.substr(0, dot2), which = rest.substr(dot2 + 1);
     if (which != "lora_A" && which != "lora_B") return fail("bad adapter weight name " + name);
     const bool isA = which == "lora_A";
-    const int64_t R = lora_R, H = cfg.hidden, F = Fl, kvd = (int64_t)nkv * HEAD_DIM, s = slot - 1;
+    const int64_t R = lora_R, H = cfg.hidden, F = Fl, kvd = (int64_t)nkv * kv_head_dim, s = slot - 1;
     LoraLayerW& ll = lora_layers[li];
     bf16* dst = nullptr;
     int64_t fin = 0, fout = 0, cap = R;   // module geometry; cap: rank capacity of the stored tensor (row length of B)
@@ -1096,6 +1100,9 @@ struct tgis_engine {
         throw CudaError("OPT checkpoint incomplete: " + std::to_string(opt_loaded.size()) + " of " + std::to_string(expected) +
                         " tensors loaded (embed_tokens, embed_positions, final_layer_norm.{weight,bias} and 16 per layer)");
     }
+    if (rope_table_required && !cos_sin_loaded)
+      throw CudaError("this model's rotary embedding is scaled (rope_scaling): load its table as tgis.rope_cos_sin before "
+                      "starting; the built-in table is the unscaled one");
     if (!lm_head_loaded)  // tie_word_embeddings (tp == 1: with the zero padding rows)
       CK(cudaMemcpy(lm_head, embed + (size_t)rank * Vl * cfg.hidden, (size_t)(tp == 1 ? Vpad : Vl) * cfg.hidden * sizeof(bf16),
                     cudaMemcpyDeviceToDevice));
@@ -1154,13 +1161,13 @@ struct tgis_engine {
     const int n_std = n_tiles - step_ctiles;
     if (n_std > 0) {
       CK(attn_prefill_launch(qkv.p, qkv_dim, kc, vc, d_seqs, ds<int32_t>(off_tileseq), ds<int32_t>(off_tileq0), n_std,
-                             d_bt, bt_stride, attn_out.p, q_dim, nq, nkv, scale, stream));
+                             d_bt, bt_stride, attn_out.p, q_dim, nq, nkv, scale, stream, kv_head_dim));
       ++n_launches;
     }
     if (step_ctiles > 0) {
       CK(attn_prefill_split_launch(qkv.p, qkv_dim, kc, vc, d_seqs, ds<int32_t>(off_tileseq) + n_std,
                                    ds<int32_t>(off_tileq0) + n_std, step_ctiles, d_bt, bt_stride, attn_out.p, q_dim, nq,
-                                   nkv, scale, stream));
+                                   nkv, scale, stream, kv_head_dim));
       ++n_launches;
     }
   }
@@ -1202,14 +1209,16 @@ struct tgis_engine {
     // add), so the fused epilogues are switched off for the step and the deltas land between the GEMM and its consumer
     const bool lora = (samp_complex & 4) != 0 && max_loras > 0;
     const int32_t* d_toklora = ds<int32_t>(off_toklora);
-    const int LR = lora_R, kvd = nkv * HEAD_DIM;
+    const int LR = lora_R, kvd = nkv * kv_head_dim;
     auto lora_apply = [&](const LoraGroup& g, const bf16* x, int ldx, bf16* y, int ldy) {
       CK(lora_shrink_launch(x, ldx, d_toklora, g, lora_v.p, T, stream));
       CK(lora_expand_launch(lora_v.p, d_toklora, g, y, ldy, T, stream));
       n_launches += 2;
     };
     if (lora) ++lora_steps;
-    const bool rope_fused = !lora && fuse_rope && !cfg.debug_gemm_ref && gemm_even_split(T, qkv_dim, H, num_sms) >= 2 &&
+    // (the fused epilogue exists for 128-dim heads only: 64-dim heads always take rope_kvwrite, one more launch per layer)
+    const bool rope_fused = !lora && fuse_rope && kv_head_dim == HEAD_DIM && !cfg.debug_gemm_ref &&
+                            gemm_even_split(T, qkv_dim, H, num_sms) >= 2 &&
                             T <= (qkv_cluster > 0 ? std::max(rope_fuse_max_t, rope_fuse_cluster_max_t) : rope_fuse_max_t);
     for (int li = 0; li < (opt ? 0 : c.n_layers); ++li) {  // Llama stack (OPT: opt_layers() above)
       LayerW& l = layers[li];
@@ -1241,14 +1250,14 @@ struct tgis_engine {
       bf16* vc = v_cache.p + (size_t)li * kv_layer_elems;
       if (!rope_fused) {
         CK(rope_kvwrite_launch(qkv.p, ds<int32_t>(off_pos), ds<int32_t>(off_slotmap), cos_sin, kc, vc, T, nq, nkv,
-                               stream));
+                               stream, kv_head_dim));
         ++n_launches;
       }
       if (n_dec > 0) {
         const int max_splits = (max_dec_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
         CK(attn_decode_launch(qkv.p, qkv_dim, kc, vc, ds<DecItem>(items_off(S)), n_dec * max_splits, d_seqs,
                               ds<int32_t>(off_decids), n_dec, max_splits, part_o.p, part_ml.p, attn_out.p, q_dim, nq,
-                              nkv, scale, num_sms, stream));
+                              nkv, scale, num_sms, stream, kv_head_dim));
         n_launches += max_splits > 1 ? 2 : 1;
       }
       if (n_tiles > 0) prefill_attention(kc, vc, scale, n_tiles);
@@ -2137,12 +2146,18 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
     if (cfg->hidden != cfg->n_q_heads * cfg->head_dim) return fail("OPT: hidden must be n_q_heads * head_dim");
     if (cfg->tp_size > 1) return fail("OPT runs on a single GPU only (tp_size must be 1)");
     if (cfg->max_loras > 0) return fail("OPT: LoRA adapter slots are not supported (max_loras must be 0)");
+  } else if (cfg->head_dim == 64) {
+    // the 64-dim kernels are exercised on a single GPU without adapters; the other combinations are refused until tested
+    if (cfg->tp_size > 1) return fail("head_dim 64 is supported on a single GPU only (tp_size must be 1)");
+    if (cfg->max_loras > 0) return fail("head_dim 64: LoRA adapter slots are not supported (max_loras must be 0)");
   } else if (cfg->head_dim != HEAD_DIM) {
-    return fail("head_dim must be 128");
+    return fail("head_dim must be 128 or 64");
   }
   if (cfg->n_kv_heads <= 0 || cfg->n_q_heads % cfg->n_kv_heads != 0) return fail("n_q_heads must be a multiple of n_kv_heads");
   const int G = cfg->n_q_heads / cfg->n_kv_heads;
   if (!(G == 1 || G == 2 || G == 3 || G == 4 || G == 8)) return fail("GQA group size must be 1, 2, 3, 4 or 8");
+  if (cfg->arch == TGIS_ARCH_LLAMA && cfg->head_dim == 64 && G == 3)
+    return fail("head_dim 64: GQA group size must be 1, 2, 4 or 8");
   if (cfg->hidden % 64 || cfg->ffn % 64) return fail("hidden/ffn must be multiples of 64");
   if (cfg->vocab < 1) return fail("vocab must be positive");
   if (cfg->hidden > 8192) return fail("hidden > 8192 unsupported");
@@ -2192,6 +2207,8 @@ int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, fl
   const bool llama = embedding_multiplier == 1.f && residual_multiplier == 1.f && attention_multiplier == 0.f &&
                      logit_scale == 1.f;
   if (e->opt && !llama) return fail("model scalars (Granite) apply to the Llama layer stack only, not OPT");
+  if (e->kv_head_dim != HEAD_DIM && !llama)
+    return fail("model scalars (Granite) need head_dim 128: Granite with 64-dim heads is not supported yet");
   // the tensor-parallel exchange kernels (ar_add_rmsnorm / ar2_add_rmsnorm) and the NCCL path's norm do not implement
   // the residual multiplier
   if (e->tp > 1 && residual_multiplier != 1.f)
@@ -2200,6 +2217,14 @@ int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, fl
   e->res_mult = residual_multiplier;
   e->logit_scale = logit_scale;
   e->attn_scale = attention_multiplier > 0.f ? attention_multiplier : 1.0f / std::sqrt((float)e->model_head_dim);
+  return 0;
+}
+
+int tgis_engine_require_rope_table(tgis_engine* e) {
+  if (!e) return fail("null engine");
+  if (e->started) return fail("the rotary table requirement must be set before tgis_engine_start");
+  if (e->opt) return fail("OPT has learned positions, no rotary table");
+  e->rope_table_required = true;
   return 0;
 }
 

@@ -145,6 +145,10 @@ cudaError_t gather_rows_launch(const __nv_bfloat16* x, const int32_t* rows, __nv
 //   K: [num_blocks][n_kv][HEAD_DIM/8][BLOCK][8] bf16  (8-dim chunk major: lanes=tokens read conflict-free 16 B)
 //   V: [num_blocks][n_kv][BLOCK][16 chunks ^ (tok&7)][8] bf16  (row-major with the 16-B chunk index XOR-swizzled)
 // one (block, kv_head) K or V tile is a contiguous BLOCK*HEAD_DIM*2 bytes.
+// The RoPE + KV writer and the attention kernels also exist for 64-dim heads (their trailing head_dim argument): the same
+// two layouts at half the width, K [8 chunks][BLOCK][8] and V [BLOCK][8 chunks ^ (tok&7)][8], 4 KiB per tile; qkv rows are
+// (n_q + 2 n_kv) * 64 and cos_sin rows cos(32) | sin(32).  Any other head_dim, or a (head_dim, group size) pair that is not
+// instantiated, returns cudaErrorInvalidValue.  The GEMM's fused RoPE epilogue (GemmRope) and opt.cu are 128 only.
 constexpr int KV_BLOCK = 32;
 constexpr int HEAD_DIM = 128;
 
@@ -152,7 +156,7 @@ constexpr int HEAD_DIM = 128;
 // cos_sin: [max_pos][128] bf16 = cos(64) | sin(64)   (vllm: rotary_embedding/base.py cache.to(dtype))
 cudaError_t rope_kvwrite_launch(__nv_bfloat16* qkv, const int32_t* positions, const int32_t* slot_mapping,
                                 const __nv_bfloat16* cos_sin, __nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int T,
-                                int n_q, int n_kv, cudaStream_t stream);
+                                int n_q, int n_kv, cudaStream_t stream, int head_dim = HEAD_DIM);
 
 // ---- attention.cu ------------------------------------------------------------------------------------------------
 struct AttnSeq {        // one entry per sequence scheduled this step (device array)
@@ -205,12 +209,13 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
                                const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits, float* part_o,
                                float* part_ml, __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                               int num_sms, cudaStream_t stream);
+                               int num_sms, cudaStream_t stream, int head_dim = HEAD_DIM);
 // Prefill / chunked prefill (q_len >= 1), causal over the paged cache.
 cudaError_t attn_prefill_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
                                 const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                 const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
-                                __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale, cudaStream_t stream);
+                                __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale, cudaStream_t stream,
+                                int head_dim = HEAD_DIM);
 // Split-context prefill: same arguments and result layout; one cluster of PF_CLUSTER CTAs per (tile, kv head), each
 // streaming a contiguous share of the tile's context, merged through distributed shared memory (attention.cu).
 constexpr int PF_CLUSTER = 8;
@@ -218,7 +223,7 @@ cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, cons
                                       const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                       const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
                                       __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                                      cudaStream_t stream);
+                                      cudaStream_t stream, int head_dim = HEAD_DIM);
 // Which prefill sequences the split-context kernel takes when prefix caching is on: a short query span over a long
 // context already in the cache (the shape of a prefix-cache hit).  A function of the sequence's own (q_len, kv_len)
 // only, never of the rest of the step, so a sequence's bits do not depend on what it is batched with.  Measured on an

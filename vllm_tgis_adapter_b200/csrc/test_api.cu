@@ -176,15 +176,22 @@ int tgis_k_silu_mul(const void* gate_up_dev, void* act_dev, int32_t T, int32_t f
   return 0;
 }
 
-int tgis_k_rope_kv(void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
-                   const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q, int32_t n_kv) {
+int tgis_k_rope_kv_hd(int32_t head_dim, void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
+                      const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q,
+                      int32_t n_kv) {
   Tmp<int32_t> pos, sm;
   KCK(pos.upload(positions_host, T));
   KCK(sm.upload(slot_mapping_host, T));
   KCK(rope_kvwrite_launch((bf16*)qkv_dev, pos.p, sm.p, (const bf16*)cos_sin_dev, (bf16*)k_cache_dev, (bf16*)v_cache_dev,
-                          T, n_q, n_kv, 0));
+                          T, n_q, n_kv, 0, head_dim));
   KCK(cudaDeviceSynchronize());
   return 0;
+}
+
+int tgis_k_rope_kv(void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
+                   const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q, int32_t n_kv) {
+  return tgis_k_rope_kv_hd(HEAD_DIM, qkv_dev, positions_host, slot_mapping_host, cos_sin_dev, k_cache_dev, v_cache_dev, T,
+                           n_q, n_kv);
 }
 
 // qkv projection with the fused RoPE + KV-scatter epilogue (in the cluster or the global split-tile reduction).  Returns 1
@@ -220,6 +227,7 @@ namespace {
 // synchronisation in between, as in the engine's step.
 struct AttnCall {
   int n_q = 0, n_kv = 0, n_dec = 0, n_tiles = 0, n_ctiles = 0, max_splits = 1, bt_stride = 0;
+  int head_dim = HEAD_DIM;  // set before prepare()
   Tmp<AttnSeq> seqs;
   Tmp<int32_t> dec, tseq, tq0, bt;
   Tmp<float> po, pml;
@@ -263,7 +271,7 @@ struct AttnCall {
     KCK(bt.upload(block_table_host, (size_t)bt_rows * bt_stride));
     max_splits = (max_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
     const size_t nd = n_dec ? n_dec : 1;
-    KCK(po.alloc(nd * n_kv * max_splits * G * HEAD_DIM));
+    KCK(po.alloc(nd * n_kv * max_splits * G * head_dim));
     KCK(pml.alloc(nd * n_kv * max_splits * G * 2));
     std::vector<DecItem> h_items(1 + nd * max_splits);
     decode_items_build(h_items.data(), h_seqs.data(), h_dec.data(), n_dec, block_table_host, bt_stride);
@@ -273,41 +281,56 @@ struct AttnCall {
   // decode (+ split merge), then prefill, then split-context prefill: the engine's order
   int launch(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, void* out_dev, float scale,
              cudaStream_t st, bool decode = true) {
-    const int qkv_ld = (n_q + 2 * n_kv) * HEAD_DIM, out_ld = n_q * HEAD_DIM;
+    const int qkv_ld = (n_q + 2 * n_kv) * head_dim, out_ld = n_q * head_dim;
     if (decode)
       KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, items.p,
                              n_dec * max_splits, seqs.p, dec.p, n_dec, max_splits, po.p, pml.p, (bf16*)out_dev, out_ld,
-                             n_q, n_kv, scale, test_num_sms(), st));
+                             n_q, n_kv, scale, test_num_sms(), st, head_dim));
     const int n_std = n_tiles - n_ctiles;
     KCK(attn_prefill_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, seqs.p,
-                            tseq.p, tq0.p, n_std, bt.p, bt_stride, (bf16*)out_dev, out_ld, n_q, n_kv, scale, st));
+                            tseq.p, tq0.p, n_std, bt.p, bt_stride, (bf16*)out_dev, out_ld, n_q, n_kv, scale, st,
+                            head_dim));
     KCK(attn_prefill_split_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev,
                                   seqs.p, tseq.p + n_std, tq0.p + n_std, n_ctiles, bt.p, bt_stride, (bf16*)out_dev,
-                                  out_ld, n_q, n_kv, scale, st));
+                                  out_ld, n_q, n_kv, scale, st, head_dim));
     return 0;
   }
 };
 }  // namespace
 
-int tgis_k_attention(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, const int32_t* seqs_host,
-                     int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride, void* out_dev,
-                     int32_t n_q, int32_t n_kv, float scale) {
+int tgis_k_attention_split_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                              const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                              int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
+                              int32_t mode) {
+  if (mode < 0 || mode > 2) return kfail("mode must be 0 (existing prefill kernel), 1 (split-context) or 2 (selection)");
+  if (head_dim != 64 && head_dim != HEAD_DIM) return kfail("head_dim must be 64 or 128");
   AttnCall call;
-  if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv) != 0) return -1;
+  call.head_dim = head_dim;
+  if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv, mode) != 0) return -1;
   if (call.launch(qkv_dev, k_cache_dev, v_cache_dev, out_dev, scale, 0) != 0) return -1;
   KCK(cudaDeviceSynchronize());
   return 0;
 }
 
+int tgis_k_attention_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                        const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
+                        int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale) {
+  return tgis_k_attention_split_hd(head_dim, qkv_dev, k_cache_dev, v_cache_dev, seqs_host, n_seqs, block_table_host,
+                                   bt_rows, bt_stride, out_dev, n_q, n_kv, scale, 0);
+}
+
+int tgis_k_attention(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev, const int32_t* seqs_host,
+                     int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride, void* out_dev,
+                     int32_t n_q, int32_t n_kv, float scale) {
+  return tgis_k_attention_split_hd(HEAD_DIM, qkv_dev, k_cache_dev, v_cache_dev, seqs_host, n_seqs, block_table_host,
+                                   bt_rows, bt_stride, out_dev, n_q, n_kv, scale, 0);
+}
+
 int tgis_k_attention_split(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
                            const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
                            int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale, int32_t mode) {
-  if (mode < 0 || mode > 2) return kfail("mode must be 0 (existing prefill kernel), 1 (split-context) or 2 (selection)");
-  AttnCall call;
-  if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv, mode) != 0) return -1;
-  if (call.launch(qkv_dev, k_cache_dev, v_cache_dev, out_dev, scale, 0) != 0) return -1;
-  KCK(cudaDeviceSynchronize());
-  return 0;
+  return tgis_k_attention_split_hd(HEAD_DIM, qkv_dev, k_cache_dev, v_cache_dev, seqs_host, n_seqs, block_table_host,
+                                   bt_rows, bt_stride, out_dev, n_q, n_kv, scale, mode);
 }
 
 // prefill attention only (decode sequences in seqs_host are skipped), timed: `iters` launches of the mode's prefill
@@ -393,13 +416,14 @@ int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, 
 
 // decode attention only, timed: `iters` launches rotating over `n_layers` cache copies (layer_stride_bytes apart) so that
 // a small batch does not simply sit in L2; us_out = average device time per launch
-int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
-                           const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
-                           int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale, int32_t n_layers,
-                           int64_t layer_stride_bytes, int32_t iters, float* us_out) {
+int tgis_k_attention_bench_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                              const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                              int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
+                              int32_t n_layers, int64_t layer_stride_bytes, int32_t iters, float* us_out) {
   if (n_kv <= 0 || n_q % n_kv) return kfail("bad head counts");
+  if (head_dim != 64 && head_dim != HEAD_DIM) return kfail("head_dim must be 64 or 128");
   const int G = n_q / n_kv;
-  const int qkv_ld = (n_q + 2 * n_kv) * HEAD_DIM, out_ld = n_q * HEAD_DIM;
+  const int qkv_ld = (n_q + 2 * n_kv) * head_dim, out_ld = n_q * head_dim;
   std::vector<AttnSeq> seqs(n_seqs);
   int max_kv = 1;
   for (int s = 0; s < n_seqs; ++s) {
@@ -413,7 +437,7 @@ int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const v
   KCK(d_seqs.upload(seqs.data(), n_seqs));
   KCK(d_bt.upload(block_table_host, (size_t)bt_rows * bt_stride));
   const int max_splits = (max_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
-  KCK(po.alloc((size_t)n_seqs * n_kv * max_splits * G * HEAD_DIM));
+  KCK(po.alloc((size_t)n_seqs * n_kv * max_splits * G * head_dim));
   KCK(pml.alloc((size_t)n_seqs * n_kv * max_splits * G * 2));
   std::vector<DecItem> items(1 + (size_t)n_seqs * max_splits);
   decode_items_build(items.data(), seqs.data(), nullptr, n_seqs, block_table_host, bt_stride);
@@ -430,7 +454,7 @@ int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const v
     const char* vc = (const char*)v_cache_dev + (size_t)l * layer_stride_bytes;
     KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)kc, (const bf16*)vc, d_items.p,
                            n_seqs * max_splits, d_seqs.p, nullptr, n_seqs, max_splits, po.p, pml.p, (bf16*)out_dev,
-                           out_ld, n_q, n_kv, scale, num_sms, 0));
+                           out_ld, n_q, n_kv, scale, num_sms, 0, head_dim));
   }
   KCK(cudaEventRecord(e1, 0));
   KCK(cudaDeviceSynchronize());
@@ -440,6 +464,15 @@ int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const v
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
   return 0;
+}
+
+int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                           const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
+                           int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale, int32_t n_layers,
+                           int64_t layer_stride_bytes, int32_t iters, float* us_out) {
+  return tgis_k_attention_bench_hd(HEAD_DIM, qkv_dev, k_cache_dev, v_cache_dev, seqs_host, n_seqs, block_table_host,
+                                   bt_rows, bt_stride, out_dev, n_q, n_kv, scale, n_layers, layer_stride_bytes, iters,
+                                   us_out);
 }
 
 // Host-only: the launch plan of the GEMM for a shape (pure functions of the shape; no GPU needed): token-tile size,

@@ -20,7 +20,10 @@ class ModelConfig:
     rms_eps carries the LayerNorm epsilon, rope_theta unused) -- include/tgis_engine.h TGIS_ARCH_*.
 
     Granite (GraniteForCausalLM) is arch "llama" with the four scalars of its config.json set; their defaults are the
-    Llama stack (tgis_engine_set_model_scalars)."""
+    Llama stack (tgis_engine_set_model_scalars).
+
+    arch "llama" takes head_dim 128 or 64 (Llama-3.2-1B; single GPU, no LoRA slots, no Granite scalars), and the
+    rope_type "llama3" frequency scaling of Llama-3.1 / 3.2 (rope_scaling_factor > 1; loader.rope_cos_sin)."""
 
     n_layers: int        # num_hidden_layers
     hidden: int          # hidden_size
@@ -38,6 +41,14 @@ class ModelConfig:
     residual_multiplier: float = 1.0    # Granite: r = bf16(r + bf16(x * m)) after o_proj and down_proj
     attention_multiplier: float = 0.0   # Granite: softmax scale; 0 = 1/sqrt(head_dim)
     logits_scaling: float = 1.0         # Granite: logits = bf16(logits * (1 / logits_scaling))
+    rope_scaling_factor: float = 0.0    # rope_scaling / rope_parameters of rope_type "llama3": factor (0 or 1 = unscaled)
+    rope_low_freq_factor: float = 1.0   # low_freq_factor
+    rope_high_freq_factor: float = 4.0  # high_freq_factor
+    rope_original_max_pos: int = 8192   # original_max_position_embeddings
+
+    @property
+    def rope_scaled(self) -> bool:
+        return self.rope_scaling_factor not in (0.0, 1.0)
 
     @property
     def is_granite(self) -> bool:
@@ -59,6 +70,19 @@ PRESETS: dict[str, ModelConfig] = {
                              max_model_len=8192),
     "llama3-70b": ModelConfig(n_layers=80, hidden=8192, n_q_heads=64, n_kv_heads=8, ffn=28672, vocab=128256,
                               max_model_len=8192),
+    # Llama-3.1 / 3.2: rope_type "llama3" frequency scaling; 3.2-1B has 64-dim heads and tied embeddings
+    "llama3.1-8b": ModelConfig(n_layers=32, hidden=4096, n_q_heads=32, n_kv_heads=8, ffn=14336, vocab=128256,
+                               max_model_len=8192, rope_scaling_factor=8.0, rope_low_freq_factor=1.0,
+                               rope_high_freq_factor=4.0, rope_original_max_pos=8192),
+    "llama3.2-1b": ModelConfig(n_layers=16, hidden=2048, n_q_heads=32, n_kv_heads=8, ffn=8192, vocab=128256, head_dim=64,
+                               max_model_len=8192, tie_word_embeddings=True, rope_scaling_factor=32.0,
+                               rope_low_freq_factor=1.0, rope_high_freq_factor=4.0, rope_original_max_pos=8192),
+    # CPU-oracle-sized 64-dim-head stack; original_max_position_embeddings 64 puts its 32 rotary frequencies into all
+    # three bands of the llama3 rule and lets short prompts run past it
+    "llama-tiny-hd64": ModelConfig(n_layers=2, hidden=256, n_q_heads=4, n_kv_heads=2, ffn=512, vocab=1024, head_dim=64,
+                                   rope_theta=10000.0, max_model_len=2048, tie_word_embeddings=True,
+                                   rope_scaling_factor=8.0, rope_low_freq_factor=1.0, rope_high_freq_factor=4.0,
+                                   rope_original_max_pos=64),
     # Granite: a CPU-oracle-sized stack with an odd vocabulary and scalars that round (1/3 is not a power of two), and
     # the Granite 3.x 8B shape.  The granite-3-8b values are those of the published ibm-granite/granite-3.1-8b config.json
     # as recalled; they could not be checked against the file when this preset was written.
@@ -160,6 +184,8 @@ class NativeEngine:
                               "row-parallel exchange kernels do not implement the multiplier (use tensor_parallel_size 1)")
         if model.arch not in ("llama", "opt"):
             raise EngineError(f"unknown architecture {model.arch!r}")
+        if model.arch == "llama" and model.head_dim != 128 and model.is_granite:
+            raise EngineError(f"Granite with head_dim {model.head_dim} is not supported yet (Granite needs head_dim 128)")
         cfg.arch = _lib.ARCH_OPT if model.arch == "opt" else _lib.ARCH_LLAMA
         self.max_loras, self.max_lora_rank = int(max_loras), int(max_lora_rank)
         self._h = C.c_void_p()
@@ -171,6 +197,16 @@ class NativeEngine:
             msg = _lib.last_error(self.lib)
             self.close()
             raise EngineError(f"tgis_engine_set_model_scalars failed: {msg}")
+        if model.arch == "llama" and model.rope_scaled:
+            # the engine's built-in rotary table is the unscaled one: mark the table as required (start fails without it)
+            # and load the scaled one here, so that every way of building an engine gets it
+            if self.lib.tgis_engine_require_rope_table(self._h) != 0:
+                msg = _lib.last_error(self.lib)
+                self.close()
+                raise EngineError(f"tgis_engine_require_rope_table failed: {msg}")
+            from .rope import rope_cos_sin
+
+            self.load_weight("tgis.rope_cos_sin", rope_cos_sin(model))
         self.enable_prefix_caching = bool(enable_prefix_caching)
         if self.enable_prefix_caching and self.lib.tgis_engine_set_prefix_caching(self._h, 1) != 0:
             msg = _lib.last_error(self.lib)

@@ -13,6 +13,7 @@ from pathlib import Path
 
 from .async_engine import AsyncTGISEngine
 from .core import PRESETS, ModelConfig, NativeEngine
+from .rope import rope_cos_sin, rope_inv_freq  # noqa: F401  (the table every Llama engine is given: rope.py)
 from .tokenizer import load_tokenizer
 
 logger = logging.getLogger("vllm_tgis_adapter.engine")
@@ -30,17 +31,37 @@ def model_config_from_hf(path: Path, max_model_len: int | None) -> ModelConfig:
                          "decoders (RMSNorm, RoPE, GQA, SwiGLU) and OPT are implemented")
     hidden, heads = cfg["hidden_size"], cfg["num_attention_heads"]
     head_dim = cfg.get("head_dim") or hidden // heads
-    if head_dim != 128:
-        raise ValueError(f"head_dim {head_dim} unsupported (kernels are specialised for 128)")
-    if cfg.get("rope_scaling"):
-        raise ValueError("rope_scaling is not supported yet")
+    if head_dim not in (64, 128):
+        raise ValueError(f"head_dim {head_dim} unsupported (the attention kernels exist for 64 and 128)")
+    theta, scaling = _llama_rope(cfg)
     derived = cfg.get("max_position_embeddings", 8192)
     if max_model_len is not None and max_model_len > derived:
         raise ValueError(f"max_model_len {max_model_len} exceeds the model's max_position_embeddings {derived}")
     return ModelConfig(n_layers=cfg["num_hidden_layers"], hidden=hidden, n_q_heads=heads,
                        n_kv_heads=cfg.get("num_key_value_heads", heads), ffn=cfg["intermediate_size"],
-                       vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=float(cfg.get("rope_theta", 10000.0)),
-                       rms_eps=float(cfg.get("rms_norm_eps", 1e-5)), max_model_len=max_model_len or min(derived, 8192))
+                       vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=theta,
+                       rms_eps=float(cfg.get("rms_norm_eps", 1e-5)), max_model_len=max_model_len or min(derived, 8192),
+                       tie_word_embeddings=bool(cfg.get("tie_word_embeddings", False)), **scaling)
+
+
+def _llama_rope(cfg: dict) -> tuple[float, dict]:
+    """(rope_theta, ModelConfig rope_* fields) of a Llama config.json, from either spelling: `rope_scaling` beside a
+    top-level `rope_theta` (transformers 4), or `rope_parameters` holding both (transformers 5).  Only the default rotary
+    embedding and rope_type "llama3" (Llama-3.1 / 3.2) are implemented; every other type is refused by name."""
+    rope = cfg.get("rope_parameters") or cfg.get("rope_scaling") or {}
+    theta = float(rope.get("rope_theta") or cfg.get("rope_theta") or 10000.0)
+    kind = rope.get("rope_type") or rope.get("type") or "default"
+    if kind == "default":
+        return theta, {}
+    if kind != "llama3":
+        raise ValueError(f"rope scaling type {kind!r} is not supported (only 'default' and 'llama3' are implemented)")
+    missing = [k for k in ("factor", "low_freq_factor", "high_freq_factor", "original_max_position_embeddings")
+               if k not in rope]
+    if missing:
+        raise ValueError(f"rope scaling type 'llama3' needs {', '.join(missing)}")
+    return theta, dict(rope_scaling_factor=float(rope["factor"]), rope_low_freq_factor=float(rope["low_freq_factor"]),
+                       rope_high_freq_factor=float(rope["high_freq_factor"]),
+                       rope_original_max_pos=int(rope["original_max_position_embeddings"]))
 
 
 def _granite_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
@@ -104,16 +125,6 @@ def _opt_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
                        max_model_len=max_model_len or derived, arch="opt")
 
 
-def rope_cos_sin(mc: ModelConfig):
-    """HF LlamaRotaryEmbedding / vllm rotary_embedding base.py: fp32 table -> bf16."""
-    import torch
-
-    d = mc.head_dim
-    inv_freq = 1.0 / (mc.rope_theta ** (torch.arange(0, d, 2, dtype=torch.float32) / d))
-    freqs = torch.outer(torch.arange(mc.max_model_len, dtype=torch.float32), inv_freq)
-    return torch.cat([freqs.cos(), freqs.sin()], dim=-1).to(torch.bfloat16)
-
-
 def load_synthetic_weights(eng: NativeEngine, mc: ModelConfig, seed: int, device: int) -> None:
     import torch
 
@@ -151,7 +162,7 @@ def load_synthetic_weights(eng: NativeEngine, mc: ModelConfig, seed: int, device
     q_dim, kv_dim = mc.n_q_heads * mc.head_dim, mc.n_kv_heads * mc.head_dim
     ones = torch.ones(mc.hidden, dtype=torch.bfloat16, device=f"cuda:{device}")
     eng.load_weight("model.embed_tokens.weight", rnd(mc.vocab, mc.hidden))
-    if not mc.tie_word_embeddings:   # tied (Granite): the engine copies embed_tokens into the lm_head at start
+    if not mc.tie_word_embeddings:   # tied (Granite, Llama-3.2): the engine copies embed_tokens into the lm_head at start
         eng.load_weight("lm_head.weight", rnd(mc.vocab, mc.hidden))
     eng.load_weight("model.norm.weight", ones)
     for i in range(mc.n_layers):
