@@ -50,8 +50,10 @@ typedef struct tgis_engine tgis_engine;
  * vLLM pick the architecture from the checkpoint's config.json; the host-side loader does the same and passes it here.
  *   LLAMA: RMSNorm, neox RoPE, GQA, SwiGLU, no biases (BASELINE configs[1..4])
  *   OPT:   learned positions (offset 2), LayerNorm with bias, biased q/k/v/out/fc1/fc2, ReLU, tied lm_head,
- *          do_layer_norm_before = true, word_embed_proj_dim == hidden -- facebook/opt-125m, the reference's own test
- *          model (/root/reference/tests/conftest.py:79-91 (no --model: vLLM's default, facebook/opt-125m) and tests/test_hub.py:17; BASELINE configs[0]).  64-dim heads (head_dim = 64) run on the
+ *          do_layer_norm_before = true, word_embed_proj_dim == hidden -- facebook/opt-125m, which BASELINE configs[0]
+ *          names (and the reference's tests/test_hub.py:17).  The reference's integration tests start the server without
+ *          --model (tests/conftest.py:83-91), so they run vLLM's default model, which in vLLM 0.22 is Qwen/Qwen3-0.6B:
+ *          TGIS_ARCH_LLAMA with tgis_engine_set_qk_norm.  64-dim heads (head_dim = 64) run on the
  *          128-dim attention tiles: the engine zero-pads every head's q/k/v rows and out_proj columns at load time, which
  *          leaves every dot product unchanged.  Single GPU, no LoRA slots. */
 #define TGIS_ARCH_LLAMA 0
@@ -216,6 +218,14 @@ int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, fl
  * tgis_engine_start fails unless that table was loaded, instead of serving the built-in unscaled one.  Valid only between
  * tgis_engine_create and tgis_engine_start, TGIS_ARCH_LLAMA only. */
 int tgis_engine_require_rope_table(tgis_engine* e);
+/* Qwen3 (Qwen3ForCausalLM: the Llama layer stack plus an RMSNorm over each q head and each k head after the qkv
+ * projection, before RoPE; vllm model_executor/models/qwen3.py).  on != 0 allocates the per-layer vectors (2 x n_layers
+ * x 128 bf16, outside the weight arena) and makes "model.layers.{i}.self_attn.q_norm.weight" and ".k_norm.weight"
+ * (rows = 128, cols = 1) legal weight names; tgis_engine_start then fails, naming the layer, unless every layer has both.
+ * The norm uses tgis_config.rms_eps and rmsnorm's rounding points: y = bf16(bf16(x * rsqrt(mean(x^2) + eps)) * w).
+ * TGIS_ARCH_LLAMA with head_dim 128 on a single GPU only.  Valid only between tgis_engine_create and tgis_engine_start;
+ * on = 0 turns it off again. */
+int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on);
 /* Automatic prefix caching (vLLM's enable_prefix_caching; default off here, on in vLLM).  Valid only between
  * tgis_engine_create and tgis_engine_start.  A full 32-token KV block that a completed step wrote is keyed by (its
  * parent's key, its 32 token ids, LoRA slot + the slot's generation, bumped by every clear / weight load of the slot);

@@ -86,6 +86,13 @@ int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, 
 int tgis_k_rope_kv_hd(int32_t head_dim, void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
                       const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q,
                       int32_t n_kv);
+/* tgis_k_rope_kv with Qwen3's per-head RMSNorm of q and k before the rotation (head_dim 128): q_norm_dev / k_norm_dev
+ * [128] bf16 and the model's rms_eps; both null = the plain writer.  The writer runs max(iters, 1) times in place on
+ * stream 0; us_out (may be null): mean microseconds per launch between CUDA events. */
+int tgis_k_rope_kv_qknorm(void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
+                          const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q,
+                          int32_t n_kv, const void* q_norm_dev, const void* k_norm_dev, float eps, int32_t iters,
+                          float* us_out);
 int tgis_k_attention_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
                         const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
                         int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale);

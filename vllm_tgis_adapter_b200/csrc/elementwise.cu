@@ -630,12 +630,30 @@ cudaError_t silu_mul_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, in
 // (i..i+7, i+64..i+71): every global access is a 16-byte vector, and 8 consecutive dims are exactly one chunk of the
 // K / V cache layouts, so the scatter is one 16-byte store per half.
 // D = 64: 32 heads x 4 threads, pairs (i..i+7, i+32..i+39), 8 chunks per K / V row.
-template <int D>
+//
+// QKNORM (Qwen3; D = 128 only): every q and k head is RMS-normalised over its 128 dims before the rotation, with
+// rmsnorm_kernel's rounding points: rs = rsqrtf(ss / 128 + eps), y = bf16(bf16(x * rs) * w), w = q_norm or k_norm [128].
+// The fp32 sum of squares ss has a fixed order: thread c (c = 0..7 of the head's 8) adds, starting from 0, the squares of
+// lo[0..7] and then of hi[0..7] (dims 8c..8c+7, then 64+8c..64+8c+7), one at a time; xor-shuffles over the 8 lanes at
+// distances 1, 2, 4 then give every lane ((s0 + s1) + (s2 + s3)) + ((s4 + s5) + (s6 + s7)).  A bf16 square is exact in
+// fp32, so a contraction into a fused multiply-add changes nothing.  RoPE then rotates y; V heads are not normalised.
+template <int D, bool QKNORM = false>
 __global__ void __launch_bounds__(128)
 rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ positions,
                     const int32_t* __restrict__ slot_mapping, const __nv_bfloat16* __restrict__ cos_sin,
-                    __nv_bfloat16* __restrict__ k_cache, __nv_bfloat16* __restrict__ v_cache, int n_q, int n_kv) {
+                    __nv_bfloat16* __restrict__ k_cache, __nv_bfloat16* __restrict__ v_cache, int n_q, int n_kv,
+                    const __nv_bfloat16* __restrict__ q_norm, const __nv_bfloat16* __restrict__ k_norm, float eps) {
+  static_assert(!QKNORM || D == 128, "the q / k norm variant exists for 128-dim heads");
   griddep_launch();
+  BF8 wlo, whi;  // QKNORM: this thread's 16 norm weights (static: read before the wait, as rmsnorm_kernel does)
+  if constexpr (QKNORM) {
+    const int head = blockIdx.y * 16 + threadIdx.x / 8;
+    if (head < n_q + n_kv) {
+      const BF8* w = reinterpret_cast<const BF8*>(head < n_q ? q_norm : k_norm);
+      wlo = w[threadIdx.x % 8];
+      whi = w[8 + threadIdx.x % 8];
+    }
+  }
   griddep_wait();
   const int t = blockIdx.x;
   constexpr int CH = D / 16;      // chunks per half of a head = threads per head
@@ -648,6 +666,32 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
   BF8 lo = reinterpret_cast<const BF8*>(h)[c];
   BF8 hi = reinterpret_cast<const BF8*>(h)[CH + c];
   if (head < n_q + n_kv) {
+    if constexpr (QKNORM) {
+      float ss = 0.f;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float f = __bfloat162float(lo.v[e]);
+        ss += f * f;
+      }
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float f = __bfloat162float(hi.v[e]);
+        ss += f * f;
+      }
+      // the lanes in this branch: the warp's first `groups` 8-lane groups (heads run q, k, v; V heads and the tail
+      // CTA's missing heads sit above them)
+      const int groups = min(n_q + n_kv - (int)(blockIdx.y * 16 + (threadIdx.x / 32) * 4), 4);
+      const unsigned mask = groups == 4 ? 0xffffffffu : (1u << (8 * groups)) - 1u;
+      ss += __shfl_xor_sync(mask, ss, 1);
+      ss += __shfl_xor_sync(mask, ss, 2);
+      ss += __shfl_xor_sync(mask, ss, 4);
+      const float rs = rsqrtf(ss / 128.f + eps);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        lo.v[e] = __float2bfloat16_rn(bf16_round(__bfloat162float(lo.v[e]) * rs) * __bfloat162float(wlo.v[e]));
+        hi.v[e] = __float2bfloat16_rn(bf16_round(__bfloat162float(hi.v[e]) * rs) * __bfloat162float(whi.v[e]));
+      }
+    }
     const int pos = positions[t];
     const BF8 cs = reinterpret_cast<const BF8*>(cos_sin + (size_t)pos * D)[c];
     const BF8 sn = reinterpret_cast<const BF8*>(cos_sin + (size_t)pos * D + D / 2)[c];
@@ -678,16 +722,23 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
 
 cudaError_t rope_kvwrite_launch(__nv_bfloat16* qkv, const int32_t* positions, const int32_t* slot_mapping,
                                 const __nv_bfloat16* cos_sin, __nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int T,
-                                int n_q, int n_kv, cudaStream_t stream, int head_dim) {
+                                int n_q, int n_kv, cudaStream_t stream, int head_dim, const __nv_bfloat16* q_norm,
+                                const __nv_bfloat16* k_norm, float eps) {
   if (T <= 0) return cudaSuccess;
   const int n_heads = n_q + 2 * n_kv;
+  const __nv_bfloat16* none = nullptr;
+  if (q_norm || k_norm) {
+    if (head_dim != 128 || !q_norm || !k_norm) return cudaErrorInvalidValue;
+    return launch_k(rope_kvwrite_kernel<128, true>, dim3(T, (n_heads + 15) / 16), dim3(128), 0, stream, qkv, positions,
+                    slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, q_norm, k_norm, eps);
+  }
   if (head_dim == 64)
     return launch_k(rope_kvwrite_kernel<64>, dim3(T, (n_heads + 31) / 32), dim3(128), 0, stream, qkv, positions,
-                    slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv);
+                    slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, none, none, 0.f);
   if (head_dim != 128) return cudaErrorInvalidValue;
   dim3 grid(T, (n_heads + 15) / 16);
   return launch_k(rope_kvwrite_kernel<128>, grid, dim3(128), 0, stream, qkv, positions, slot_mapping, cos_sin, k_cache,
-                  v_cache, n_q, n_kv);
+                  v_cache, n_q, n_kv, none, none, 0.f);
 }
 
 }  // namespace tgis

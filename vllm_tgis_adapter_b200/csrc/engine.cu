@@ -253,6 +253,11 @@ struct tgis_engine {
   bf16 *embed = nullptr, *lm_head = nullptr, *final_norm = nullptr, *cos_sin = nullptr;
   bool lm_head_loaded = false, cos_sin_loaded = false;
   bool rope_table_required = false;  // scaled RoPE: default_rope_table() is not this model's table
+  // Qwen3 (tgis_engine_set_qk_norm): layer l's q_norm [128] at qk_norm_w + 256 l, its k_norm 128 further, in an
+  // allocation of their own, so that the arena and the KV block count of every other model stay as they are;
+  // qk_norm_loaded: per layer, bit 0 = q_norm, bit 1 = k_norm
+  DevBuf<bf16> qk_norm_w;
+  std::vector<uint8_t> qk_norm_loaded;
   // OPT (opt.cu): learned positions [max_model_len + 2, hidden], final LayerNorm bias; model head dim (64 or 128: every
   // head is zero-padded to the 128-dim attention tiles at load time); fp32 GEMM accumulators of the biased projections
   bool opt = false;
@@ -997,6 +1002,11 @@ struct tgis_engine {
       else if (sub == "mlp.down_proj.weight") cols_shard(l.wd, H, F, Fl);
       else if (sub == "input_layernorm.weight") full(l.ln1, H, 1);
       else if (sub == "post_attention_layernorm.weight") full(l.ln2, H, 1);
+      else if (qk_norm_w.p && (sub == "self_attn.q_norm.weight" || sub == "self_attn.k_norm.weight")) {
+        const int k = sub[10] == 'k';
+        full(qk_norm_w.p + (size_t)li * 2 * HEAD_DIM + k * HEAD_DIM, HEAD_DIM, 1);
+        if (rows * cols == HEAD_DIM) qk_norm_loaded[li] |= 1 << k;
+      }
       else return fail("unknown layer weight " + name);
     } else {
       return fail("unknown weight " + name);
@@ -1103,6 +1113,11 @@ struct tgis_engine {
     if (rope_table_required && !cos_sin_loaded)
       throw CudaError("this model's rotary embedding is scaled (rope_scaling): load its table as tgis.rope_cos_sin before "
                       "starting; the built-in table is the unscaled one");
+    for (size_t li = 0; li < qk_norm_loaded.size(); ++li)
+      if (qk_norm_loaded[li] != 3)
+        throw CudaError("q/k norm (Qwen3) weights missing: layer " + std::to_string(li) + " has no " +
+                        (qk_norm_loaded[li] & 1 ? "" : "model.layers." + std::to_string(li) + ".self_attn.q_norm.weight ") +
+                        (qk_norm_loaded[li] & 2 ? "" : "model.layers." + std::to_string(li) + ".self_attn.k_norm.weight"));
     if (!lm_head_loaded)  // tie_word_embeddings (tp == 1: with the zero padding rows)
       CK(cudaMemcpy(lm_head, embed + (size_t)rank * Vl * cfg.hidden, (size_t)(tp == 1 ? Vpad : Vl) * cfg.hidden * sizeof(bf16),
                     cudaMemcpyDeviceToDevice));
@@ -1216,8 +1231,9 @@ struct tgis_engine {
       n_launches += 2;
     };
     if (lora) ++lora_steps;
-    // (the fused epilogue exists for 128-dim heads only: 64-dim heads always take rope_kvwrite, one more launch per layer)
-    const bool rope_fused = !lora && fuse_rope && kv_head_dim == HEAD_DIM && !cfg.debug_gemm_ref &&
+    // (the fused epilogue exists for 128-dim heads without a q/k norm only: 64-dim heads and Qwen3 always take
+    // rope_kvwrite, one more launch per layer)
+    const bool rope_fused = !lora && fuse_rope && kv_head_dim == HEAD_DIM && !qk_norm_w.p && !cfg.debug_gemm_ref &&
                             gemm_even_split(T, qkv_dim, H, num_sms) >= 2 &&
                             T <= (qkv_cluster > 0 ? std::max(rope_fuse_max_t, rope_fuse_cluster_max_t) : rope_fuse_max_t);
     for (int li = 0; li < (opt ? 0 : c.n_layers); ++li) {  // Llama stack (OPT: opt_layers() above)
@@ -1249,8 +1265,10 @@ struct tgis_engine {
       bf16* kc = k_cache.p + (size_t)li * kv_layer_elems;
       bf16* vc = v_cache.p + (size_t)li * kv_layer_elems;
       if (!rope_fused) {
+        // Qwen3: the q / k norm runs on the raw projections, LoRA deltas included (vllm models/qwen3.py)
+        const bf16* qn = qk_norm_w.p ? qk_norm_w.p + (size_t)li * 2 * HEAD_DIM : nullptr;
         CK(rope_kvwrite_launch(qkv.p, ds<int32_t>(off_pos), ds<int32_t>(off_slotmap), cos_sin, kc, vc, T, nq, nkv,
-                               stream, kv_head_dim));
+                               stream, kv_head_dim, qn, qn ? qn + HEAD_DIM : nullptr, c.rms_eps));
         ++n_launches;
       }
       if (n_dec > 0) {
@@ -2225,6 +2243,29 @@ int tgis_engine_require_rope_table(tgis_engine* e) {
   if (e->started) return fail("the rotary table requirement must be set before tgis_engine_start");
   if (e->opt) return fail("OPT has learned positions, no rotary table");
   e->rope_table_required = true;
+  return 0;
+}
+
+int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on) {
+  if (!e) return fail("null engine");
+  if (e->started) return fail("the q/k norm must be set before tgis_engine_start");
+  if (!on) {
+    if (e->qk_norm_w.p) cudaFree(e->qk_norm_w.p);
+    e->qk_norm_w.p = nullptr;
+    e->qk_norm_loaded.clear();
+    return 0;
+  }
+  if (e->opt) return fail("q/k norm (Qwen3) applies to the Llama layer stack only, not OPT");
+  if (e->kv_head_dim != HEAD_DIM) return fail("q/k norm (Qwen3) needs head_dim 128");
+  if (e->tp > 1) return fail("q/k norm (Qwen3) is supported on a single GPU only (tp_size must be 1)");
+  if (e->qk_norm_w.p) return 0;
+  try {
+    CK(cudaSetDevice(e->cfg.device));
+    e->qk_norm_w.alloc((size_t)2 * e->cfg.n_layers * HEAD_DIM);
+  } catch (const std::exception& ex) {
+    return fail(ex.what());
+  }
+  e->qk_norm_loaded.assign(e->cfg.n_layers, 0);
   return 0;
 }
 

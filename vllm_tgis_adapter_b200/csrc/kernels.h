@@ -154,9 +154,13 @@ constexpr int HEAD_DIM = 128;
 
 // neox RoPE on q,k in-place inside qkv[T, (nq+2nkv)*128] and scatter of k,v into the paged cache.
 // cos_sin: [max_pos][128] bf16 = cos(64) | sin(64)   (vllm: rotary_embedding/base.py cache.to(dtype))
+// q_norm / k_norm [128] (Qwen3, head_dim 128 only; both or neither): each q and k head is RMS-normalised with epsilon eps
+// before the rotation (vllm models/qwen3.py Qwen3Attention.forward)
 cudaError_t rope_kvwrite_launch(__nv_bfloat16* qkv, const int32_t* positions, const int32_t* slot_mapping,
                                 const __nv_bfloat16* cos_sin, __nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int T,
-                                int n_q, int n_kv, cudaStream_t stream, int head_dim = HEAD_DIM);
+                                int n_q, int n_kv, cudaStream_t stream, int head_dim = HEAD_DIM,
+                                const __nv_bfloat16* q_norm = nullptr, const __nv_bfloat16* k_norm = nullptr,
+                                float eps = 0.f);
 
 // ---- attention.cu ------------------------------------------------------------------------------------------------
 struct AttnSeq {        // one entry per sequence scheduled this step (device array)

@@ -23,7 +23,10 @@ class ModelConfig:
     Llama stack (tgis_engine_set_model_scalars).
 
     arch "llama" takes head_dim 128 or 64 (Llama-3.2-1B; single GPU, no LoRA slots, no Granite scalars), and the
-    rope_type "llama3" frequency scaling of Llama-3.1 / 3.2 (rope_scaling_factor > 1; loader.rope_cos_sin)."""
+    rope_type "llama3" frequency scaling of Llama-3.1 / 3.2 (rope_scaling_factor > 1; loader.rope_cos_sin).
+
+    Qwen3 (Qwen3ForCausalLM) is arch "llama" with qk_norm set: an RMSNorm over each q and k head before RoPE, with the
+    per-layer weights self_attn.q_norm / k_norm (tgis_engine_set_qk_norm; head_dim 128, single GPU)."""
 
     n_layers: int        # num_hidden_layers
     hidden: int          # hidden_size
@@ -45,6 +48,7 @@ class ModelConfig:
     rope_low_freq_factor: float = 1.0   # low_freq_factor
     rope_high_freq_factor: float = 4.0  # high_freq_factor
     rope_original_max_pos: int = 8192   # original_max_position_embeddings
+    qk_norm: bool = False               # Qwen3: per-head RMSNorm of q and k (self_attn.q_norm / k_norm)
 
     @property
     def rope_scaled(self) -> bool:
@@ -93,6 +97,18 @@ PRESETS: dict[str, ModelConfig] = {
                                 rope_theta=10000000.0, max_model_len=8192, tie_word_embeddings=True,
                                 embedding_multiplier=12.0, residual_multiplier=0.22, attention_multiplier=0.0078125,
                                 logits_scaling=16.0),
+    # Qwen3: a CPU-oracle-sized stack whose q width (4 x 128) is not its hidden size, with an odd vocabulary, and the
+    # Qwen3-0.6B and Qwen3-8B shapes.  The qwen3-0.6b / qwen3-8b values are those of the published Qwen/Qwen3-0.6B and
+    # Qwen/Qwen3-8B config.json files as recalled; they could not be checked against the files when these presets were
+    # written.
+    "qwen3-tiny": ModelConfig(n_layers=2, hidden=256, n_q_heads=4, n_kv_heads=2, ffn=512, vocab=1021,
+                              rope_theta=1000000.0, rms_eps=1e-6, max_model_len=2048, tie_word_embeddings=True,
+                              qk_norm=True),
+    "qwen3-0.6b": ModelConfig(n_layers=28, hidden=1024, n_q_heads=16, n_kv_heads=8, ffn=3072, vocab=151936,
+                              rope_theta=1000000.0, rms_eps=1e-6, max_model_len=8192, tie_word_embeddings=True,
+                              qk_norm=True),
+    "qwen3-8b": ModelConfig(n_layers=36, hidden=4096, n_q_heads=32, n_kv_heads=8, ffn=12288, vocab=151936,
+                            rope_theta=1000000.0, rms_eps=1e-6, max_model_len=8192, qk_norm=True),
 }
 
 
@@ -182,6 +198,9 @@ class NativeEngine:
         if model.residual_multiplier != 1.0 and tp_size > 1:
             raise EngineError("Granite (residual_multiplier != 1) is not supported with tensor parallelism: the "
                               "row-parallel exchange kernels do not implement the multiplier (use tensor_parallel_size 1)")
+        if model.qk_norm and tp_size > 1:
+            raise EngineError("Qwen3 (qk_norm) is not supported with tensor parallelism: the q/k norm is implemented on a "
+                              "single GPU only (use tensor_parallel_size 1)")
         if model.arch not in ("llama", "opt"):
             raise EngineError(f"unknown architecture {model.arch!r}")
         if model.arch == "llama" and model.head_dim != 128 and model.is_granite:
@@ -207,6 +226,10 @@ class NativeEngine:
             from .rope import rope_cos_sin
 
             self.load_weight("tgis.rope_cos_sin", rope_cos_sin(model))
+        if model.qk_norm and self.lib.tgis_engine_set_qk_norm(self._h, 1) != 0:
+            msg = _lib.last_error(self.lib)
+            self.close()
+            raise EngineError(f"tgis_engine_set_qk_norm failed: {msg}")
         self.enable_prefix_caching = bool(enable_prefix_caching)
         if self.enable_prefix_caching and self.lib.tgis_engine_set_prefix_caching(self._h, 1) != 0:
             msg = _lib.last_error(self.lib)

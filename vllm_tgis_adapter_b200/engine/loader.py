@@ -26,6 +26,8 @@ def model_config_from_hf(path: Path, max_model_len: int | None) -> ModelConfig:
         return _opt_model_config(cfg, max_model_len)
     if cfg.get("model_type") == "granite" or "GraniteForCausalLM" in archs:
         return _granite_model_config(cfg, max_model_len)
+    if cfg.get("model_type") == "qwen3" or "Qwen3ForCausalLM" in archs:
+        return _qwen3_model_config(cfg, max_model_len)
     if cfg.get("model_type") != "llama" and not any("Llama" in a for a in archs):
         raise ValueError(f"unsupported model architecture {archs or cfg.get('model_type')}: only Llama-family "
                          "decoders (RMSNorm, RoPE, GQA, SwiGLU) and OPT are implemented")
@@ -95,6 +97,35 @@ def _granite_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
                        residual_multiplier=float(cfg.get("residual_multiplier", 1.0)),
                        attention_multiplier=float(cfg.get("attention_multiplier") or 0.0),
                        logits_scaling=float(cfg.get("logits_scaling", 1.0)))
+
+
+def _qwen3_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
+    """Qwen/Qwen3-* Qwen3ForCausalLM config.json -> the Llama stack plus the per-head q / k RMSNorm (vllm
+    model_executor/models/qwen3.py).  Variants the engine would serve wrongly are refused, each with its reason; the
+    rotary embedding is read as for Llama (_llama_rope: yarn and the other scaled types are refused by name)."""
+    hidden, heads = cfg["hidden_size"], cfg["num_attention_heads"]
+    head_dim = cfg.get("head_dim") or hidden // heads
+    problems = []
+    if cfg.get("attention_bias"):
+        problems.append("attention_bias (the Llama stack has no projection biases)")
+    if cfg.get("use_sliding_window"):
+        problems.append("use_sliding_window (every layer attends to the whole context here)")
+    other = sorted({t for t in cfg.get("layer_types") or [] if t != "full_attention"})
+    if other:
+        problems.append(f"layer_types {other} (only full_attention is implemented)")
+    if head_dim != 128:
+        problems.append(f"head_dim {head_dim} (the q/k norm is implemented for 128-dim heads)")
+    if problems:
+        raise ValueError("unsupported Qwen3 variant: " + "; ".join(problems))
+    theta, scaling = _llama_rope(cfg)
+    derived = cfg.get("max_position_embeddings", 40960)
+    if max_model_len is not None and max_model_len > derived:
+        raise ValueError(f"max_model_len {max_model_len} exceeds the model's max_position_embeddings {derived}")
+    return ModelConfig(n_layers=cfg["num_hidden_layers"], hidden=hidden, n_q_heads=heads,
+                       n_kv_heads=cfg.get("num_key_value_heads", heads), ffn=cfg["intermediate_size"],
+                       vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=theta,
+                       rms_eps=float(cfg.get("rms_norm_eps", 1e-6)), max_model_len=max_model_len or min(derived, 8192),
+                       tie_word_embeddings=bool(cfg.get("tie_word_embeddings", False)), qk_norm=True, **scaling)
 
 
 def _opt_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
@@ -176,6 +207,9 @@ def load_synthetic_weights(eng: NativeEngine, mc: ModelConfig, seed: int, device
         eng.load_weight(p + "mlp.down_proj.weight", rnd(mc.hidden, mc.ffn))
         eng.load_weight(p + "input_layernorm.weight", ones)
         eng.load_weight(p + "post_attention_layernorm.weight", ones)
+        if mc.qk_norm:   # Qwen3: per-head norm weights of one head's width
+            eng.load_weight(p + "self_attn.q_norm.weight", ones[:mc.head_dim])
+            eng.load_weight(p + "self_attn.k_norm.weight", ones[:mc.head_dim])
 
 
 def load_safetensors_dir(eng: NativeEngine, path: Path) -> None:
@@ -252,6 +286,8 @@ def build_engine(args) -> AsyncTGISEngine:
     tp = args.tensor_parallel_size or 1
     mc, path = _resolve_model(args)
     tp_kw = {}
+    if tp > 1 and mc.qk_norm:
+        raise ValueError(f"Qwen3 (per-head q/k norm) is supported on a single GPU only: tensor_parallel_size {tp}")
     if tp > 1:
         import multiprocessing as mp
         import os
