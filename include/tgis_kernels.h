@@ -127,6 +127,32 @@ int tgis_k_gemm_blocks_per_sm(int32_t T, int32_t lean, int32_t* out);
  * blocks[4]); record 0 holds the entry count; entries are listed longest first */
 int tgis_k_decode_items(const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_stride,
                         int32_t* items_out, int32_t capacity);
+/* Tensor-parallel exchange kernels (csrc/elementwise.cu), one rank per call, so that every rank can be run on one device.
+ * tgis_k_tp_area_bytes: bytes of one receive area for hidden (mode 1: one-shot, mode 2: two-shot).
+ * tgis_k_tp_exchange: rank `rank`'s exchange of mode 1 (one-shot push + rank-order sum + residual add + RMSNorm) or 2
+ *   (two-shot: reduce-scatter by row owner t mod tp, all-gather of the reduced rows, then the same norm).  partial_dev,
+ *   residual_dev, out_dev: bf16 [T, hidden] (residual updated in place); w_dev: bf16 [hidden]; areas_host[q]: device
+ *   address of rank q's receive area (areas_host[rank]: this rank's own), laid out as csrc/kernels.h documents.  The
+ *   exchange's epoch is epoch_base + epoch_idx (uint32 arithmetic).  Before launching, every line epoch word or flag the
+ *   kernel will wait for is checked to hold that epoch; if one does not, nothing is launched and the error names it.
+ * tgis_k_tp_exchange_check / tgis_k_logits_wait_check: that check alone (0: every line or flag is in place), never a
+ *   launch, so a test can show a refusal without any way to reach a kernel.
+ * tgis_k_logits_push: rank `rank` >= 1 of the vocab-parallel lm_head gather writes its bf16 shard [R, Vl] into columns
+ *   [rank * Vl, (rank + 1) * Vl) of dst_dev [R, V]; its last block raises *flag_dev = epoch (counter_dev: this rank's
+ *   int32 block counter, left at 0).  Vl and V multiples of 8.
+ * tgis_k_logits_wait: rank 0's wait for flags_dev[1 .. tp-1] == epoch (checked before launching, as above).
+ * tgis_k_gather_relayout: the NCCL fallback's re-layout, gathered [tp][R][Vl] bf16 -> out [R][tp * Vl]. */
+int tgis_k_tp_area_bytes(int32_t mode, int32_t hidden, int64_t* out);
+int tgis_k_tp_exchange(int32_t mode, int32_t tp, int32_t rank, const void* partial_dev, const uint64_t* areas_host,
+                       void* residual_dev, const void* w_dev, void* out_dev, int32_t T, int32_t hidden, float eps,
+                       uint32_t epoch_base, uint32_t epoch_idx);
+int tgis_k_logits_push(const void* shard_dev, void* dst_dev, int32_t R, int32_t Vl, int32_t V, int32_t rank,
+                       void* flag_dev, void* counter_dev, uint32_t epoch_base, uint32_t epoch_idx);
+int tgis_k_logits_wait(const void* flags_dev, int32_t tp, uint32_t epoch_base, uint32_t epoch_idx);
+int tgis_k_tp_exchange_check(int32_t mode, int32_t tp, int32_t rank, const uint64_t* areas_host, int32_t T,
+                             int32_t hidden, uint32_t epoch_base, uint32_t epoch_idx);
+int tgis_k_logits_wait_check(const void* flags_dev, int32_t tp, uint32_t epoch_base, uint32_t epoch_idx);
+int tgis_k_gather_relayout(const void* gathered_dev, void* out_dev, int32_t R, int32_t Vl, int32_t tp);
 /* decode-only, timed over `iters` launches rotating through n_layers cache copies; us_out = avg device us per launch */
 int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
                            const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,

@@ -267,7 +267,7 @@ ar_add_rmsnorm_kernel(ArPeers P, int tp, int rank, const uint32_t* __restrict__ 
   const int row = blockIdx.x;
   const size_t base = (size_t)row * hidden;
   const int nvec = hidden / 8;
-  // receive-area line index of (source rank, row, vector i): ((src * AR_MAX_ROWS + row) * nvec + i) * 2
+  // receive-area line index of (source rank, row, vector i): ar_line (kernels.h)
   uint4 own[NORM_MAX_VEC];
 #pragma unroll
   for (int j = 0; j < NORM_MAX_VEC; ++j) {
@@ -275,7 +275,7 @@ ar_add_rmsnorm_kernel(ArPeers P, int tp, int rank, const uint32_t* __restrict__ 
     if (i < nvec) {
       own[j] = reinterpret_cast<const uint4*>(P.own + base)[i];
       const uint4 l0 = make_uint4(own[j].x, epoch, own[j].y, epoch), l1 = make_uint4(own[j].z, epoch, own[j].w, epoch);
-      const size_t line = (((size_t)rank * AR_MAX_ROWS + row) * nvec + i) * 2;
+      const size_t line = ar_line(rank, row, nvec, i);
       for (int q = 0; q < tp; ++q) {
         if (q == rank) continue;
         st_volatile_v4(P.recv[q] + line, l0);
@@ -297,7 +297,7 @@ ar_add_rmsnorm_kernel(ArPeers P, int tp, int rank, const uint32_t* __restrict__ 
         if (q == rank) {
           raw = own[j];
         } else {
-          const uint4* src = P.recv[rank] + (((size_t)q * AR_MAX_ROWS + row) * nvec + i) * 2;
+          const uint4* src = P.recv[rank] + ar_line(q, row, nvec, i);
           uint4 l0, l1;
           const long long t0 = clock64();
           for (;;) {
@@ -371,8 +371,7 @@ cudaError_t ar_add_rmsnorm_launch(const ArPeers& peers, int tp, int rank, const 
 //   3. every rank adds the residual and normalises all rows (replicated, from its local copy of the reduced row).
 // Egress per rank: 2 (tp-1)/tp T H 2 bytes (7 MB in the example).  A row's CTA never waits for another row, so there is
 // no cross-row dependency to dead-lock on; the two parity areas alternate exactly like the one-shot kernel's.
-// Area layout (per rank, per parity):  recv1 [8 src][AR_MAX_ROWS][H] bf16 | recv2 [AR_MAX_ROWS][H] bf16 |
-//                                      flags1 [8 src][AR_MAX_ROWS] u32 | flags2 [AR_MAX_ROWS] u32
+// Area layout (per rank, per parity): kernels.h, beside ar2_area_bytes, with the offset helpers this kernel indexes it by
 __device__ __forceinline__ uint32_t ld_acquire_sys_u32(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.sys.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
@@ -406,16 +405,15 @@ ar2_add_rmsnorm_kernel(Ar2Peers P, int tp, int rank, const uint32_t* __restrict_
   const int owner = row % tp;
   const size_t base = (size_t)row * hidden;
   const int nvec = hidden / 8;
-  const size_t recv2_off = (size_t)8 * AR_MAX_ROWS * hidden * 2;
-  const size_t flags_off = (size_t)9 * AR_MAX_ROWS * hidden * 2;
+  const size_t recv2_off = ar2_recv2_off(hidden);
+  const size_t flags_off = ar2_flags_off(hidden);
   auto recv1 = [&](int q) { return reinterpret_cast<uint4*>(P.area[q]); };
   auto recv2 = [&](int q) { return reinterpret_cast<uint4*>(P.area[q] + recv2_off); };
-  auto flags1 = [&](int q) { return reinterpret_cast<uint32_t*>(P.area[q] + flags_off); };
-  auto flags2 = [&](int q) { return reinterpret_cast<uint32_t*>(P.area[q] + flags_off) + 8 * AR_MAX_ROWS; };
+  auto flags = [&](int q) { return reinterpret_cast<uint32_t*>(P.area[q] + flags_off); };
   uint4 sum[NORM_MAX_VEC];  // the reduced row, bf16
   if (owner != rank) {
     // ---- 1. my partial of this row -> the owner
-    uint4* dst = recv1(owner) + ((size_t)rank * AR_MAX_ROWS + row) * nvec;
+    uint4* dst = recv1(owner) + ar2_recv1_vec(rank, row, nvec);
 #pragma unroll
     for (int j = 0; j < NORM_MAX_VEC; ++j) {
       const int i = threadIdx.x + j * NORM_THREADS;
@@ -424,19 +422,19 @@ ar2_add_rmsnorm_kernel(Ar2Peers P, int tp, int rank, const uint32_t* __restrict_
     // publish: CTA barrier, then ONE system-scope release by thread 0 (cumulative over the barrier: covers every thread's
     // stores) -- no per-thread fence
     __syncthreads();
-    if (threadIdx.x == 0) st_release_sys_u32(flags1(owner) + rank * AR_MAX_ROWS + row, epoch);
+    if (threadIdx.x == 0) st_release_sys_u32(ar2_flag1(flags(owner), rank, row), epoch);
     // ---- 3a. wait for the reduced row
-    if (threadIdx.x == 0) spin_flag(flags2(rank) + row, epoch, rank, row, 2);
+    if (threadIdx.x == 0) spin_flag(ar2_flag2(flags(rank), row), epoch, rank, row, 2);
     __syncthreads();
 #pragma unroll
     for (int j = 0; j < NORM_MAX_VEC; ++j) {
       const int i = threadIdx.x + j * NORM_THREADS;
-      if (i < nvec) sum[j] = ld_volatile_v4(recv2(rank) + (size_t)row * nvec + i);
+      if (i < nvec) sum[j] = ld_volatile_v4(recv2(rank) + ar2_recv2_vec(row, nvec) + i);
     }
   } else {
     // ---- 2. owner: all partials of this row, summed in rank order
     if ((int)threadIdx.x < tp && (int)threadIdx.x != rank)
-      spin_flag(flags1(rank) + threadIdx.x * AR_MAX_ROWS + row, epoch, rank, row, 1);
+      spin_flag(ar2_flag1(flags(rank), threadIdx.x, row), epoch, rank, row, 1);
     __syncthreads();
 #pragma unroll
     for (int j = 0; j < NORM_MAX_VEC; ++j) {
@@ -447,7 +445,7 @@ ar2_add_rmsnorm_kernel(Ar2Peers P, int tp, int rank, const uint32_t* __restrict_
         for (int e = 0; e < 8; ++e) acc[e] = 0.f;
         for (int q = 0; q < tp; ++q) {
           const uint4 raw = (q == rank) ? reinterpret_cast<const uint4*>(P.own + base)[i]
-                                        : ld_volatile_v4(recv1(rank) + ((size_t)q * AR_MAX_ROWS + row) * nvec + i);
+                                        : ld_volatile_v4(recv1(rank) + ar2_recv1_vec(q, row, nvec) + i);
           const uint32_t* rw = &raw.x;
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
@@ -462,11 +460,11 @@ ar2_add_rmsnorm_kernel(Ar2Peers P, int tp, int rank, const uint32_t* __restrict_
           sw[e] = *reinterpret_cast<const uint32_t*>(&pr);
         }
         for (int q = 0; q < tp; ++q)
-          if (q != rank) recv2(q)[(size_t)row * nvec + i] = sum[j];
+          if (q != rank) recv2(q)[ar2_recv2_vec(row, nvec) + i] = sum[j];
       }
     }
     __syncthreads();
-    if ((int)threadIdx.x < tp && (int)threadIdx.x != rank) st_release_sys_u32(flags2(threadIdx.x) + row, epoch);
+    if ((int)threadIdx.x < tp && (int)threadIdx.x != rank) st_release_sys_u32(ar2_flag2(flags(threadIdx.x), row), epoch);
   }
   // ---- 3b. residual add + RMSNorm (arithmetic of rmsnorm_kernel<true> on the bf16 reduced row)
   BF8 z[NORM_MAX_VEC];
@@ -591,6 +589,29 @@ cudaError_t logits_push_launch(const void* shard, void* dst_peer0, int R, int Vl
 cudaError_t logits_wait_launch(const uint32_t* flags, int tp, const uint32_t* epoch_base, uint32_t epoch_idx,
                                cudaStream_t stream) {
   return launch_k(logits_wait_kernel, dim3(1), dim3(32), 0, stream, flags, tp, epoch_base, epoch_idx);
+}
+
+// The NCCL fallback of the same gather: after ncclAllGather of the shards, gathered: [tp][R][Vl] -> out: [R][tp*Vl],
+// elements moved as 16-byte vectors (Vl bytes % 16 == 0)
+__global__ void gather_relayout_kernel(const uint4* __restrict__ gathered, uint4* __restrict__ out, int R, int Vl16,
+                                       int tp) {
+  griddep_launch();
+  griddep_wait();
+  const size_t total = (size_t)tp * R * Vl16;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int rk = (int)(i / ((size_t)R * Vl16));
+    const size_t rem = i % ((size_t)R * Vl16);
+    const int r = (int)(rem / Vl16), v = (int)(rem % Vl16);
+    out[(size_t)r * tp * Vl16 + (size_t)rk * Vl16 + v] = gathered[i];
+  }
+}
+
+cudaError_t gather_relayout_launch(const void* gathered, void* out, int R, int Vl_bytes, int tp, int num_sms,
+                                   cudaStream_t stream) {
+  if (R <= 0) return cudaSuccess;
+  if (Vl_bytes % 16 || tp < 1) return cudaErrorInvalidValue;
+  return launch_k(gather_relayout_kernel, dim3(num_sms * 4), dim3(256), 0, stream, (const uint4*)gathered, (uint4*)out, R,
+                  Vl_bytes / 16, tp);
 }
 
 // ------------------------------------------------------------------------------------------------ SiLU * mul

@@ -185,20 +185,6 @@ struct ShmCtl {
 static_assert(sizeof(ShmCtl) <= 1024, "ShmCtl must fit below SHM_STAGE_OFF");
 constexpr size_t SHM_STAGE_OFF = 1024;
 
-// gathered: [tp][R][Vl] -> out: [R][tp*Vl], elements of `esz` bytes moved as 16-byte vectors (Vl * esz % 16 == 0)
-__global__ void gather_relayout_kernel(const uint4* __restrict__ gathered, uint4* __restrict__ out, int R, int Vl16,
-                                       int tp) {
-  griddep_launch();
-  griddep_wait();
-  const size_t total = (size_t)tp * R * Vl16;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int rk = (int)(i / ((size_t)R * Vl16));
-    const size_t rem = i % ((size_t)R * Vl16);
-    const int r = (int)(rem / Vl16), v = (int)(rem % Vl16);
-    out[(size_t)r * tp * Vl16 + (size_t)rk * Vl16 + v] = gathered[i];
-  }
-}
-
 // Prefix caching: the identity of a full KV block's content.  parent = uid of the cache entry of the block before it (0:
 // the first block of a sequence), so a key names the whole token prefix; the adapter is (LoRA slot, its generation).
 // Keys are compared field by field (all 32 token ids included): a hash collision can never give a wrong hit.
@@ -1417,8 +1403,7 @@ struct tgis_engine {
       gemm(xm_last, m_lm, last_hidden.p, lm_head, logits_shard.p, rows, Vl, H);
       NK(nccl().AllGather(logits_shard.p, logits_gather.p, (size_t)rows * Vl * sizeof(bf16), ncclInt8, comm, stream));
       if (rank == 0) {
-        CK(launch_k(gather_relayout_kernel, dim3(num_sms * 4), dim3(256), 0, stream, (const uint4*)logits_gather.p,
-                    (uint4*)logits.p, rows, (int)(Vl * sizeof(bf16) / 16), tp));
+        CK(gather_relayout_launch(logits_gather.p, logits.p, rows, (int)(Vl * sizeof(bf16)), tp, num_sms, stream));
         ++n_launches;
       }
     }

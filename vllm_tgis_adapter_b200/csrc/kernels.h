@@ -68,6 +68,11 @@ cudaError_t add_rmsnorm_launch(const __nv_bfloat16* x, __nv_bfloat16* residual, 
 // [hidden / 8 vectors][2 lines of 16 bytes = {data, epoch, data, epoch}].
 constexpr int AR_MAX_ROWS = 256;
 inline size_t ar_recv_bytes(int hidden) { return (size_t)8 * AR_MAX_ROWS * (hidden / 8) * 2 * 16; }
+// Index (in 16-byte lines) of the first of the two lines of (source rank src, row, vector i) in a receive area, nvec =
+// hidden / 8.  Shared by the kernel and the test hook's check of what it will wait for, so the two cannot disagree.
+__host__ __device__ __forceinline__ size_t ar_line(int src, int row, int nvec, int i) {
+  return (((size_t)src * AR_MAX_ROWS + row) * nvec + i) * 2;
+}
 struct ArPeers {
   const __nv_bfloat16* own;
   uint4* recv[8];
@@ -78,7 +83,24 @@ cudaError_t ar_add_rmsnorm_launch(const ArPeers& peers, int tp, int rank, const 
                                   float eps, cudaStream_t stream);
 // Two-shot variant (reduce-scatter by row owner t mod tp, all-gather of the bf16 reduced rows; elementwise.cu) for
 // exchanges whose one-shot egress would be large.  area[q]: rank q's two-shot area for this exchange parity, mapped here.
+// Area layout:  recv1 [8 src][AR_MAX_ROWS][hidden] bf16 | recv2 [AR_MAX_ROWS][hidden] bf16 |
+//               flags1 [8 src][AR_MAX_ROWS] u32 | flags2 [AR_MAX_ROWS] u32
 inline size_t ar2_area_bytes(int hidden) { return (size_t)9 * AR_MAX_ROWS * hidden * 2 + (size_t)9 * AR_MAX_ROWS * 4; }
+// Byte offsets of recv2 and of the flags (flags1, then flags2) inside an area
+__host__ __device__ __forceinline__ size_t ar2_recv2_off(int hidden) { return (size_t)8 * AR_MAX_ROWS * hidden * 2; }
+__host__ __device__ __forceinline__ size_t ar2_flags_off(int hidden) { return (size_t)9 * AR_MAX_ROWS * hidden * 2; }
+// 16-byte vector index in recv1 of the first vector of (source rank src, row); of row in recv2
+__host__ __device__ __forceinline__ size_t ar2_recv1_vec(int src, int row, int nvec) {
+  return ((size_t)src * AR_MAX_ROWS + row) * nvec;
+}
+__host__ __device__ __forceinline__ size_t ar2_recv2_vec(int row, int nvec) { return (size_t)row * nvec; }
+// flags1 word of (source rank src, row) and flags2 word of row, from the area's first flag word.  src is a template
+// parameter so that the kernel's unsigned threadIdx.x keeps its unsigned index arithmetic (and its SASS); hosts pass int.
+template <class S>
+__host__ __device__ __forceinline__ uint32_t* ar2_flag1(uint32_t* flags, S src, int row) {
+  return flags + src * AR_MAX_ROWS + row;
+}
+__host__ __device__ __forceinline__ uint32_t* ar2_flag2(uint32_t* flags, int row) { return flags + 8 * AR_MAX_ROWS + row; }
 struct Ar2Peers {
   const __nv_bfloat16* own;
   uint8_t* area[8];
@@ -93,6 +115,9 @@ cudaError_t logits_push_launch(const void* shard, void* dst_peer0, int R, int Vl
                                cudaStream_t stream);
 cudaError_t logits_wait_launch(const uint32_t* flags, int tp, const uint32_t* epoch_base, uint32_t epoch_idx,
                                cudaStream_t stream);
+// NCCL fallback of the same gather (elementwise.cu): gathered [tp][R][Vl] (ncclAllGather of the shards) -> out [R][tp * Vl]
+cudaError_t gather_relayout_launch(const void* gathered, void* out, int R, int Vl_bytes, int tp, int num_sms,
+                                   cudaStream_t stream);
 // logits[r, :vocab] = bf16(logits * scale) in place (bf16 logits; fp32 logits: fp32 product), rows of ld elements
 cudaError_t logits_scale_launch(void* logits, int logits_bf16, int ld, int vocab, int rows, float scale,
                                 cudaStream_t stream);

@@ -627,6 +627,138 @@ int tgis_k_decode_items(const int32_t* seqs_host, int32_t n_seqs, const int32_t*
                             bt_stride);
 }
 
+// ---- tensor-parallel exchange kernels, one rank at a time on one device.  The other ranks' receive areas are plain
+// device buffers here; what they would have pushed is staged by the caller.  Before launching, every line or flag the
+// kernel will poll is read back and must already hold this exchange's epoch: a staging mistake is an error return,
+// never a kernel spinning until its timeout.
+
+int tgis_k_tp_area_bytes(int32_t mode, int32_t hidden, int64_t* out) {
+  if (hidden <= 0 || hidden % 8) return kfail("hidden must be a positive multiple of 8");
+  if (mode == 1) *out = (int64_t)ar_recv_bytes(hidden);
+  else if (mode == 2) *out = (int64_t)ar2_area_bytes(hidden);
+  else return kfail("mode must be 1 (one-shot) or 2 (two-shot)");
+  return 0;
+}
+
+}  // extern "C"
+
+namespace {
+// What rank `rank`'s exchange kernel will wait for, read back: 0 when every line epoch word or flag holds the epoch,
+// else an error naming the first one that does not
+int tp_exchange_precheck(int mode, int tp, int rank, const uint64_t* areas_host, int T, int hidden, uint32_t epoch) {
+  if (mode != 1 && mode != 2) return kfail("mode must be 1 (one-shot) or 2 (two-shot)");
+  if (tp < 2 || tp > 8 || rank < 0 || rank >= tp) return kfail("need 2 <= tp <= 8 and 0 <= rank < tp");
+  if (T < 1 || T > AR_MAX_ROWS || hidden <= 0 || hidden % 8) return kfail("bad T or hidden");
+  const int nvec = hidden / 8;
+  const uint8_t* own_area = (const uint8_t*)areas_host[rank];
+  if (mode == 1) {
+    // lines of every other source, rows 0..T-1: one contiguous run of T * nvec line pairs per source
+    std::vector<uint4> lines((size_t)T * nvec * 2);
+    for (int q = 0; q < tp; ++q) {
+      if (q == rank) continue;
+      KCK(cudaMemcpy(lines.data(), (const uint4*)own_area + ar_line(q, 0, nvec, 0), lines.size() * sizeof(uint4),
+                     cudaMemcpyDeviceToHost));
+      for (int row = 0; row < T; ++row)
+        for (int i = 0; i < nvec; ++i) {
+          const uint4* l = lines.data() + (ar_line(q, row, nvec, i) - ar_line(q, 0, nvec, 0));
+          if (l[0].y != epoch || l[0].w != epoch || l[1].y != epoch || l[1].w != epoch)
+            return kfail("rank " + std::to_string(rank) + " would wait for source " + std::to_string(q) + " row " +
+                         std::to_string(row) + " vector " + std::to_string(i));
+        }
+    }
+    return 0;
+  }
+  std::vector<uint32_t> flags(9 * AR_MAX_ROWS);
+  KCK(cudaMemcpy(flags.data(), own_area + ar2_flags_off(hidden), flags.size() * sizeof(uint32_t),
+                 cudaMemcpyDeviceToHost));
+  for (int row = 0; row < T; ++row) {
+    const int owner = row % tp;
+    if (owner == rank) {
+      for (int q = 0; q < tp; ++q)
+        if (q != rank && *ar2_flag1(flags.data(), q, row) != epoch)
+          return kfail("rank " + std::to_string(rank) + " would wait for source " + std::to_string(q) + " row " +
+                       std::to_string(row) + " (partial flag)");
+    } else if (*ar2_flag2(flags.data(), row) != epoch) {
+      return kfail("rank " + std::to_string(rank) + " would wait for owner " + std::to_string(owner) + " row " +
+                   std::to_string(row) + " (reduced-row flag)");
+    }
+  }
+  return 0;
+}
+
+int logits_wait_precheck(const void* flags_dev, int tp, uint32_t epoch) {
+  if (tp < 2 || tp > 33) return kfail("need 2 <= tp <= 33");
+  std::vector<uint32_t> flags(tp);
+  KCK(cudaMemcpy(flags.data(), flags_dev, tp * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  for (int r = 1; r < tp; ++r)
+    if (flags[r] != epoch) return kfail("rank 0 would wait for rank " + std::to_string(r));
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int tgis_k_tp_exchange_check(int32_t mode, int32_t tp, int32_t rank, const uint64_t* areas_host, int32_t T,
+                             int32_t hidden, uint32_t epoch_base, uint32_t epoch_idx) {
+  return tp_exchange_precheck(mode, tp, rank, areas_host, T, hidden, epoch_base + epoch_idx);
+}
+
+int tgis_k_tp_exchange(int32_t mode, int32_t tp, int32_t rank, const void* partial_dev, const uint64_t* areas_host,
+                       void* residual_dev, const void* w_dev, void* out_dev, int32_t T, int32_t hidden, float eps,
+                       uint32_t epoch_base, uint32_t epoch_idx) {
+  if (tp_exchange_precheck(mode, tp, rank, areas_host, T, hidden, epoch_base + epoch_idx) != 0) return -1;
+  Tmp<uint32_t> base;
+  KCK(base.upload(&epoch_base, 1));
+  if (mode == 1) {
+    ArPeers P;
+    memset(&P, 0, sizeof(P));
+    P.own = (const bf16*)partial_dev;
+    for (int q = 0; q < tp; ++q) P.recv[q] = (uint4*)areas_host[q];
+    KCK(ar_add_rmsnorm_launch(P, tp, rank, base.p, epoch_idx, (bf16*)residual_dev, (const bf16*)w_dev, (bf16*)out_dev, T,
+                              hidden, eps, 0));
+  } else {
+    Ar2Peers P;
+    memset(&P, 0, sizeof(P));
+    P.own = (const bf16*)partial_dev;
+    for (int q = 0; q < tp; ++q) P.area[q] = (uint8_t*)areas_host[q];
+    KCK(ar2_add_rmsnorm_launch(P, tp, rank, base.p, epoch_idx, (bf16*)residual_dev, (const bf16*)w_dev, (bf16*)out_dev,
+                               T, hidden, eps, 0));
+  }
+  KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
+int tgis_k_logits_push(const void* shard_dev, void* dst_dev, int32_t R, int32_t Vl, int32_t V, int32_t rank,
+                       void* flag_dev, void* counter_dev, uint32_t epoch_base, uint32_t epoch_idx) {
+  if (R < 1 || Vl < 1 || V < Vl || rank < 1 || (int64_t)(rank + 1) * Vl > V) return kfail("bad shape or rank");
+  Tmp<uint32_t> base;
+  KCK(base.upload(&epoch_base, 1));
+  KCK(logits_push_launch(shard_dev, dst_dev, R, Vl * 2, V * 2, rank * Vl * 2, (uint32_t*)flag_dev, (int*)counter_dev,
+                         base.p, epoch_idx, 0));
+  KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
+int tgis_k_logits_wait_check(const void* flags_dev, int32_t tp, uint32_t epoch_base, uint32_t epoch_idx) {
+  return logits_wait_precheck(flags_dev, tp, epoch_base + epoch_idx);
+}
+
+int tgis_k_logits_wait(const void* flags_dev, int32_t tp, uint32_t epoch_base, uint32_t epoch_idx) {
+  if (logits_wait_precheck(flags_dev, tp, epoch_base + epoch_idx) != 0) return -1;
+  Tmp<uint32_t> base;
+  KCK(base.upload(&epoch_base, 1));
+  KCK(logits_wait_launch((const uint32_t*)flags_dev, tp, base.p, epoch_idx, 0));
+  KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
+int tgis_k_gather_relayout(const void* gathered_dev, void* out_dev, int32_t R, int32_t Vl, int32_t tp) {
+  if (R < 1 || Vl < 1 || tp < 1 || Vl % 8) return kfail("bad shape (Vl must be a multiple of 8)");
+  KCK(gather_relayout_launch(gathered_dev, out_dev, R, Vl * 2, tp, test_num_sms(), 0));
+  KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
 // logits_bf16 = 0: fp32 logits, 1: bf16 logits.  iters > 1: the launch is repeated and us_out (optional) receives the
 // average device time per launch (CUDA events on the launching stream).
 }  // extern "C"

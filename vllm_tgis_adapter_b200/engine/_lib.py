@@ -79,7 +79,8 @@ KERNEL_SYMBOLS = [
     "tgis_k_attention_bench", "tgis_k_decode_items", "tgis_k_gemm_plan", "tgis_k_gemm_schedule", "tgis_k_gemm_chain", "tgis_k_gemm_blocks_per_sm",
     "tgis_k_sampler", "tgis_k_sampler_ex", "tgis_k_sampler_masked", "tgis_k_sampler_scaled", "tgis_k_lora", "tgis_k_lora_bench", "tgis_k_silu_mul_interleaved", "tgis_k_sizeof_sample_row", "tgis_k_sizeof_sample_out", "tgis_k_kv_block",
     "tgis_k_rope_kv_hd", "tgis_k_attention_hd", "tgis_k_attention_split_hd", "tgis_k_attention_bench_hd",
-    "tgis_k_rope_kv_qknorm",
+    "tgis_k_rope_kv_qknorm", "tgis_k_tp_area_bytes", "tgis_k_tp_exchange", "tgis_k_logits_push", "tgis_k_logits_wait",
+    "tgis_k_gather_relayout", "tgis_k_tp_exchange_check", "tgis_k_logits_wait_check",
 ]
 
 _LIB: C.CDLL | None = None
@@ -168,6 +169,14 @@ def load_library() -> C.CDLL:
     lib.tgis_k_lora_bench.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, i32, C.POINTER(f32), C.POINTER(f32)]
     lib.tgis_k_sampler_masked.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, i32, C.POINTER(f32)]
     lib.tgis_k_sampler_scaled.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, f32]
+    u32 = C.c_uint32
+    lib.tgis_k_tp_area_bytes.argtypes = [i32, i32, C.POINTER(i64)]
+    lib.tgis_k_tp_exchange.argtypes = [i32, i32, i32, vp, C.POINTER(C.c_uint64), vp, vp, vp, i32, i32, f32, u32, u32]
+    lib.tgis_k_logits_push.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, u32, u32]
+    lib.tgis_k_logits_wait.argtypes = [vp, i32, u32, u32]
+    lib.tgis_k_tp_exchange_check.argtypes = [i32, i32, i32, C.POINTER(C.c_uint64), i32, i32, u32, u32]
+    lib.tgis_k_logits_wait_check.argtypes = [vp, i32, u32, u32]
+    lib.tgis_k_gather_relayout.argtypes = [vp, vp, i32, i32, i32]
     _LIB = lib
     return lib
 
