@@ -226,6 +226,13 @@ int tgis_engine_require_rope_table(tgis_engine* e);
  * TGIS_ARCH_LLAMA with head_dim 128 on a single GPU only.  Valid only between tgis_engine_create and tgis_engine_start;
  * on = 0 turns it off again. */
 int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on);
+/* Sliding-window attention in every layer (Mistral: config.json sliding_window; vLLM applies a model-wide window to each
+ * layer).  The query at position p attends to the keys at positions p - window < k <= p, window keys including itself;
+ * window = 0 (the default) attends to the whole context.  Decode, prefill, chunked prefill, prompt logprobs, the
+ * split-context prefill of prefix-cache hits and CUDA-graph replays all apply it.  KV blocks stay allocated for the whole
+ * sequence.  Refused: window < 0, TGIS_ARCH_OPT and tp_size > 1.  Valid only between tgis_engine_create and
+ * tgis_engine_start. */
+int tgis_engine_set_sliding_window(tgis_engine* e, int32_t window);
 /* Automatic prefix caching (vLLM's enable_prefix_caching; default off here, on in vLLM).  Valid only between
  * tgis_engine_create and tgis_engine_start.  A full 32-token KV block that a completed step wrote is keyed by (its
  * parent's key, its 32 token ids, LoRA slot + the slot's generation, bumped by every clear / weight load of the slot);

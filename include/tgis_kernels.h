@@ -104,6 +104,18 @@ int tgis_k_attention_bench_hd(int32_t head_dim, const void* qkv_dev, const void*
                               const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
                               int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
                               int32_t n_layers, int64_t layer_stride_bytes, int32_t iters, float* us_out);
+/* Sliding-window attention: tgis_k_attention_split_hd / tgis_k_attention_bench_hd with every query at position p
+ * attending to the keys p - window < k <= p (window = 0: the whole context, the calls above).  Decode lists only the
+ * splits holding a visible key and streams no block wholly below the window. */
+int tgis_k_attention_window(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                            const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
+                            int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale, int32_t mode,
+                            int32_t window);
+int tgis_k_attention_bench_window(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev,
+                                  const void* v_cache_dev, const int32_t* seqs_host, int32_t n_seqs,
+                                  const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride, void* out_dev,
+                                  int32_t n_q, int32_t n_kv, float scale, int32_t n_layers, int64_t layer_stride_bytes,
+                                  int32_t iters, float* us_out, int32_t window);
 /* host-only: GEMM launch plan for a shape: token tile (16..256), grid, even-split factor (0: stream-K + global fix-up) */
 int tgis_k_gemm_plan(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32_t* bt_out, int32_t* grid_out,
                      int32_t* even_split_out);
@@ -123,10 +135,15 @@ int tgis_k_gemm_schedule(int32_t T, int32_t N, int32_t K, int32_t num_sms, int32
 int tgis_k_gemm_chain(int32_t n, const int32_t* desc_host, const uint64_t* ptrs_host, int32_t* counters_left_out);
 /* CTAs per SM of the GEMM instantiation a T-token launch runs (lean = 0: the one-CTA-per-SM instantiation) */
 int tgis_k_gemm_blocks_per_sm(int32_t T, int32_t lean, int32_t* out);
-/* host-only: the decode work-item list of a step (csrc/kernels.h DecItem: q_row, kv_len, seq | split << 16, 0,
+/* host-only: the decode work-item list of a step (csrc/kernels.h DecItem: q_row, kv_len, seq | split << 16, lo,
  * blocks[4]); record 0 holds the entry count; entries are listed longest first */
 int tgis_k_decode_items(const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_stride,
                         int32_t* items_out, int32_t capacity);
+/* the same list under a sliding window (0: none, = tgis_k_decode_items): only the splits holding a position >= lo =
+ * max(0, kv_len - window); lo in the fourth field; the split holding lo past its first token sorts among the tails by
+ * its visible blocks (from the block holding lo) */
+int tgis_k_decode_items_window(const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                               int32_t bt_stride, int32_t* items_out, int32_t capacity, int32_t window);
 /* Tensor-parallel exchange kernels (csrc/elementwise.cu), one rank per call, so that every rank can be run on one device.
  * tgis_k_tp_area_bytes: bytes of one receive area for hidden (mode 1: one-shot, mode 2: two-shot).
  * tgis_k_tp_exchange: rank `rank`'s exchange of mode 1 (one-shot push + rank-order sum + residual add + RMSNorm) or 2

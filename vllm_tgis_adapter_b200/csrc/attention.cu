@@ -142,12 +142,15 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
     const int n_tok = min(DEC_TOK, it.y - (it.z >> 16) * DEC_TOK);
     return (n_tok + KV_BLOCK - 1) / KV_BLOCK;
   };
+  // Sliding window: it.w = lo, the first visible position (0 without a window).  The split holding lo starts at the
+  // block holding lo, so blocks wholly below the window are never requested; every other split starts at block 0.
+  auto blk0_of = [&](const int4& it) { return max(0, it.w - (it.z >> 16) * DEC_TOK) / KV_BLOCK; };
   auto pick = [](const int4& b, int j) { return j == 0 ? b.x : j == 1 ? b.y : j == 2 ? b.z : b.w; };
   const uint64_t kv_policy = policy_evict_first();
   int4 c_it = item_at(f);
   int4 c_nxt = c_it;
   // ---- issue cursor: runs DEC_RING tiles ahead of consumption, across item boundaries
-  int i_f = f, i_kvh = f % n_kv, i_jb = 0, i_nblk = n_blk_of(c_it), i_kv = 0, i_buf = 0;
+  int i_f = f, i_kvh = f % n_kv, i_jb = blk0_of(c_it), i_nblk = n_blk_of(c_it), i_kv = 0, i_buf = 0;
   int4 i_nxt = c_it, i_blks = blocks_at(f), i_blks_nxt = i_blks;  // block ids of the item being issued / the next one
   int4 i_cur = c_it;                                                // record of the item being issued
   int i_k = 0, c_k = 0;  // round of the issue cursor / of the consumer
@@ -173,7 +176,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
       i_f = item_of_round(++i_k);
       if (i_f >= n_flat) return;
       i_kvh = i_f % n_kv;
-      i_jb = 0;
+      i_jb = blk0_of(i_nxt);
       i_nblk = n_blk_of(i_nxt);
       i_cur = i_nxt;
       i_blks = i_blks_nxt;
@@ -220,6 +223,8 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
     const int n_splits = (kv_len + DEC_TOK - 1) / DEC_TOK;
     const int n_tok = min(DEC_TOK, kv_len - split * DEC_TOK);
     const int n_blk = (n_tok + KV_BLOCK - 1) / KV_BLOCK;
+    const int lo_tok = c_it.w - split * DEC_TOK;  // first visible token of the split (<= 0: all of them)
+    const int jb0 = blk0_of(c_it);
     const int f_next = item_of_round(c_k + 1);
     const bool has_next = f_next < n_flat;
     if (has_next) c_nxt = item_at(f_next);
@@ -239,7 +244,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
     for (int i = 0; i < D / 16; ++i) ot[i][0] = ot[i][1] = ot[i][2] = ot[i][3] = 0.f;
     float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};  // l_r: this thread's share (reduced at the end)
 
-    for (int jb = 0; jb < n_blk; ++jb) {
+    for (int jb = jb0; jb < n_blk; ++jb) {
       // ---- S^T = K Q^T : 2 m-tiles (16 tokens) x 8 k-steps (16 dims = chunks 2ks, 2ks+1); ldmatrix.x4 = one A
       // fragment: matrices (tok lo, chunk 2ks), (tok hi, chunk 2ks), (tok lo, chunk 2ks+1), (tok hi, chunk 2ks+1)
       mbar_wait(&full[c_buf], c_ph);
@@ -259,18 +264,21 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
       __syncwarp();
       issue_tile();  // refills the K buffer just consumed (tile t + DEC_RING of this warp's stream)
       if (++c_buf == DEC_RING) { c_buf = 0; c_ph ^= 1; }
-      if (jb == 0) {  // q_s was copied to registers above; by now the next item's record has arrived
+      if (jb == jb0) {  // q_s was copied to registers above; by now the next item's record has arrived
         __syncwarp();
         if (has_next) issue_q(c_nxt, f_next % n_kv);
       }
       // ---- online softmax; st[mt][e]: token mt*16 + hr + (e>>1)*8, head 2*t4 + (e&1)
+      // tokens [first, valid) of the block are visible: first > 0 only in the block holding lo
       const int valid = min(KV_BLOCK, n_tok - jb * KV_BLOCK);
+      const int first = lo_tok - jb * KV_BLOCK;
       float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          st[mt][e] = (mt * 16 + hr + (e >> 1) * 8 < valid) ? st[mt][e] * sl2 : -INFINITY;
+          const int tk = mt * 16 + hr + (e >> 1) * 8;
+          st[mt][e] = (tk < valid && tk >= first) ? st[mt][e] * sl2 : -INFINITY;
           mx[e & 1] = fmaxf(mx[e & 1], st[mt][e]);
         }
       float corr[2];
@@ -279,7 +287,9 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
         mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 4));
         mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 8));
         mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 16));
-        const float m_new = fmaxf(m_r[hh], mx[hh]);  // finite: token 0 of every block of the split is valid
+        // finite: every processed block holds a visible token.  The first block holds lo (or token 0 of the split),
+        // every later block holds its token 0, and a block starts below kv_len.
+        const float m_new = fmaxf(m_r[hh], mx[hh]);
         corr[hh] = (m_r[hh] == -INFINITY) ? 0.f : exp2f(m_r[hh] - m_new);
         m_r[hh] = m_new;
         l_r[hh] *= corr[hh];
@@ -338,8 +348,8 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
       l_r[hh] += __shfl_xor_sync(0xffffffffu, l_r[hh], 16);
     }
 
-    // ---- item epilogue
-    if (n_splits == 1) {
+    // ---- item epilogue: with one visible split the kernel writes the row itself
+    if (n_splits - c_it.w / DEC_TOK == 1) {
       __nv_bfloat16* o_dst = out + (size_t)c_it.x * out_ld + (size_t)(kvh * G + 2 * t4) * D + hr;
       const float inv[2] = {1.f / l_r[0], 1.f / l_r[1]};
 #pragma unroll
@@ -373,20 +383,22 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
   STL_EXIT();
 }
 
-// Split merge: one CTA per (decode sequence, kv head) with more than one split, thread = dim.  Reads the partials in
-// split order (deterministic), writes the normalised bf16 rows.
+// Split merge: one CTA per (decode sequence, kv head) with more than one visible split, thread = dim.  Reads the
+// partials of the visible splits (from the one holding lo = max(0, kv_len - window); window 0: all) in split order
+// (deterministic), writes the normalised bf16 rows.  The partials stay indexed by absolute split.
 template <int D, int G>
 __global__ void __launch_bounds__(D)
 attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ seq_ids, int max_splits,
                   const float* __restrict__ part_o, const float* __restrict__ part_ml,
-                  __nv_bfloat16* __restrict__ out, int out_ld, int n_kv) {
+                  __nv_bfloat16* __restrict__ out, int out_ld, int n_kv, int window) {
   __shared__ float ml_s[64 * G * 2];
   STL_ENTER(4);
   griddep_launch();
   const int sidx = blockIdx.x, kvh = blockIdx.y, d = threadIdx.x;
   const AttnSeq sq = seqs[seq_ids ? seq_ids[sidx] : sidx];  // host-written
   const int n_splits = (sq.kv_len + DEC_TOK - 1) / DEC_TOK;
-  if (n_splits == 1) return;  // the streaming kernel wrote the row itself
+  const int s0 = window > 0 ? max(0, sq.kv_len - window) / DEC_TOK : 0;  // first visible split
+  if (n_splits - s0 == 1) return;  // the streaming kernel wrote the row itself
   griddep_wait();
   STL_WAITED();
   const size_t pbase = (size_t)(sidx * n_kv + kvh) * max_splits;
@@ -394,7 +406,7 @@ attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ 
 #pragma unroll
   for (int g = 0; g < G; ++g) m_f[g] = -INFINITY, l_f[g] = 0.f, o_f[g] = 0.f;
   // pass 1: row maxima (the (m, l) pairs go through shared memory in chunks of 64 splits)
-  for (int c0 = 0; c0 < n_splits; c0 += 64) {
+  for (int c0 = s0; c0 < n_splits; c0 += 64) {
     const int nc = min(64, n_splits - c0);
     __syncthreads();
     for (int i = d; i < nc * G * 2; i += D) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
@@ -405,9 +417,9 @@ attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ 
   }
   // pass 2: weighted sums in split order, SPB splits of loads in flight per thread
   constexpr int SPB = 4;
-  for (int c0 = 0; c0 < n_splits; c0 += 64) {
+  for (int c0 = s0; c0 < n_splits; c0 += 64) {
     const int nc = min(64, n_splits - c0);
-    if (n_splits > 64) {
+    if (n_splits - s0 > 64) {
       __syncthreads();
       for (int i = d; i < nc * G * 2; i += D) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
       __syncthreads();
@@ -443,7 +455,7 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
                                    const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                    const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits,
                                    float* part_o, float* part_ml, __nv_bfloat16* out, int out_ld, int n_kv,
-                                   float scale, int num_sms, cudaStream_t stream) {
+                                   float scale, int num_sms, cudaStream_t stream, int window) {
   static bool attr = false;
   if (!attr) {
     cudaError_t e =
@@ -459,21 +471,21 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
                            k_cache, v_cache, items, max_splits, part_o, part_ml, out, out_ld, n_kv, scale, prefetch_old);
   if (e != cudaSuccess || max_splits <= 1) return e;
   return launch_k(attn_merge_kernel<D, G>, dim3(n_seqs, n_kv), dim3(D), 0, stream, seqs, seq_ids, max_splits,
-                  (const float*)part_o, (const float*)part_ml, out, out_ld, n_kv);
+                  (const float*)part_o, (const float*)part_ml, out, out_ld, n_kv, window);
 }
 
 cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
                                const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits, float* part_o,
                                float* part_ml, __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                               int num_sms, cudaStream_t stream, int head_dim) {
+                               int num_sms, cudaStream_t stream, int head_dim, int window) {
   if (max_entries <= 0 || n_seqs <= 0) return cudaSuccess;
-  if (n_q % n_kv != 0) return cudaErrorInvalidValue;
+  if (n_q % n_kv != 0 || window < 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
 #define TGIS_DEC(DD, GG)                                                                                      \
   case GG:                                                                                                    \
     return decode_launch_g<DD, GG>(qkv, qkv_ld, k_cache, v_cache, items, max_entries, seqs, seq_ids, n_seqs, \
-                                   max_splits, part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream)
+                                   max_splits, part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream, window)
   if (head_dim == 128) {
     switch (G) {
       TGIS_DEC(128, 1);
@@ -513,7 +525,7 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
                     const __nv_bfloat16* __restrict__ v_cache, const AttnSeq* __restrict__ seqs,
                     const int32_t* __restrict__ tile_seq, const int32_t* __restrict__ tile_q0,
                     const int32_t* __restrict__ block_table, int bt_stride, __nv_bfloat16* __restrict__ out,
-                    int out_ld, int n_kv, int G, float scale) {
+                    int out_ld, int n_kv, int G, float scale, int window) {
   __shared__ __align__(128) uint8_t kv_static[SPLIT ? 16 : 2 * 2 * TILE_BYTES<D>];  // 2 stages x (K | V)
   extern __shared__ __align__(128) uint8_t kv_dyn[];
   uint8_t* kv_s = SPLIT ? kv_dyn : kv_static;
@@ -528,9 +540,12 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   const int pos0 = sq.kv_len - sq.q_len + q0;        // absolute position of row 0
   const int last_pos = pos0 + n_rows - 1;
   const int n_blk = last_pos / KV_BLOCK + 1;
-  // blocks [jb0, jb1) of the causal range are this CTA's (all of them without SPLIT; may be empty with SPLIT)
-  const int jb0 = SPLIT ? crank * n_blk / PF_CLUSTER : 0;
-  const int jb1 = SPLIT ? (crank + 1) * n_blk / PF_CLUSTER : n_blk;
+  // sliding window (0: none): row p sees keys p - window < k <= p, so no row of the tile sees a block below blk_lo
+  const int blk_lo = window > 0 ? max(0, pos0 - window + 1) / KV_BLOCK : 0;
+  // blocks [jb0, jb1) of the visible range [blk_lo, n_blk) are this CTA's (all of them without SPLIT; may be empty
+  // with SPLIT)
+  const int jb0 = SPLIT ? blk_lo + crank * (n_blk - blk_lo) / PF_CLUSTER : blk_lo;
+  const int jb1 = SPLIT ? blk_lo + (crank + 1) * (n_blk - blk_lo) / PF_CLUSTER : n_blk;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int head = kvh * G + warp;
@@ -576,6 +591,9 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};
   const float sl2 = scale * 1.4426950408889634f;  // exp2 domain
   const int row_pos[2] = {pos0 + g, pos0 + g + 8};
+  // keys at or below row_lo are outside the row's window (-1 without one).  A row may see no key of a block, or a
+  // split rank none of its share: it keeps m = -inf and p = 0 there, and the cluster merge weighs that rank by 0.
+  const int row_lo[2] = {window > 0 ? row_pos[0] - window : -1, window > 0 ? row_pos[1] - window : -1};
 
   for (int j = jb0; j < jb1; ++j) {
     const int st = (j - jb0) & 1;
@@ -603,7 +621,7 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
       for (int e = 0; e < 4; ++e) {
         const int kpos = j * KV_BLOCK + nt * 8 + t * 2 + (e & 1);
         const int r = e >> 1;
-        s[nt][e] = (kpos <= row_pos[r]) ? s[nt][e] * sl2 : -INFINITY;
+        s[nt][e] = (kpos <= row_pos[r] && kpos > row_lo[r]) ? s[nt][e] * sl2 : -INFINITY;
         mx[r] = fmaxf(mx[r], s[nt][e]);
       }
     float corr[2];
@@ -746,17 +764,17 @@ cudaError_t attn_prefill_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv
                                 const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                 const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
                                 __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale, cudaStream_t stream,
-                                int head_dim) {
+                                int head_dim, int window) {
   if (n_tiles <= 0) return cudaSuccess;
-  if (n_q % n_kv != 0) return cudaErrorInvalidValue;
+  if (n_q % n_kv != 0 || window < 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
   if (G > 8 || (head_dim != 128 && head_dim != 64)) return cudaErrorInvalidValue;
   dim3 grid(n_tiles, n_kv);
   if (head_dim == 64)
     return launch_k(attn_prefill_kernel<64, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
-                    tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale);
+                    tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
   return launch_k(attn_prefill_kernel<128, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
-                  tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale);
+                  tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
 }
 
 template <int D>
@@ -764,7 +782,7 @@ static cudaError_t prefill_split_launch_d(const __nv_bfloat16* qkv, int qkv_ld, 
                                           const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                           const int32_t* tile_q0, int n_tiles, const int32_t* block_table,
                                           int bt_stride, __nv_bfloat16* out, int out_ld, int n_kv, int G, float scale,
-                                          cudaStream_t stream) {
+                                          cudaStream_t stream, int window) {
   // the shared-memory opt-in is per device: one bit per device ordinal, set once (racing setters set the same value)
   static std::atomic<uint64_t> attr_set{0};
   int dev = 0;
@@ -781,24 +799,24 @@ static cudaError_t prefill_split_launch_d(const __nv_bfloat16* qkv, int qkv_ld, 
   dim3 grid(n_tiles * PF_CLUSTER, n_kv);
   return launch_k_cluster(attn_prefill_kernel<D, true>, grid, dim3(32 * G), (size_t)smem, stream, PF_CLUSTER, qkv,
                           qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv,
-                          G, scale);
+                          G, scale, window);
 }
 
 cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
                                       const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                       const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
                                       __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                                      cudaStream_t stream, int head_dim) {
+                                      cudaStream_t stream, int head_dim, int window) {
   if (n_tiles <= 0) return cudaSuccess;
-  if (n_q % n_kv != 0) return cudaErrorInvalidValue;
+  if (n_q % n_kv != 0 || window < 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
   if (G > 8) return cudaErrorInvalidValue;
   if (head_dim == 128)
     return prefill_split_launch_d<128>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
-                                       bt_stride, out, out_ld, n_kv, G, scale, stream);
+                                       bt_stride, out, out_ld, n_kv, G, scale, stream, window);
   if (head_dim == 64)
     return prefill_split_launch_d<64>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
-                                      bt_stride, out, out_ld, n_kv, G, scale, stream);
+                                      bt_stride, out, out_ld, n_kv, G, scale, stream, window);
   return cudaErrorInvalidValue;
 }
 

@@ -271,6 +271,9 @@ struct tgis_engine {
   // full block whose KV a completed step wrote, its cache entry.  A keyed block nobody references sits in the evictable
   // LRU (front = least recently used) and keeps its key until it is reallocated.
   bool prefix_caching = false;
+  // sliding-window attention (tgis_engine_set_sliding_window): every layer's query at position p sees the keys
+  // p - window < k <= p; 0 = the whole context.  KV blocks stay allocated for the whole sequence.
+  int attn_window = 0;
   struct PcBlock {
     int ref = 0;
     uint64_t uid = 0;            // cache entry id (0: not keyed)
@@ -1162,13 +1165,13 @@ struct tgis_engine {
     const int n_std = n_tiles - step_ctiles;
     if (n_std > 0) {
       CK(attn_prefill_launch(qkv.p, qkv_dim, kc, vc, d_seqs, ds<int32_t>(off_tileseq), ds<int32_t>(off_tileq0), n_std,
-                             d_bt, bt_stride, attn_out.p, q_dim, nq, nkv, scale, stream, kv_head_dim));
+                             d_bt, bt_stride, attn_out.p, q_dim, nq, nkv, scale, stream, kv_head_dim, attn_window));
       ++n_launches;
     }
     if (step_ctiles > 0) {
       CK(attn_prefill_split_launch(qkv.p, qkv_dim, kc, vc, d_seqs, ds<int32_t>(off_tileseq) + n_std,
                                    ds<int32_t>(off_tileq0) + n_std, step_ctiles, d_bt, bt_stride, attn_out.p, q_dim, nq,
-                                   nkv, scale, stream, kv_head_dim));
+                                   nkv, scale, stream, kv_head_dim, attn_window));
       ++n_launches;
     }
   }
@@ -1261,7 +1264,7 @@ struct tgis_engine {
         const int max_splits = (max_dec_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
         CK(attn_decode_launch(qkv.p, qkv_dim, kc, vc, ds<DecItem>(items_off(S)), n_dec * max_splits, d_seqs,
                               ds<int32_t>(off_decids), n_dec, max_splits, part_o.p, part_ml.p, attn_out.p, q_dim, nq,
-                              nkv, scale, num_sms, stream, kv_head_dim));
+                              nkv, scale, num_sms, stream, kv_head_dim, attn_window));
         n_launches += max_splits > 1 ? 2 : 1;
       }
       if (n_tiles > 0) prefill_attention(kc, vc, scale, n_tiles);
@@ -1638,7 +1641,7 @@ struct tgis_engine {
     // decode work items: (sequence, DECODE_SPLIT-token split) entries; the copy covers the worst case for this
     // (S, max_splits) so that its size is a function of the CUDA-graph key
     const int max_splits_step = (max_dec_kv + DECODE_SPLIT - 1) / DECODE_SPLIT;
-    decode_items_build(hs<DecItem>(items_off(S)), seqs, decids, n_dec, bt, bt_stride);
+    decode_items_build(hs<DecItem>(items_off(S)), seqs, decids, n_dec, bt, bt_stride, attn_window);
     const size_t copy_bytes = items_off(S) + sizeof(DecItem) * (1 + (size_t)n_dec * max_splits_step);
     const double t_ev0 = debug_launch ? now_s() : 0.0;
     CK(cudaEventRecord(ev0, stream));
@@ -2251,6 +2254,17 @@ int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on) {
     return fail(ex.what());
   }
   e->qk_norm_loaded.assign(e->cfg.n_layers, 0);
+  return 0;
+}
+
+int tgis_engine_set_sliding_window(tgis_engine* e, int32_t window) {
+  if (!e) return fail("null engine");
+  if (e->started) return fail("the sliding window must be set before tgis_engine_start");
+  if (window < 0) return fail("sliding window must be >= 0 (0 = attend to the whole context)");
+  if (window > 0 && e->opt) return fail("sliding-window attention applies to the Llama layer stack only, not OPT");
+  if (window > 0 && e->tp > 1)
+    return fail("sliding-window attention is supported on a single GPU only (tp_size must be 1)");
+  e->attn_window = window;
   return 0;
 }
 

@@ -7,6 +7,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 namespace tgis {
 
 // ---- gemm_wgmma.cu ---------------------------------------------------------------------------------------------
@@ -201,32 +203,46 @@ struct DecItem {       // 32 bytes
   int32_t q_row;       // row of the sequence's token in qkv / out            ([0]: number of entries)
   int32_t kv_len;      // of the whole sequence
   int32_t seq_split;   // seq | split << 16; seq = index among this step's decode sequences (partial buffers)
-  int32_t reserved;
+  int32_t lo;          // first visible position: max(0, kv_len - window) under a sliding window, else 0
   int32_t blocks[DECODE_SPLIT / KV_BLOCK];  // physical KV blocks of the split (resolved on the host: no table walk)
 };
 static_assert(DECODE_SPLIT / KV_BLOCK == 4 && sizeof(DecItem) == 32, "DecItem is read as two int4");
 // Entries are listed longest first (all full splits, then the partial tails by decreasing length): the kernel deals
 // them to its warps round-robin, so the order is the load balance.  Ties keep (sequence, split) order: deterministic.
+// Sliding window (window > 0; 0 = none): only the splits holding a position >= lo are listed.  A split that holds lo
+// past its first token counts as a tail of its visible blocks, those from the block holding lo to its last.
 inline int decode_items_build(DecItem* items, const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs,
-                              const int32_t* block_table, int bt_stride) {
+                              const int32_t* block_table, int bt_stride, int window = 0) {
   constexpr int BPS = DECODE_SPLIT / KV_BLOCK;
   int n = 0;
+  auto lo_of = [&](const AttnSeq& sq) { return window > 0 ? std::max(0, sq.kv_len - window) : 0; };
   auto emit = [&](int i, const AttnSeq& sq, int sp) {
     const int n_blocks = (sq.kv_len + KV_BLOCK - 1) / KV_BLOCK;
     const int32_t* row = block_table + (size_t)sq.block_row * bt_stride;
     DecItem& it = items[++n];
-    it = DecItem{sq.q_start, sq.kv_len, i | (sp << 16), 0, {0, 0, 0, 0}};
+    it = DecItem{sq.q_start, sq.kv_len, i | (sp << 16), lo_of(sq), {0, 0, 0, 0}};
     for (int j = 0; j < BPS; ++j) it.blocks[j] = sp * BPS + j < n_blocks ? row[sp * BPS + j] : 0;
+  };
+  // blocks the kernel streams for split sp, and whether every one of its DECODE_SPLIT tokens is visible
+  auto visible_blocks = [&](const AttnSeq& sq, int sp) {
+    const int n_tok = std::min(DECODE_SPLIT, sq.kv_len - sp * DECODE_SPLIT);
+    return (n_tok + KV_BLOCK - 1) / KV_BLOCK - std::max(0, lo_of(sq) - sp * DECODE_SPLIT) / KV_BLOCK;
+  };
+  auto whole = [&](const AttnSeq& sq, int sp) {
+    return (sp + 1) * DECODE_SPLIT <= sq.kv_len && lo_of(sq) <= sp * DECODE_SPLIT;
   };
   for (int i = 0; i < n_seqs; ++i) {  // full splits
     const AttnSeq& sq = seqs[seq_ids ? seq_ids[i] : i];
-    for (int sp = 0; sp < sq.kv_len / DECODE_SPLIT; ++sp) emit(i, sq, sp);
+    for (int sp = lo_of(sq) / DECODE_SPLIT; sp < sq.kv_len / DECODE_SPLIT; ++sp)
+      if (whole(sq, sp)) emit(i, sq, sp);
   }
   for (int nb = BPS; nb >= 1; --nb) {  // tails: 4, 3, 2, 1 blocks (a tail of exactly DECODE_SPLIT tokens was a full split)
     for (int i = 0; i < n_seqs; ++i) {
       const AttnSeq& sq = seqs[seq_ids ? seq_ids[i] : i];
-      const int rem = sq.kv_len % DECODE_SPLIT;
-      if (rem > 0 && (rem + KV_BLOCK - 1) / KV_BLOCK == nb) emit(i, sq, sq.kv_len / DECODE_SPLIT);
+      // at most two per sequence: the split holding lo and the last split
+      const int sp_cand[2] = {lo_of(sq) / DECODE_SPLIT, (sq.kv_len - 1) / DECODE_SPLIT};
+      for (int c = 0; c < (sp_cand[1] > sp_cand[0] ? 2 : 1); ++c)
+        if (!whole(sq, sp_cand[c]) && visible_blocks(sq, sp_cand[c]) == nb) emit(i, sq, sp_cand[c]);
     }
   }
   items[0] = DecItem{n, 0, 0, 0, {0, 0, 0, 0}};
@@ -238,13 +254,15 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
                                const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits, float* part_o,
                                float* part_ml, __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                               int num_sms, cudaStream_t stream, int head_dim = HEAD_DIM);
-// Prefill / chunked prefill (q_len >= 1), causal over the paged cache.
+                               int num_sms, cudaStream_t stream, int head_dim = HEAD_DIM, int window = 0);
+// Prefill / chunked prefill (q_len >= 1), causal over the paged cache.  window > 0: sliding-window attention, query
+// position p sees the keys p - window < k <= p (transformers' sliding_window, vLLM's window_left = window - 1); 0: none.
+// The decode launch's items must have been built with the same window.
 cudaError_t attn_prefill_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
                                 const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                 const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
                                 __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale, cudaStream_t stream,
-                                int head_dim = HEAD_DIM);
+                                int head_dim = HEAD_DIM, int window = 0);
 // Split-context prefill: same arguments and result layout; one cluster of PF_CLUSTER CTAs per (tile, kv head), each
 // streaming a contiguous share of the tile's context, merged through distributed shared memory (attention.cu).
 constexpr int PF_CLUSTER = 8;
@@ -252,7 +270,7 @@ cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, cons
                                       const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                       const int32_t* tile_q0, int n_tiles, const int32_t* block_table, int bt_stride,
                                       __nv_bfloat16* out, int out_ld, int n_q, int n_kv, float scale,
-                                      cudaStream_t stream, int head_dim = HEAD_DIM);
+                                      cudaStream_t stream, int head_dim = HEAD_DIM, int window = 0);
 // Which prefill sequences the split-context kernel takes when prefix caching is on: a short query span over a long
 // context already in the cache (the shape of a prefix-cache hit).  A function of the sequence's own (q_len, kv_len)
 // only, never of the rest of the step, so a sequence's bits do not depend on what it is batched with.  Measured on an

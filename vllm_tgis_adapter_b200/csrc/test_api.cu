@@ -255,6 +255,7 @@ namespace {
 struct AttnCall {
   int n_q = 0, n_kv = 0, n_dec = 0, n_tiles = 0, n_ctiles = 0, max_splits = 1, bt_stride = 0;
   int head_dim = HEAD_DIM;  // set before prepare()
+  int window = 0;           // sliding window (0: none), set before prepare()
   Tmp<AttnSeq> seqs;
   Tmp<int32_t> dec, tseq, tq0, bt;
   Tmp<float> po, pml;
@@ -301,7 +302,7 @@ struct AttnCall {
     KCK(po.alloc(nd * n_kv * max_splits * G * head_dim));
     KCK(pml.alloc(nd * n_kv * max_splits * G * 2));
     std::vector<DecItem> h_items(1 + nd * max_splits);
-    decode_items_build(h_items.data(), h_seqs.data(), h_dec.data(), n_dec, block_table_host, bt_stride);
+    decode_items_build(h_items.data(), h_seqs.data(), h_dec.data(), n_dec, block_table_host, bt_stride, window);
     KCK(items.upload(h_items.data(), h_items.size()));
     return 0;
   }
@@ -312,31 +313,41 @@ struct AttnCall {
     if (decode)
       KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, items.p,
                              n_dec * max_splits, seqs.p, dec.p, n_dec, max_splits, po.p, pml.p, (bf16*)out_dev, out_ld,
-                             n_q, n_kv, scale, test_num_sms(), st, head_dim));
+                             n_q, n_kv, scale, test_num_sms(), st, head_dim, window));
     const int n_std = n_tiles - n_ctiles;
     KCK(attn_prefill_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev, seqs.p,
                             tseq.p, tq0.p, n_std, bt.p, bt_stride, (bf16*)out_dev, out_ld, n_q, n_kv, scale, st,
-                            head_dim));
+                            head_dim, window));
     KCK(attn_prefill_split_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)k_cache_dev, (const bf16*)v_cache_dev,
                                   seqs.p, tseq.p + n_std, tq0.p + n_std, n_ctiles, bt.p, bt_stride, (bf16*)out_dev,
-                                  out_ld, n_q, n_kv, scale, st, head_dim));
+                                  out_ld, n_q, n_kv, scale, st, head_dim, window));
     return 0;
   }
 };
 }  // namespace
 
-int tgis_k_attention_split_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
-                              const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
-                              int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
-                              int32_t mode) {
+int tgis_k_attention_window(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                            const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
+                            int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale, int32_t mode,
+                            int32_t window) {
   if (mode < 0 || mode > 2) return kfail("mode must be 0 (existing prefill kernel), 1 (split-context) or 2 (selection)");
   if (head_dim != 64 && head_dim != HEAD_DIM) return kfail("head_dim must be 64 or 128");
+  if (window < 0) return kfail("window must be >= 0 (0: none)");
   AttnCall call;
   call.head_dim = head_dim;
+  call.window = window;
   if (call.prepare(seqs_host, n_seqs, block_table_host, bt_rows, bt_stride, n_q, n_kv, mode) != 0) return -1;
   if (call.launch(qkv_dev, k_cache_dev, v_cache_dev, out_dev, scale, 0) != 0) return -1;
   KCK(cudaDeviceSynchronize());
   return 0;
+}
+
+int tgis_k_attention_split_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                              const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                              int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
+                              int32_t mode) {
+  return tgis_k_attention_window(head_dim, qkv_dev, k_cache_dev, v_cache_dev, seqs_host, n_seqs, block_table_host,
+                                 bt_rows, bt_stride, out_dev, n_q, n_kv, scale, mode, 0);
 }
 
 int tgis_k_attention_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
@@ -443,12 +454,14 @@ int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, 
 
 // decode attention only, timed: `iters` launches rotating over `n_layers` cache copies (layer_stride_bytes apart) so that
 // a small batch does not simply sit in L2; us_out = average device time per launch
-int tgis_k_attention_bench_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
-                              const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
-                              int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
-                              int32_t n_layers, int64_t layer_stride_bytes, int32_t iters, float* us_out) {
+int tgis_k_attention_bench_window(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev,
+                                  const void* v_cache_dev, const int32_t* seqs_host, int32_t n_seqs,
+                                  const int32_t* block_table_host, int32_t bt_rows, int32_t bt_stride, void* out_dev,
+                                  int32_t n_q, int32_t n_kv, float scale, int32_t n_layers, int64_t layer_stride_bytes,
+                                  int32_t iters, float* us_out, int32_t window) {
   if (n_kv <= 0 || n_q % n_kv) return kfail("bad head counts");
   if (head_dim != 64 && head_dim != HEAD_DIM) return kfail("head_dim must be 64 or 128");
+  if (window < 0) return kfail("window must be >= 0 (0: none)");
   const int G = n_q / n_kv;
   const int qkv_ld = (n_q + 2 * n_kv) * head_dim, out_ld = n_q * head_dim;
   std::vector<AttnSeq> seqs(n_seqs);
@@ -467,7 +480,7 @@ int tgis_k_attention_bench_hd(int32_t head_dim, const void* qkv_dev, const void*
   KCK(po.alloc((size_t)n_seqs * n_kv * max_splits * G * head_dim));
   KCK(pml.alloc((size_t)n_seqs * n_kv * max_splits * G * 2));
   std::vector<DecItem> items(1 + (size_t)n_seqs * max_splits);
-  decode_items_build(items.data(), seqs.data(), nullptr, n_seqs, block_table_host, bt_stride);
+  decode_items_build(items.data(), seqs.data(), nullptr, n_seqs, block_table_host, bt_stride, window);
   Tmp<DecItem> d_items;
   KCK(d_items.upload(items.data(), items.size()));
   const int num_sms = test_num_sms();
@@ -481,7 +494,7 @@ int tgis_k_attention_bench_hd(int32_t head_dim, const void* qkv_dev, const void*
     const char* vc = (const char*)v_cache_dev + (size_t)l * layer_stride_bytes;
     KCK(attn_decode_launch((const bf16*)qkv_dev, qkv_ld, (const bf16*)kc, (const bf16*)vc, d_items.p,
                            n_seqs * max_splits, d_seqs.p, nullptr, n_seqs, max_splits, po.p, pml.p, (bf16*)out_dev,
-                           out_ld, n_q, n_kv, scale, num_sms, 0, head_dim));
+                           out_ld, n_q, n_kv, scale, num_sms, 0, head_dim, window));
   }
   KCK(cudaEventRecord(e1, 0));
   KCK(cudaDeviceSynchronize());
@@ -491,6 +504,15 @@ int tgis_k_attention_bench_hd(int32_t head_dim, const void* qkv_dev, const void*
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
   return 0;
+}
+
+int tgis_k_attention_bench_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
+                              const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                              int32_t bt_rows, int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale,
+                              int32_t n_layers, int64_t layer_stride_bytes, int32_t iters, float* us_out) {
+  return tgis_k_attention_bench_window(head_dim, qkv_dev, k_cache_dev, v_cache_dev, seqs_host, n_seqs, block_table_host,
+                                       bt_rows, bt_stride, out_dev, n_q, n_kv, scale, n_layers, layer_stride_bytes, iters,
+                                       us_out, 0);
 }
 
 int tgis_k_attention_bench(const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
@@ -613,8 +635,9 @@ int tgis_k_gemm_blocks_per_sm(int32_t T, int32_t lean, int32_t* out) {
 
 // Host-only: the decode work-item list the scheduler builds for a step (no GPU needed).  seqs_host as in
 // tgis_k_attention (all decode sequences); items_out: (1 + capacity) x 8 int32 records; returns the entry count or -1.
-int tgis_k_decode_items(const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_stride,
-                        int32_t* items_out, int32_t capacity) {
+int tgis_k_decode_items_window(const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host,
+                               int32_t bt_stride, int32_t* items_out, int32_t capacity, int32_t window) {
+  if (window < 0) return kfail("window must be >= 0 (0: none)");
   std::vector<AttnSeq> seqs(n_seqs);
   long long need = 0;
   for (int s = 0; s < n_seqs; ++s) {
@@ -624,7 +647,12 @@ int tgis_k_decode_items(const int32_t* seqs_host, int32_t n_seqs, const int32_t*
   if (need > capacity) return kfail("capacity too small");
   static_assert(sizeof(DecItem) == 32, "8 int32 per record");
   return decode_items_build(reinterpret_cast<DecItem*>(items_out), seqs.data(), nullptr, n_seqs, block_table_host,
-                            bt_stride);
+                            bt_stride, window);
+}
+
+int tgis_k_decode_items(const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_stride,
+                        int32_t* items_out, int32_t capacity) {
+  return tgis_k_decode_items_window(seqs_host, n_seqs, block_table_host, bt_stride, items_out, capacity, 0);
 }
 
 // ---- tensor-parallel exchange kernels, one rank at a time on one device.  The other ranks' receive areas are plain

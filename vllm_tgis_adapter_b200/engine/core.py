@@ -26,7 +26,10 @@ class ModelConfig:
     rope_type "llama3" frequency scaling of Llama-3.1 / 3.2 (rope_scaling_factor > 1; loader.rope_cos_sin).
 
     Qwen3 (Qwen3ForCausalLM) is arch "llama" with qk_norm set: an RMSNorm over each q and k head before RoPE, with the
-    per-layer weights self_attn.q_norm / k_norm (tgis_engine_set_qk_norm; head_dim 128, single GPU)."""
+    per-layer weights self_attn.q_norm / k_norm (tgis_engine_set_qk_norm; head_dim 128, single GPU).
+
+    Mistral (MistralForCausalLM) is arch "llama" with sliding_window set: every layer's query at position p attends to
+    the keys p - sliding_window < k <= p (tgis_engine_set_sliding_window; single GPU)."""
 
     n_layers: int        # num_hidden_layers
     hidden: int          # hidden_size
@@ -49,6 +52,7 @@ class ModelConfig:
     rope_high_freq_factor: float = 4.0  # high_freq_factor
     rope_original_max_pos: int = 8192   # original_max_position_embeddings
     qk_norm: bool = False               # Qwen3: per-head RMSNorm of q and k (self_attn.q_norm / k_norm)
+    sliding_window: int | None = None   # Mistral: keys per query, itself included, in every layer; None = all
 
     @property
     def rope_scaled(self) -> bool:
@@ -109,6 +113,18 @@ PRESETS: dict[str, ModelConfig] = {
                               qk_norm=True),
     "qwen3-8b": ModelConfig(n_layers=36, hidden=4096, n_q_heads=32, n_kv_heads=8, ffn=12288, vocab=151936,
                             rope_theta=1000000.0, rms_eps=1e-6, max_model_len=8192, qk_norm=True),
+    # Mistral: a CPU-oracle-sized stack whose q width (4 x 128) is not its hidden size, with an odd vocabulary and a
+    # window of 40 (shorter than the test prompts, not a multiple of the 32-token KV block), and the Mistral-7B v0.1 /
+    # v0.3 and Mistral-Nemo-12B shapes.  Those three are the published mistralai config.json values as recalled, not
+    # checked against the files when these presets were written.
+    "mistral-tiny": ModelConfig(n_layers=2, hidden=256, n_q_heads=4, n_kv_heads=1, ffn=512, vocab=1021,
+                                rope_theta=10000.0, rms_eps=1e-5, max_model_len=2048, sliding_window=40),
+    "mistral-7b-v0.1": ModelConfig(n_layers=32, hidden=4096, n_q_heads=32, n_kv_heads=8, ffn=14336, vocab=32000,
+                                   rope_theta=10000.0, rms_eps=1e-5, max_model_len=8192, sliding_window=4096),
+    "mistral-7b-v0.3": ModelConfig(n_layers=32, hidden=4096, n_q_heads=32, n_kv_heads=8, ffn=14336, vocab=32768,
+                                   rope_theta=1000000.0, rms_eps=1e-5, max_model_len=8192),
+    "mistral-nemo-12b": ModelConfig(n_layers=40, hidden=5120, n_q_heads=32, n_kv_heads=8, ffn=14336, vocab=131072,
+                                    rope_theta=1000000.0, rms_eps=1e-5, max_model_len=8192),
 }
 
 
@@ -201,6 +217,9 @@ class NativeEngine:
         if model.qk_norm and tp_size > 1:
             raise EngineError("Qwen3 (qk_norm) is not supported with tensor parallelism: the q/k norm is implemented on a "
                               "single GPU only (use tensor_parallel_size 1)")
+        if model.sliding_window and tp_size > 1:
+            raise EngineError("sliding-window attention (Mistral) is not supported with tensor parallelism: it is "
+                              "implemented on a single GPU only (use tensor_parallel_size 1)")
         if model.arch not in ("llama", "opt"):
             raise EngineError(f"unknown architecture {model.arch!r}")
         if model.arch == "llama" and model.head_dim != 128 and model.is_granite:
@@ -230,6 +249,10 @@ class NativeEngine:
             msg = _lib.last_error(self.lib)
             self.close()
             raise EngineError(f"tgis_engine_set_qk_norm failed: {msg}")
+        if model.sliding_window and self.lib.tgis_engine_set_sliding_window(self._h, int(model.sliding_window)) != 0:
+            msg = _lib.last_error(self.lib)
+            self.close()
+            raise EngineError(f"tgis_engine_set_sliding_window failed: {msg}")
         self.enable_prefix_caching = bool(enable_prefix_caching)
         if self.enable_prefix_caching and self.lib.tgis_engine_set_prefix_caching(self._h, 1) != 0:
             msg = _lib.last_error(self.lib)

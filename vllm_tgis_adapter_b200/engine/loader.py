@@ -28,6 +28,8 @@ def model_config_from_hf(path: Path, max_model_len: int | None) -> ModelConfig:
         return _granite_model_config(cfg, max_model_len)
     if cfg.get("model_type") == "qwen3" or "Qwen3ForCausalLM" in archs:
         return _qwen3_model_config(cfg, max_model_len)
+    if cfg.get("model_type") == "mistral" or "MistralForCausalLM" in archs:
+        return _mistral_model_config(cfg, max_model_len)
     if cfg.get("model_type") != "llama" and not any("Llama" in a for a in archs):
         raise ValueError(f"unsupported model architecture {archs or cfg.get('model_type')}: only Llama-family "
                          "decoders (RMSNorm, RoPE, GQA, SwiGLU) and OPT are implemented")
@@ -126,6 +128,41 @@ def _qwen3_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
                        vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=theta,
                        rms_eps=float(cfg.get("rms_norm_eps", 1e-6)), max_model_len=max_model_len or min(derived, 8192),
                        tie_word_embeddings=bool(cfg.get("tie_word_embeddings", False)), qk_norm=True, **scaling)
+
+
+def _mistral_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
+    """mistralai MistralForCausalLM config.json -> the Llama stack with a sliding window in every layer (vLLM applies a
+    model-wide window to each layer).  transformers' MistralConfig defaults sliding_window to 4096, so a config.json
+    without the key is windowed; null or 0 is no window.  Variants the engine would serve wrongly are refused, each with
+    its reason; the rotary embedding is read as for Llama (_llama_rope: yarn and the other scaled types are refused)."""
+    hidden, heads = cfg["hidden_size"], cfg["num_attention_heads"]
+    head_dim = cfg.get("head_dim") or hidden // heads
+    window = cfg.get("sliding_window", 4096)
+    problems = []
+    if cfg.get("attention_bias") or cfg.get("mlp_bias"):
+        problems.append("attention_bias / mlp_bias (the Llama stack has no projection biases)")
+    if cfg.get("llama_4_scaling"):
+        problems.append("llama_4_scaling (position-dependent query scaling is not implemented)")
+    kinds = sorted(set(cfg.get("layer_types") or []))
+    if len(kinds) > 1:
+        problems.append(f"layer_types mixing {kinds} (per-layer windows are not implemented: one window serves every "
+                        "layer)")
+    if window is not None and (not isinstance(window, int) or isinstance(window, bool) or window < 0):
+        problems.append(f"sliding_window {window!r} (a non-negative integer or null)")
+    if head_dim not in (64, 128):
+        problems.append(f"head_dim {head_dim} (the attention kernels exist for 64 and 128)")
+    if problems:
+        raise ValueError("unsupported Mistral variant: " + "; ".join(problems))
+    theta, scaling = _llama_rope(cfg)
+    derived = cfg.get("max_position_embeddings", 32768)
+    if max_model_len is not None and max_model_len > derived:
+        raise ValueError(f"max_model_len {max_model_len} exceeds the model's max_position_embeddings {derived}")
+    return ModelConfig(n_layers=cfg["num_hidden_layers"], hidden=hidden, n_q_heads=heads,
+                       n_kv_heads=cfg.get("num_key_value_heads", heads), ffn=cfg["intermediate_size"],
+                       vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=theta,
+                       rms_eps=float(cfg.get("rms_norm_eps", 1e-6)), max_model_len=max_model_len or min(derived, 8192),
+                       tie_word_embeddings=bool(cfg.get("tie_word_embeddings", False)), sliding_window=window or None,
+                       **scaling)
 
 
 def _opt_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
@@ -288,6 +325,8 @@ def build_engine(args) -> AsyncTGISEngine:
     tp_kw = {}
     if tp > 1 and mc.qk_norm:
         raise ValueError(f"Qwen3 (per-head q/k norm) is supported on a single GPU only: tensor_parallel_size {tp}")
+    if tp > 1 and mc.sliding_window:
+        raise ValueError(f"Mistral (sliding-window attention) is supported on a single GPU only: tensor_parallel_size {tp}")
     if tp > 1:
         import multiprocessing as mp
         import os
