@@ -226,6 +226,15 @@ int tgis_engine_require_rope_table(tgis_engine* e);
  * TGIS_ARCH_LLAMA with head_dim 128 on a single GPU only.  Valid only between tgis_engine_create and tgis_engine_start;
  * on = 0 turns it off again. */
 int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on);
+/* Qwen2 / Qwen2.5 (Qwen2ForCausalLM: the Llama layer stack with a bias on the q, k and v projections and nowhere else;
+ * vllm model_executor/models/qwen2.py).  on != 0 allocates the per-layer vectors (n_layers x (n_q + 2 n_kv) x head_dim
+ * bf16, outside the weight arena) and fp32 scratch for the qkv projection, and makes
+ * "model.layers.{i}.self_attn.{q,k,v}_proj.bias" (rows = n_q x head_dim or n_kv x head_dim, cols = 1) legal weight
+ * names; tgis_engine_start then fails, naming the layer and tensor, unless every layer has all three.  The projection is
+ * rounded once after the fp32 bias add, y = bf16(x . W^T + b) (F.linear with a bias in bf16); LoRA deltas are added to
+ * that biased output, then RoPE runs.  TGIS_ARCH_LLAMA (head_dim 128 or 64) on a single GPU, not together with
+ * tgis_engine_set_qk_norm.  Valid only between tgis_engine_create and tgis_engine_start; on = 0 turns it off again. */
+int tgis_engine_set_qkv_bias(tgis_engine* e, int32_t on);
 /* Sliding-window attention in every layer (Mistral: config.json sliding_window; vLLM applies a model-wide window to each
  * layer).  The query at position p attends to the keys at positions p - window < k <= p, window keys including itself;
  * window = 0 (the default) attends to the whole context.  Decode, prefill, chunked prefill, prompt logprobs, the

@@ -82,7 +82,8 @@ int tgis_k_rope_attention(int32_t writer, const void* x_dev, const void* w_dev, 
                           void* out_dev, int32_t n_q, int32_t n_kv, float scale);
 /* The same hooks for either head geometry: head_dim 128 (the calls above) or 64, where qkv rows are (n_q + 2 n_kv) * 64,
  * cos_sin rows cos(32) | sin(32), a K tile is [8 chunks][32 tok][8] and a V tile [32 tok][8 chunks ^ (tok & 7)][8] (4 KiB
- * each), for group sizes n_q / n_kv in {1, 2, 4, 8}.  tgis_k_attention_hd = tgis_k_attention_split_hd with mode 0. */
+ * each), for group sizes n_q / n_kv in {1, 2, 4, 5, 6, 7, 8} (head_dim 128 also takes 3).  tgis_k_attention_hd =
+ * tgis_k_attention_split_hd with mode 0. */
 int tgis_k_rope_kv_hd(int32_t head_dim, void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
                       const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q,
                       int32_t n_kv);
@@ -93,6 +94,15 @@ int tgis_k_rope_kv_qknorm(void* qkv_dev, const int32_t* positions_host, const in
                           const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q,
                           int32_t n_kv, const void* q_norm_dev, const void* k_norm_dev, float eps, int32_t iters,
                           float* us_out);
+/* The Qwen2 writer (head_dim 128 or 64): acc_dev fp32 [T, (n_q + 2 n_kv) * head_dim], the qkv GEMM's accumulators, and
+ * bias_dev bf16 [(n_q + 2 n_kv) * head_dim].  Every element is rounded once as bf16(acc + bias); q and k are then rotated
+ * as by tgis_k_rope_kv_hd, all heads are written to qkv_dev and k / v scattered into the caches.  The writer runs
+ * max(iters, 1) times on stream 0 (it reads acc_dev, so repeats are idempotent); us_out (may be null): mean
+ * microseconds per launch between CUDA events. */
+int tgis_k_rope_kv_bias(int32_t head_dim, const void* acc_dev, const void* bias_dev, void* qkv_dev,
+                        const int32_t* positions_host, const int32_t* slot_mapping_host, const void* cos_sin_dev,
+                        void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q, int32_t n_kv, int32_t iters,
+                        float* us_out);
 int tgis_k_attention_hd(int32_t head_dim, const void* qkv_dev, const void* k_cache_dev, const void* v_cache_dev,
                         const int32_t* seqs_host, int32_t n_seqs, const int32_t* block_table_host, int32_t bt_rows,
                         int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale);

@@ -492,13 +492,19 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
       TGIS_DEC(128, 2);
       TGIS_DEC(128, 3);
       TGIS_DEC(128, 4);
+      TGIS_DEC(128, 5);
+      TGIS_DEC(128, 6);
+      TGIS_DEC(128, 7);
       TGIS_DEC(128, 8);
     }
   } else if (head_dim == 64) {
-    switch (G) {
+    switch (G) {  // (G = 3 is not instantiated for 64-dim heads)
       TGIS_DEC(64, 1);
       TGIS_DEC(64, 2);
       TGIS_DEC(64, 4);
+      TGIS_DEC(64, 5);
+      TGIS_DEC(64, 6);
+      TGIS_DEC(64, 7);
       TGIS_DEC(64, 8);
     }
   }

@@ -658,13 +658,20 @@ cudaError_t silu_mul_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, in
 // lo[0..7] and then of hi[0..7] (dims 8c..8c+7, then 64+8c..64+8c+7), one at a time; xor-shuffles over the 8 lanes at
 // distances 1, 2, 4 then give every lane ((s0 + s1) + (s2 + s3)) + ((s4 + s5) + (s6 + s7)).  A bf16 square is exact in
 // fp32, so a contraction into a fused multiply-add changes nothing.  RoPE then rotates y; V heads are not normalised.
-template <int D, bool QKNORM = false>
+//
+// BIAS (Qwen2; D = 128 and 64): the input is the qkv GEMM's fp32 accumulators acc [T, (n_q + 2 n_kv) * D] and every
+// element is first rounded once as bf16(acc + bias) (the fp32 add of F.linear with a bias, in model dtype; bias [(n_q +
+// 2 n_kv) * D] in qkv's q | k | v row order).  q and k are then rotated as above and written to qkv with the raw v, so
+// qkv and the caches hold exactly what opt_bias_act_kernel (no activation) followed by the plain writer leaves.
+template <int D, bool QKNORM = false, bool BIAS = false>
 __global__ void __launch_bounds__(128)
 rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ positions,
                     const int32_t* __restrict__ slot_mapping, const __nv_bfloat16* __restrict__ cos_sin,
                     __nv_bfloat16* __restrict__ k_cache, __nv_bfloat16* __restrict__ v_cache, int n_q, int n_kv,
-                    const __nv_bfloat16* __restrict__ q_norm, const __nv_bfloat16* __restrict__ k_norm, float eps) {
+                    const __nv_bfloat16* __restrict__ q_norm, const __nv_bfloat16* __restrict__ k_norm, float eps,
+                    const float* __restrict__ acc, const __nv_bfloat16* __restrict__ bias) {
   static_assert(!QKNORM || D == 128, "the q / k norm variant exists for 128-dim heads");
+  static_assert(!(QKNORM && BIAS), "no model has both a q / k norm and a qkv bias");
   griddep_launch();
   BF8 wlo, whi;  // QKNORM: this thread's 16 norm weights (static: read before the wait, as rmsnorm_kernel does)
   if constexpr (QKNORM) {
@@ -673,6 +680,16 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
       const BF8* w = reinterpret_cast<const BF8*>(head < n_q ? q_norm : k_norm);
       wlo = w[threadIdx.x % 8];
       whi = w[8 + threadIdx.x % 8];
+    }
+  }
+  BF8 blo, bhi;  // BIAS: this thread's 16 bias values (static: read before the wait)
+  if constexpr (BIAS) {
+    constexpr int CHB = D / 16;
+    const int head = blockIdx.y * (128 / CHB) + threadIdx.x / CHB;
+    if (head < n_q + 2 * n_kv) {
+      const BF8* b = reinterpret_cast<const BF8*>(bias + (size_t)head * D);
+      blo = b[threadIdx.x % CHB];
+      bhi = b[CHB + threadIdx.x % CHB];
     }
   }
   griddep_wait();
@@ -684,8 +701,21 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
   if (head >= n_heads) return;
   __nv_bfloat16* h = qkv + ((size_t)t * n_heads + head) * D;
   const int slot = slot_mapping[t];
-  BF8 lo = reinterpret_cast<const BF8*>(h)[c];
-  BF8 hi = reinterpret_cast<const BF8*>(h)[CH + c];
+  BF8 lo, hi;
+  if constexpr (BIAS) {
+    const float4* a = reinterpret_cast<const float4*>(acc + ((size_t)t * n_heads + head) * D);
+    const float4 l0 = a[2 * c], l1 = a[2 * c + 1], h0 = a[2 * (CH + c)], h1 = a[2 * (CH + c) + 1];
+    const float al[8] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
+    const float ah[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      lo.v[e] = __float2bfloat16_rn(al[e] + __bfloat162float(blo.v[e]));
+      hi.v[e] = __float2bfloat16_rn(ah[e] + __bfloat162float(bhi.v[e]));
+    }
+  } else {
+    lo = reinterpret_cast<const BF8*>(h)[c];
+    hi = reinterpret_cast<const BF8*>(h)[CH + c];
+  }
   if (head < n_q + n_kv) {
     if constexpr (QKNORM) {
       float ss = 0.f;
@@ -732,7 +762,12 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
       kb[c * KV_BLOCK + off] = lo;        // K layout: [chunk = d/8][token][8]
       kb[(CH + c) * KV_BLOCK + off] = hi;
     }
-  } else if (slot >= 0) {
+  } else {
+    if constexpr (BIAS) {
+      reinterpret_cast<BF8*>(h)[c] = lo;
+      reinterpret_cast<BF8*>(h)[CH + c] = hi;
+    }
+    if (slot < 0) return;
     const int kvh = head - n_q - n_kv;
     const int blk = slot / KV_BLOCK, off = slot % KV_BLOCK;
     BF8* vb = reinterpret_cast<BF8*>(v_cache + ((size_t)blk * n_kv + kvh) * (KV_BLOCK * D) + (size_t)off * D);
@@ -748,18 +783,35 @@ cudaError_t rope_kvwrite_launch(__nv_bfloat16* qkv, const int32_t* positions, co
   if (T <= 0) return cudaSuccess;
   const int n_heads = n_q + 2 * n_kv;
   const __nv_bfloat16* none = nullptr;
+  const float* no_acc = nullptr;
   if (q_norm || k_norm) {
     if (head_dim != 128 || !q_norm || !k_norm) return cudaErrorInvalidValue;
     return launch_k(rope_kvwrite_kernel<128, true>, dim3(T, (n_heads + 15) / 16), dim3(128), 0, stream, qkv, positions,
-                    slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, q_norm, k_norm, eps);
+                    slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, q_norm, k_norm, eps, no_acc, none);
   }
   if (head_dim == 64)
     return launch_k(rope_kvwrite_kernel<64>, dim3(T, (n_heads + 31) / 32), dim3(128), 0, stream, qkv, positions,
-                    slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, none, none, 0.f);
+                    slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, none, none, 0.f, no_acc, none);
   if (head_dim != 128) return cudaErrorInvalidValue;
   dim3 grid(T, (n_heads + 15) / 16);
   return launch_k(rope_kvwrite_kernel<128>, grid, dim3(128), 0, stream, qkv, positions, slot_mapping, cos_sin, k_cache,
-                  v_cache, n_q, n_kv, none, none, 0.f);
+                  v_cache, n_q, n_kv, none, none, 0.f, no_acc, none);
+}
+
+cudaError_t rope_kvwrite_bias_launch(const float* acc, const __nv_bfloat16* bias, __nv_bfloat16* qkv,
+                                     const int32_t* positions, const int32_t* slot_mapping,
+                                     const __nv_bfloat16* cos_sin, __nv_bfloat16* k_cache, __nv_bfloat16* v_cache,
+                                     int T, int n_q, int n_kv, cudaStream_t stream, int head_dim) {
+  if (T <= 0) return cudaSuccess;
+  if (!acc || !bias) return cudaErrorInvalidValue;
+  const int n_heads = n_q + 2 * n_kv;
+  const __nv_bfloat16* none = nullptr;
+  if (head_dim == 64)
+    return launch_k(rope_kvwrite_kernel<64, false, true>, dim3(T, (n_heads + 31) / 32), dim3(128), 0, stream, qkv,
+                    positions, slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, none, none, 0.f, acc, bias);
+  if (head_dim != 128) return cudaErrorInvalidValue;
+  return launch_k(rope_kvwrite_kernel<128, false, true>, dim3(T, (n_heads + 15) / 16), dim3(128), 0, stream, qkv,
+                  positions, slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, none, none, 0.f, acc, bias);
 }
 
 }  // namespace tgis

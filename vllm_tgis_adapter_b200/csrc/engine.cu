@@ -244,6 +244,11 @@ struct tgis_engine {
   // qk_norm_loaded: per layer, bit 0 = q_norm, bit 1 = k_norm
   DevBuf<bf16> qk_norm_w;
   std::vector<uint8_t> qk_norm_loaded;
+  // Qwen2 (tgis_engine_set_qkv_bias): layer l's q | k | v bias [qkv_dim] at qkv_bias_w + qkv_dim l, in wqkv's row order
+  // and an allocation of its own (the qkv GEMM then writes fp32 to y32); qkv_bias_loaded: per layer, bit 0 = q, 1 = k,
+  // 2 = v
+  DevBuf<bf16> qkv_bias_w;
+  std::vector<uint8_t> qkv_bias_loaded;
   // OPT (opt.cu): learned positions [max_model_len + 2, hidden], final LayerNorm bias; model head dim (64 or 128: every
   // head is zero-padded to the 128-dim attention tiles at load time); fp32 GEMM accumulators of the biased projections
   bool opt = false;
@@ -996,6 +1001,13 @@ struct tgis_engine {
         full(qk_norm_w.p + (size_t)li * 2 * HEAD_DIM + k * HEAD_DIM, HEAD_DIM, 1);
         if (rows * cols == HEAD_DIM) qk_norm_loaded[li] |= 1 << k;
       }
+      else if (qkv_bias_w.p && (sub == "self_attn.q_proj.bias" || sub == "self_attn.k_proj.bias" ||
+                                sub == "self_attn.v_proj.bias")) {
+        const int k = sub[10] == 'q' ? 0 : sub[10] == 'k' ? 1 : 2;
+        const int64_t n = k == 0 ? q_dim : kvd;
+        full(qkv_bias_w.p + (size_t)li * qkv_dim + (k == 0 ? 0 : q_dim + (k - 1) * kvd), n, 1);
+        if (rows * cols == n) qkv_bias_loaded[li] |= 1 << k;
+      }
       else return fail("unknown layer weight " + name);
     } else {
       return fail("unknown weight " + name);
@@ -1107,6 +1119,14 @@ struct tgis_engine {
         throw CudaError("q/k norm (Qwen3) weights missing: layer " + std::to_string(li) + " has no " +
                         (qk_norm_loaded[li] & 1 ? "" : "model.layers." + std::to_string(li) + ".self_attn.q_norm.weight ") +
                         (qk_norm_loaded[li] & 2 ? "" : "model.layers." + std::to_string(li) + ".self_attn.k_norm.weight"));
+    for (size_t li = 0; li < qkv_bias_loaded.size(); ++li)
+      if (qkv_bias_loaded[li] != 7) {
+        std::string missing;
+        for (int k = 0; k < 3; ++k)
+          if (!(qkv_bias_loaded[li] & (1 << k)))
+            missing += " model.layers." + std::to_string(li) + ".self_attn." + "qkv"[k] + "_proj.bias";
+        throw CudaError("qkv bias (Qwen2) missing: layer " + std::to_string(li) + " has no" + missing);
+      }
     if (!lm_head_loaded)  // tie_word_embeddings (tp == 1: with the zero padding rows)
       CK(cudaMemcpy(lm_head, embed + (size_t)rank * Vl * cfg.hidden, (size_t)(tp == 1 ? Vpad : Vl) * cfg.hidden * sizeof(bf16),
                     cudaMemcpyDeviceToDevice));
@@ -1220,9 +1240,10 @@ struct tgis_engine {
       n_launches += 2;
     };
     if (lora) ++lora_steps;
-    // (the fused epilogue exists for 128-dim heads without a q/k norm only: 64-dim heads and Qwen3 always take
-    // rope_kvwrite, one more launch per layer)
-    const bool rope_fused = !lora && fuse_rope && kv_head_dim == HEAD_DIM && !qk_norm_w.p && !cfg.debug_gemm_ref &&
+    // (the fused epilogue exists for 128-dim heads without a q/k norm or a qkv bias only: 64-dim heads, Qwen3 and Qwen2
+    // always take rope_kvwrite, one more launch per layer)
+    const bool rope_fused = !lora && fuse_rope && kv_head_dim == HEAD_DIM && !qk_norm_w.p && !qkv_bias_w.p &&
+                            !cfg.debug_gemm_ref &&
                             gemm_even_split(T, qkv_dim, H, num_sms) >= 2 &&
                             T <= (qkv_cluster > 0 ? std::max(rope_fuse_max_t, rope_fuse_cluster_max_t) : rope_fuse_max_t);
     for (int li = 0; li < (opt ? 0 : c.n_layers); ++li) {  // Llama stack (OPT: opt_layers() above)
@@ -1239,7 +1260,16 @@ struct tgis_engine {
         }
         const GemmRope rp{ds<int32_t>(off_pos), ds<int32_t>(off_slotmap), cos_sin,
                           k_cache.p + (size_t)li * kv_layer_elems, v_cache.p + (size_t)li * kv_layer_elems, nq, nkv};
-        gemm(xm_xn, l.m_qkv, xn.p, l.wqkv, qkv.p, T, qkv_dim, H, 0, 0, rope_fused ? &rp : nullptr);
+        // Qwen2: the projection leaves fp32 accumulators in y32, and the bias is added before the one rounding to bf16
+        // (by the writer below; on LoRA steps first, as the deltas land on the biased output, vllm
+        // MergedQKVParallelLinearWithLoRA)
+        const bf16* qb = qkv_bias_w.p ? qkv_bias_w.p + (size_t)li * qkv_dim : nullptr;
+        gemm(xm_xn, l.m_qkv, xn.p, l.wqkv, qb ? (void*)y32.p : (void*)qkv.p, T, qkv_dim, H, qb ? 1 : 0, 0,
+             rope_fused ? &rp : nullptr);
+        if (qb && lora) {
+          CK(opt_bias_act_launch(y32.p, qkv_dim, qb, qkv.p, qkv_dim, T, qkv_dim, /*relu=*/0, num_sms, stream));
+          ++n_launches;
+        }
         if (lora) {
           const LoraLayerW& ll = lora_layers[li];
           LoraGroup g{};
@@ -1256,8 +1286,12 @@ struct tgis_engine {
       if (!rope_fused) {
         // Qwen3: the q / k norm runs on the raw projections, LoRA deltas included (vllm models/qwen3.py)
         const bf16* qn = qk_norm_w.p ? qk_norm_w.p + (size_t)li * 2 * HEAD_DIM : nullptr;
-        CK(rope_kvwrite_launch(qkv.p, ds<int32_t>(off_pos), ds<int32_t>(off_slotmap), cos_sin, kc, vc, T, nq, nkv,
-                               stream, kv_head_dim, qn, qn ? qn + HEAD_DIM : nullptr, c.rms_eps));
+        if (qkv_bias_w.p && !lora)
+          CK(rope_kvwrite_bias_launch(y32.p, qkv_bias_w.p + (size_t)li * qkv_dim, qkv.p, ds<int32_t>(off_pos),
+                                      ds<int32_t>(off_slotmap), cos_sin, kc, vc, T, nq, nkv, stream, kv_head_dim));
+        else
+          CK(rope_kvwrite_launch(qkv.p, ds<int32_t>(off_pos), ds<int32_t>(off_slotmap), cos_sin, kc, vc, T, nq, nkv,
+                                 stream, kv_head_dim, qn, qn ? qn + HEAD_DIM : nullptr, c.rms_eps));
         ++n_launches;
       }
       if (n_dec > 0) {
@@ -2161,9 +2195,12 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
   }
   if (cfg->n_kv_heads <= 0 || cfg->n_q_heads % cfg->n_kv_heads != 0) return fail("n_q_heads must be a multiple of n_kv_heads");
   const int G = cfg->n_q_heads / cfg->n_kv_heads;
-  if (!(G == 1 || G == 2 || G == 3 || G == 4 || G == 8)) return fail("GQA group size must be 1, 2, 3, 4 or 8");
+  // decode attention is instantiated for every group of 1..8 at 128-dim heads and for all but 3 at 64-dim heads (the
+  // query heads of a group share one 8-wide MMA tile, hence the upper bound)
+  if (G < 1 || G > 8) return fail("GQA group size must be 1 to 8 (n_q_heads / n_kv_heads)");
   if (cfg->arch == TGIS_ARCH_LLAMA && cfg->head_dim == 64 && G == 3)
-    return fail("head_dim 64: GQA group size must be 1, 2, 4 or 8");
+    return fail("head_dim 64: GQA group size must be 1, 2, 4 or 8, or 5, 6 or 7 (group 3 is not instantiated for "
+                "64-dim heads)");
   if (cfg->hidden % 64 || cfg->ffn % 64) return fail("hidden/ffn must be multiples of 64");
   if (cfg->vocab < 1) return fail("vocab must be positive");
   if (cfg->hidden > 8192) return fail("hidden > 8192 unsupported");
@@ -2246,6 +2283,7 @@ int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on) {
   if (e->opt) return fail("q/k norm (Qwen3) applies to the Llama layer stack only, not OPT");
   if (e->kv_head_dim != HEAD_DIM) return fail("q/k norm (Qwen3) needs head_dim 128");
   if (e->tp > 1) return fail("q/k norm (Qwen3) is supported on a single GPU only (tp_size must be 1)");
+  if (e->qkv_bias_w.p) return fail("qkv bias (Qwen2) and q/k norm (Qwen3) cannot be combined");
   if (e->qk_norm_w.p) return 0;
   try {
     CK(cudaSetDevice(e->cfg.device));
@@ -2254,6 +2292,31 @@ int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on) {
     return fail(ex.what());
   }
   e->qk_norm_loaded.assign(e->cfg.n_layers, 0);
+  return 0;
+}
+
+int tgis_engine_set_qkv_bias(tgis_engine* e, int32_t on) {
+  if (!e) return fail("null engine");
+  if (e->started) return fail("the qkv bias must be set before tgis_engine_start");
+  if (!on) {
+    if (e->qkv_bias_w.p) cudaFree(e->qkv_bias_w.p);
+    e->qkv_bias_w.p = nullptr;
+    e->qkv_bias_loaded.clear();
+    return 0;  // (y32 stays: it is scratch)
+  }
+  if (e->opt) return fail("qkv bias (Qwen2) applies to the Llama layer stack only: OPT has its own bias path");
+  if (e->tp > 1) return fail("qkv bias (Qwen2) is supported on a single GPU only (tp_size must be 1)");
+  if (e->qk_norm_w.p) return fail("qkv bias (Qwen2) and q/k norm (Qwen3) cannot be combined");
+  if (e->qkv_bias_w.p) return 0;
+  try {
+    CK(cudaSetDevice(e->cfg.device));
+    if (!e->y32.p) e->y32.alloc((size_t)std::max(e->T_max, 256) * e->qkv_dim);  // the activations' T_alloc rows
+    e->qkv_bias_loaded.assign(e->cfg.n_layers, 0);
+    e->qkv_bias_w.alloc((size_t)e->cfg.n_layers * e->qkv_dim);
+  } catch (const std::exception& ex) {
+    e->qkv_bias_loaded.clear();
+    return fail(ex.what());
+  }
   return 0;
 }
 

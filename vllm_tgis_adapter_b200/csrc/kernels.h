@@ -188,6 +188,14 @@ cudaError_t rope_kvwrite_launch(__nv_bfloat16* qkv, const int32_t* positions, co
                                 int n_q, int n_kv, cudaStream_t stream, int head_dim = HEAD_DIM,
                                 const __nv_bfloat16* q_norm = nullptr, const __nv_bfloat16* k_norm = nullptr,
                                 float eps = 0.f);
+// The same writer on the qkv GEMM's fp32 accumulators with a bias (Qwen2, head_dim 128 or 64): every element is rounded
+// once as bf16(acc + bias), then q / k are rotated and the heads written to qkv and the caches as above.  acc fp32 [T,
+// (n_q + 2 n_kv) * head_dim], bias bf16 [(n_q + 2 n_kv) * head_dim].  The result is bit for bit that of
+// opt_bias_act_launch(acc, ..., relu = 0) into qkv followed by rope_kvwrite_launch.
+cudaError_t rope_kvwrite_bias_launch(const float* acc, const __nv_bfloat16* bias, __nv_bfloat16* qkv,
+                                     const int32_t* positions, const int32_t* slot_mapping,
+                                     const __nv_bfloat16* cos_sin, __nv_bfloat16* k_cache, __nv_bfloat16* v_cache,
+                                     int T, int n_q, int n_kv, cudaStream_t stream, int head_dim = HEAD_DIM);
 
 // ---- attention.cu ------------------------------------------------------------------------------------------------
 struct AttnSeq {        // one entry per sequence scheduled this step (device array)

@@ -215,6 +215,33 @@ int tgis_k_rope_kv_qknorm(void* qkv_dev, const int32_t* positions_host, const in
   return 0;
 }
 
+int tgis_k_rope_kv_bias(int32_t head_dim, const void* acc_dev, const void* bias_dev, void* qkv_dev,
+                        const int32_t* positions_host, const int32_t* slot_mapping_host, const void* cos_sin_dev,
+                        void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q, int32_t n_kv, int32_t iters,
+                        float* us_out) {
+  if (!acc_dev || !bias_dev) return kfail("acc and bias are required");
+  Tmp<int32_t> pos, sm;
+  KCK(pos.upload(positions_host, T));
+  KCK(sm.upload(slot_mapping_host, T));
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  KCK(cudaEventCreate(&e0));
+  KCK(cudaEventCreate(&e1));
+  cudaError_t err = cudaEventRecord(e0, 0);
+  for (int i = 0; i < std::max(iters, 1) && err == cudaSuccess; ++i)
+    err = rope_kvwrite_bias_launch((const float*)acc_dev, (const bf16*)bias_dev, (bf16*)qkv_dev, pos.p, sm.p,
+                                   (const bf16*)cos_sin_dev, (bf16*)k_cache_dev, (bf16*)v_cache_dev, T, n_q, n_kv, 0,
+                                   head_dim);
+  if (err == cudaSuccess) err = cudaEventRecord(e1, 0);
+  if (err == cudaSuccess) err = cudaDeviceSynchronize();
+  float ms = 0.f;
+  if (err == cudaSuccess) err = cudaEventElapsedTime(&ms, e0, e1);
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  if (err != cudaSuccess) return kfail(std::string("rope_kvwrite (qkv bias): ") + cudaGetErrorString(err));
+  if (us_out) *us_out = ms * 1000.f / std::max(iters, 1);
+  return 0;
+}
+
 int tgis_k_rope_kv(void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,
                    const void* cos_sin_dev, void* k_cache_dev, void* v_cache_dev, int32_t T, int32_t n_q, int32_t n_kv) {
   return tgis_k_rope_kv_hd(HEAD_DIM, qkv_dev, positions_host, slot_mapping_host, cos_sin_dev, k_cache_dev, v_cache_dev, T,

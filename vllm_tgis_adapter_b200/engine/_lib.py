@@ -70,7 +70,7 @@ class TgisStatus(C.Structure):
 # Every symbol include/tgis_engine.h and include/tgis_kernels.h declare (tests/test_abi_cpu.py checks the export list)
 ENGINE_SYMBOLS = [
     "tgis_last_error", "tgis_abi_version", "tgis_engine_create", "tgis_engine_load_weight", "tgis_engine_set_model_scalars",
-    "tgis_engine_require_rope_table", "tgis_engine_set_qk_norm", "tgis_engine_set_sliding_window", "tgis_engine_set_prefix_caching", "tgis_engine_prefix_cache_stats", "tgis_engine_start",
+    "tgis_engine_require_rope_table", "tgis_engine_set_qk_norm", "tgis_engine_set_qkv_bias", "tgis_engine_set_sliding_window", "tgis_engine_set_prefix_caching", "tgis_engine_prefix_cache_stats", "tgis_engine_start",
     "tgis_engine_add_request", "tgis_engine_abort", "tgis_engine_set_mask_provider", "tgis_engine_load_adapter_weight", "tgis_engine_clear_adapter", "tgis_engine_poll", "tgis_engine_status",
     "tgis_engine_max_model_len", "tgis_engine_set_profiling", "tgis_nccl_unique_id", "tgis_engine_worker_run", "tgis_engine_shutdown", "tgis_engine_destroy", "tgis_engine_run_until_idle",
 ]
@@ -82,6 +82,7 @@ KERNEL_SYMBOLS = [
     "tgis_k_rope_kv_qknorm", "tgis_k_tp_area_bytes", "tgis_k_tp_exchange", "tgis_k_logits_push", "tgis_k_logits_wait",
     "tgis_k_gather_relayout", "tgis_k_tp_exchange_check", "tgis_k_logits_wait_check",
     "tgis_k_attention_window", "tgis_k_attention_bench_window", "tgis_k_decode_items_window",
+    "tgis_k_rope_kv_bias",
 ]
 
 _LIB: C.CDLL | None = None
@@ -118,6 +119,7 @@ def load_library() -> C.CDLL:
     lib.tgis_engine_set_model_scalars.argtypes = [vp, f32, f32, f32, f32]
     lib.tgis_engine_require_rope_table.argtypes = [vp]
     lib.tgis_engine_set_qk_norm.argtypes = [vp, i32]
+    lib.tgis_engine_set_qkv_bias.argtypes = [vp, i32]
     lib.tgis_engine_set_sliding_window.argtypes = [vp, i32]
     lib.tgis_engine_set_prefix_caching.argtypes = [vp, i32]
     lib.tgis_engine_prefix_cache_stats.argtypes = [vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i32)]
@@ -157,6 +159,8 @@ def load_library() -> C.CDLL:
     lib.tgis_k_rope_kv_hd.argtypes = [i32, vp, C.POINTER(i32), C.POINTER(i32), vp, vp, vp, i32, i32, i32]
     lib.tgis_k_rope_kv_qknorm.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), vp, vp, vp, i32, i32, i32, vp, vp, f32, i32,
                                           C.POINTER(f32)]
+    lib.tgis_k_rope_kv_bias.argtypes = [i32, vp, vp, vp, C.POINTER(i32), C.POINTER(i32), vp, vp, vp, i32, i32, i32, i32,
+                                        C.POINTER(f32)]
     lib.tgis_k_attention_hd.argtypes = [i32, vp, vp, vp, C.POINTER(i32), i32, C.POINTER(i32), i32, i32, vp, i32, i32, f32]
     lib.tgis_k_attention_split_hd.argtypes = [i32, vp, vp, vp, C.POINTER(i32), i32, C.POINTER(i32), i32, i32, vp, i32, i32,
                                               f32, i32]

@@ -29,7 +29,10 @@ class ModelConfig:
     per-layer weights self_attn.q_norm / k_norm (tgis_engine_set_qk_norm; head_dim 128, single GPU).
 
     Mistral (MistralForCausalLM) is arch "llama" with sliding_window set: every layer's query at position p attends to
-    the keys p - sliding_window < k <= p (tgis_engine_set_sliding_window; single GPU)."""
+    the keys p - sliding_window < k <= p (tgis_engine_set_sliding_window; single GPU).
+
+    Qwen2 / Qwen2.5 (Qwen2ForCausalLM) is arch "llama" with qkv_bias set: a bias on the q, k and v projections, added to
+    the fp32 accumulators before the one rounding to bf16 (tgis_engine_set_qkv_bias; head_dim 128 or 64, single GPU)."""
 
     n_layers: int        # num_hidden_layers
     hidden: int          # hidden_size
@@ -53,6 +56,7 @@ class ModelConfig:
     rope_original_max_pos: int = 8192   # original_max_position_embeddings
     qk_norm: bool = False               # Qwen3: per-head RMSNorm of q and k (self_attn.q_norm / k_norm)
     sliding_window: int | None = None   # Mistral: keys per query, itself included, in every layer; None = all
+    qkv_bias: bool = False              # Qwen2: self_attn.{q,k,v}_proj.bias
 
     @property
     def rope_scaled(self) -> bool:
@@ -125,6 +129,26 @@ PRESETS: dict[str, ModelConfig] = {
                                    rope_theta=1000000.0, rms_eps=1e-5, max_model_len=8192),
     "mistral-nemo-12b": ModelConfig(n_layers=40, hidden=5120, n_q_heads=32, n_kv_heads=8, ffn=14336, vocab=131072,
                                     rope_theta=1000000.0, rms_eps=1e-5, max_model_len=8192),
+    # Qwen2 / Qwen2.5: two CPU-oracle-sized stacks with GQA groups of 6 (128-dim heads) and 7 (64-dim heads), q widths
+    # that are not their hidden sizes and an odd vocabulary, and the Qwen2.5 0.5B, 1.5B, 7B and 14B shapes.  Those four are
+    # the published Qwen/Qwen2.5-* config.json values as recalled, not checked against the files when these presets were
+    # written.
+    "qwen2-tiny": ModelConfig(n_layers=2, hidden=768, n_q_heads=6, n_kv_heads=1, ffn=1024, vocab=1021,
+                              rope_theta=1000000.0, rms_eps=1e-6, max_model_len=2048, tie_word_embeddings=True,
+                              qkv_bias=True),
+    "qwen2-tiny-hd64": ModelConfig(n_layers=2, hidden=448, n_q_heads=7, n_kv_heads=1, ffn=512, vocab=1021, head_dim=64,
+                                   rope_theta=1000000.0, rms_eps=1e-6, max_model_len=2048, tie_word_embeddings=True,
+                                   qkv_bias=True),
+    "qwen2.5-0.5b": ModelConfig(n_layers=24, hidden=896, n_q_heads=14, n_kv_heads=2, ffn=4864, vocab=151936, head_dim=64,
+                                rope_theta=1000000.0, rms_eps=1e-6, max_model_len=8192, tie_word_embeddings=True,
+                                qkv_bias=True),
+    "qwen2.5-1.5b": ModelConfig(n_layers=28, hidden=1536, n_q_heads=12, n_kv_heads=2, ffn=8960, vocab=151936,
+                                rope_theta=1000000.0, rms_eps=1e-6, max_model_len=8192, tie_word_embeddings=True,
+                                qkv_bias=True),
+    "qwen2.5-7b": ModelConfig(n_layers=28, hidden=3584, n_q_heads=28, n_kv_heads=4, ffn=18944, vocab=152064,
+                              rope_theta=1000000.0, rms_eps=1e-6, max_model_len=8192, qkv_bias=True),
+    "qwen2.5-14b": ModelConfig(n_layers=48, hidden=5120, n_q_heads=40, n_kv_heads=8, ffn=13824, vocab=152064,
+                               rope_theta=1000000.0, rms_eps=1e-5, max_model_len=8192, qkv_bias=True),
 }
 
 
@@ -220,6 +244,9 @@ class NativeEngine:
         if model.sliding_window and tp_size > 1:
             raise EngineError("sliding-window attention (Mistral) is not supported with tensor parallelism: it is "
                               "implemented on a single GPU only (use tensor_parallel_size 1)")
+        if model.qkv_bias and tp_size > 1:
+            raise EngineError("Qwen2 (qkv_bias) is not supported with tensor parallelism: the qkv bias is implemented on a "
+                              "single GPU only (use tensor_parallel_size 1)")
         if model.arch not in ("llama", "opt"):
             raise EngineError(f"unknown architecture {model.arch!r}")
         if model.arch == "llama" and model.head_dim != 128 and model.is_granite:
@@ -249,6 +276,10 @@ class NativeEngine:
             msg = _lib.last_error(self.lib)
             self.close()
             raise EngineError(f"tgis_engine_set_qk_norm failed: {msg}")
+        if model.qkv_bias and self.lib.tgis_engine_set_qkv_bias(self._h, 1) != 0:
+            msg = _lib.last_error(self.lib)
+            self.close()
+            raise EngineError(f"tgis_engine_set_qkv_bias failed: {msg}")
         if model.sliding_window and self.lib.tgis_engine_set_sliding_window(self._h, int(model.sliding_window)) != 0:
             msg = _lib.last_error(self.lib)
             self.close()

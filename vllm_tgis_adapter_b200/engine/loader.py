@@ -30,6 +30,14 @@ def model_config_from_hf(path: Path, max_model_len: int | None) -> ModelConfig:
         return _qwen3_model_config(cfg, max_model_len)
     if cfg.get("model_type") == "mistral" or "MistralForCausalLM" in archs:
         return _mistral_model_config(cfg, max_model_len)
+    if cfg.get("model_type") == "qwen2" or "Qwen2ForCausalLM" in archs:
+        if cfg.get("attention_bias") is False:
+            # Qwen2's q / k / v projections always carry a bias (transformers and vLLM hard-code bias=True; Qwen2Config
+            # has no attention_bias key).  A config that declares bias-free projections was written for another
+            # architecture (a Llama- or Qwen3-style one) and its checkpoint has no bias tensors to load.
+            raise ValueError(f"unsupported model architecture {archs or cfg.get('model_type')}: attention_bias false "
+                             "declares projections without biases, but Qwen2ForCausalLM always has q/k/v biases")
+        return _qwen2_model_config(cfg, max_model_len)
     if cfg.get("model_type") != "llama" and not any("Llama" in a for a in archs):
         raise ValueError(f"unsupported model architecture {archs or cfg.get('model_type')}: only Llama-family "
                          "decoders (RMSNorm, RoPE, GQA, SwiGLU) and OPT are implemented")
@@ -165,6 +173,47 @@ def _mistral_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
                        **scaling)
 
 
+def _qwen2_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
+    """Qwen/Qwen2-* and Qwen2.5-* Qwen2ForCausalLM config.json -> the Llama stack with a bias on the q, k and v
+    projections (vllm model_executor/models/qwen2.py).  Where vLLM and transformers' defaults differ, vLLM's are taken:
+    head_dim is hidden_size // num_attention_heads, and a config without a rotary theta gets 1e6.  Variants the engine
+    would serve wrongly are refused, each with its reason; the rotary embedding is read as for Llama (_llama_rope: yarn
+    and the other scaled types are refused by name)."""
+    hidden, heads = cfg["hidden_size"], cfg["num_attention_heads"]
+    head_dim = hidden // heads
+    problems = []
+    if cfg.get("head_dim") not in (None, head_dim):
+        problems.append(f"head_dim {cfg['head_dim']} != hidden_size // num_attention_heads = {head_dim} (vLLM computes "
+                        "the latter, transformers reads the former: the two would build different models)")
+    if head_dim not in (64, 128):
+        problems.append(f"head_dim {head_dim} (the attention kernels exist for 64 and 128)")
+    if cfg.get("use_sliding_window"):
+        problems.append("use_sliding_window (every layer attends to the whole context here)")
+    other = sorted({t for t in cfg.get("layer_types") or [] if t != "full_attention"})
+    if other:
+        problems.append(f"layer_types {other} (only full_attention is implemented)")
+    if cfg.get("qk_norm"):
+        problems.append("qk_norm (a q/k norm together with the qkv bias is not implemented)")
+    if cfg.get("is_causal") is False:
+        problems.append("is_causal false (bidirectional embedding models are not generative)")
+    if cfg.get("dual_chunk_attention_config"):
+        problems.append("dual_chunk_attention_config (dual-chunk attention is not implemented)")
+    if problems:
+        raise ValueError("unsupported Qwen2 variant: " + "; ".join(problems))
+    rope = cfg.get("rope_parameters") or cfg.get("rope_scaling") or {}
+    if not (rope.get("rope_theta") or cfg.get("rope_theta")):
+        cfg = {**cfg, "rope_theta": 1000000.0}   # vllm qwen2.py: set_default_rope_theta(config, 1000000)
+    theta, scaling = _llama_rope(cfg)
+    derived = cfg.get("max_position_embeddings", 32768)
+    if max_model_len is not None and max_model_len > derived:
+        raise ValueError(f"max_model_len {max_model_len} exceeds the model's max_position_embeddings {derived}")
+    return ModelConfig(n_layers=cfg["num_hidden_layers"], hidden=hidden, n_q_heads=heads,
+                       n_kv_heads=cfg.get("num_key_value_heads", heads), ffn=cfg["intermediate_size"],
+                       vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=theta,
+                       rms_eps=float(cfg.get("rms_norm_eps", 1e-6)), max_model_len=max_model_len or min(derived, 8192),
+                       tie_word_embeddings=bool(cfg.get("tie_word_embeddings", False)), qkv_bias=True, **scaling)
+
+
 def _opt_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
     """facebook/opt-* config.json -> ModelConfig(arch="opt").  The variants vLLM's OPT model handles with extra modules
     (opt-350m: post-LayerNorm + project_in/out) are refused rather than silently mis-served."""
@@ -247,6 +296,10 @@ def load_synthetic_weights(eng: NativeEngine, mc: ModelConfig, seed: int, device
         if mc.qk_norm:   # Qwen3: per-head norm weights of one head's width
             eng.load_weight(p + "self_attn.q_norm.weight", ones[:mc.head_dim])
             eng.load_weight(p + "self_attn.k_norm.weight", ones[:mc.head_dim])
+        if mc.qkv_bias:  # Qwen2: projection biases (random: HF's init has zeros, which would not exercise the bias path)
+            for m, n in (("q_proj", q_dim), ("k_proj", kv_dim), ("v_proj", kv_dim)):
+                b = torch.randn(n, generator=gen, device=f"cuda:{device}", dtype=torch.float32) * 0.1
+                eng.load_weight(p + f"self_attn.{m}.bias", b.to(torch.bfloat16))
 
 
 def load_safetensors_dir(eng: NativeEngine, path: Path) -> None:
@@ -327,6 +380,8 @@ def build_engine(args) -> AsyncTGISEngine:
         raise ValueError(f"Qwen3 (per-head q/k norm) is supported on a single GPU only: tensor_parallel_size {tp}")
     if tp > 1 and mc.sliding_window:
         raise ValueError(f"Mistral (sliding-window attention) is supported on a single GPU only: tensor_parallel_size {tp}")
+    if tp > 1 and mc.qkv_bias:
+        raise ValueError(f"Qwen2 (qkv bias) is supported on a single GPU only: tensor_parallel_size {tp}")
     if tp > 1:
         import multiprocessing as mp
         import os
