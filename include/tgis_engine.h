@@ -67,7 +67,8 @@ typedef struct tgis_config {
   int32_t n_q_heads;
   int32_t n_kv_heads;
   int32_t head_dim; /* 128 or 64 (LLAMA 64: native 64-dim KV tiles, tp_size 1, max_loras 0, no Granite scalars; OPT 64:
-                       zero-padded to the 128-dim tiles) */
+                       zero-padded to the 128-dim tiles); LLAMA also 96 (Phi-3-mini: native 96-dim KV tiles, tp_size 1,
+                       max_loras 0, GQA group 1, 2, 4 or 8, no Granite scalars, q/k norm or qkv bias) */
   int32_t ffn;
   int32_t vocab;              /* any size when tp_size == 1 (the lm_head is padded to a multiple of 8 internally) */
   float rope_theta;

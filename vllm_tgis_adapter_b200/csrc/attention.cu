@@ -2,6 +2,9 @@
 // vllm v1/attention/backends/flashinfer.py:1665,1803).  Causal, GQA, bf16 in / fp32 softmax.  The head dimension D is a
 // template parameter of every kernel here: 128 (the figures quoted in the comments) or 64, where a K / V tile is 4 KiB of
 // 8 chunks, every MMA loop over the head dimension is half as long and a decode warp's ring holds twice as many tiles.
+// D = 96 (Phi-3-mini): a tile is 6 KiB of 12 chunks (still one bulk copy), the MMA loops run over 6 / 12 steps, and the
+// V tile's chunk permutation is v_chunk<96> (kernels.h) instead of chunk ^ (tok & 7), which would leave the 192-byte row;
+// v_chunk<96> keeps every ldmatrix.trans matrix on 8 distinct bank groups.  A decode warp rings DEC_RING<96> tiles.
 //
 // HBM layout of the cache (ours to choose; see kernels.h): per (block, kv_head) one contiguous 8 KiB K tile stored
 // "8-dim chunk major" [16][32 tok][8] and one 8 KiB V tile [32 tok][16 chunks ^ (tok&7)][8].  Both tiles are fetched
@@ -97,8 +100,12 @@ constexpr int DEC_THREADS = DEC_WARPS * 32;
 #ifndef TGIS_DEC_MINB
 #define TGIS_DEC_MINB 2  // CTAs per SM (register cap); shared memory must agree: MINB * 4 * (RING * 8 + 2) KiB <= 227
 #endif
-// D = 64: twice the tiles of half the size, so a warp keeps the same 24 KiB in flight in the same shared-memory budget
-template <int D> constexpr int DEC_RING = TGIS_DEC_RING * (128 / D);
+#ifndef TGIS_DEC_RING96
+#define TGIS_DEC_RING96 4  // tile buffers per warp at D = 96 (4 x 6 KiB; 2 CTAs x 4 warps x 25.5 KiB fit the SM)
+#endif
+// D = 64: twice the tiles of half the size, so a warp keeps the same 24 KiB in flight in the same shared-memory budget.
+// D = 96: the formula would give 3 tiles (18 KiB); four keep 24 KiB in flight (DESIGN 3.13 measures both).
+template <int D> constexpr int DEC_RING = D == 96 ? TGIS_DEC_RING96 : TGIS_DEC_RING * (128 / D);
 template <int D> constexpr int DEC_Q_BYTES = 8 * D * 2;                                          // up to 8 heads
 template <int D> constexpr int DEC_WARP_SMEM = DEC_RING<D> * TILE_BYTES<D> + DEC_Q_BYTES<D>;     // 26 KiB (D = 64: 25)
 // + one mbarrier per ring buffer and one for Q, per warp
@@ -330,7 +337,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
           uint32_t va[2][4];
 #pragma unroll
           for (int u = 0; u < 2; ++u)
-            ldmatrix_x4_trans(va[u], v_base + tok * (D * 2) + (((2 * (md + u) + (mi & 1)) ^ (tok & 7)) * 16));
+            ldmatrix_x4_trans(va[u], v_base + tok * (D * 2) + (v_chunk<D>(2 * (md + u) + (mi & 1), tok) * 16));
           mma_bf16_16816(ot[md], va[0], bh[kk][0], bh[kk][1]);
           mma_bf16_16816(ot[md + 1], va[1], bh[kk][0], bh[kk][1]);
           mma_bf16_16816(ot[md], va[0], bl[kk][0], bl[kk][1]);
@@ -507,6 +514,13 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
       TGIS_DEC(64, 7);
       TGIS_DEC(64, 8);
     }
+  } else if (head_dim == 96) {
+    switch (G) {  // Phi-3 checkpoints are G = 1; 2, 4 and 8 cover the grouped path
+      TGIS_DEC(96, 1);
+      TGIS_DEC(96, 2);
+      TGIS_DEC(96, 4);
+      TGIS_DEC(96, 8);
+    }
   }
 #undef TGIS_DEC
   return cudaErrorInvalidValue;
@@ -674,7 +688,7 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
         const int tok = kk * 16 + (mi & 1) * 8 + ri;
         const int chunk = nd + (mi >> 1);
         uint32_t vb[4];
-        ldmatrix_x4_trans(vb, v_base + tok * (D * 2) + ((chunk ^ (tok & 7)) * 16));
+        ldmatrix_x4_trans(vb, v_base + tok * (D * 2) + (v_chunk<D>(chunk, tok) * 16));
         mma_bf16_16816(o[nd], pa[kk], vb[0], vb[1]);
         mma_bf16_16816(o[nd + 1], pa[kk], vb[2], vb[3]);
         mma_bf16_16816(o[nd], pl[kk], vb[0], vb[1]);
@@ -723,16 +737,31 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
     for (int i = 0; i < DPT; ++i) acc[i] = 0.f;
     float l_f = 0.f;
     const uint32_t po_addr = smem_u32(po + (size_t)idx * D + d0);
+    if constexpr (DPT % 4 == 0) {
 #pragma unroll
-    for (int k = 0; k < PF_CLUSTER; ++k) {
-      const float fs = (mlk[k].x == -INFINITY) ? 0.f : exp2f(mlk[k].x - m_f);
-      float4 a[DPT / 4];
+      for (int k = 0; k < PF_CLUSTER; ++k) {
+        const float fs = (mlk[k].x == -INFINITY) ? 0.f : exp2f(mlk[k].x - m_f);
+        float4 a[DPT / 4];
 #pragma unroll
-      for (int i = 0; i < DPT / 4; ++i) a[i] = ld_dsmem_f4(dsmem_addr(po_addr + 16 * i, k));
-      l_f += mlk[k].y * fs;
+        for (int i = 0; i < DPT / 4; ++i) a[i] = ld_dsmem_f4(dsmem_addr(po_addr + 16 * i, k));
+        l_f += mlk[k].y * fs;
 #pragma unroll
-      for (int i = 0; i < DPT / 4; ++i) {
-        acc[4 * i] += a[i].x * fs; acc[4 * i + 1] += a[i].y * fs; acc[4 * i + 2] += a[i].z * fs; acc[4 * i + 3] += a[i].w * fs;
+        for (int i = 0; i < DPT / 4; ++i) {
+          acc[4 * i] += a[i].x * fs; acc[4 * i + 1] += a[i].y * fs; acc[4 * i + 2] += a[i].z * fs; acc[4 * i + 3] += a[i].w * fs;
+        }
+      }
+    } else {  // D = 96: 6 dims per thread, 24 bytes apart, so 8-byte loads
+#pragma unroll
+      for (int k = 0; k < PF_CLUSTER; ++k) {
+        const float fs = (mlk[k].x == -INFINITY) ? 0.f : exp2f(mlk[k].x - m_f);
+        float2 a[DPT / 2];
+#pragma unroll
+        for (int i = 0; i < DPT / 2; ++i) a[i] = ld_dsmem_f2(dsmem_addr(po_addr + 8 * i, k));
+        l_f += mlk[k].y * fs;
+#pragma unroll
+        for (int i = 0; i < DPT / 2; ++i) {
+          acc[2 * i] += a[i].x * fs; acc[2 * i + 1] += a[i].y * fs;
+        }
       }
     }
     cluster_sync_all();  // no CTA leaves while a peer may still read its shared memory
@@ -746,6 +775,10 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
         pk.z = pack_bf16x2(acc[4] * inv, acc[5] * inv);
         pk.w = pack_bf16x2(acc[6] * inv, acc[7] * inv);
         *reinterpret_cast<uint4*>(dst) = pk;
+      } else if constexpr (D == 96) {  // 12 bytes at a 4-byte aligned offset
+        uint32_t* d32 = reinterpret_cast<uint32_t*>(dst);
+#pragma unroll
+        for (int i = 0; i < DPT / 2; ++i) d32[i] = pack_bf16x2(acc[2 * i] * inv, acc[2 * i + 1] * inv);
       } else {
         *reinterpret_cast<uint2*>(dst) =
             make_uint2(pack_bf16x2(acc[0] * inv, acc[1] * inv), pack_bf16x2(acc[2] * inv, acc[3] * inv));
@@ -774,8 +807,11 @@ cudaError_t attn_prefill_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv
   if (n_tiles <= 0) return cudaSuccess;
   if (n_q % n_kv != 0 || window < 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
-  if (G > 8 || (head_dim != 128 && head_dim != 64)) return cudaErrorInvalidValue;
+  if (G > 8 || (head_dim != 128 && head_dim != 64 && head_dim != 96)) return cudaErrorInvalidValue;
   dim3 grid(n_tiles, n_kv);
+  if (head_dim == 96)
+    return launch_k(attn_prefill_kernel<96, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
+                    tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
   if (head_dim == 64)
     return launch_k(attn_prefill_kernel<64, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
                     tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
@@ -822,6 +858,9 @@ cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, cons
                                        bt_stride, out, out_ld, n_kv, G, scale, stream, window);
   if (head_dim == 64)
     return prefill_split_launch_d<64>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
+                                      bt_stride, out, out_ld, n_kv, G, scale, stream, window);
+  if (head_dim == 96)
+    return prefill_split_launch_d<96>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
                                       bt_stride, out, out_ld, n_kv, G, scale, stream, window);
   return cudaErrorInvalidValue;
 }

@@ -651,6 +651,8 @@ cudaError_t silu_mul_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, in
 // (i..i+7, i+64..i+71): every global access is a 16-byte vector, and 8 consecutive dims are exactly one chunk of the
 // K / V cache layouts, so the scatter is one 16-byte store per half.
 // D = 64: 32 heads x 4 threads, pairs (i..i+7, i+32..i+39), 8 chunks per K / V row.
+// D = 96: 96 threads = 16 heads x 6 threads (6 does not divide 128), pairs (i..i+7, i+48..i+55), 12 chunks per row; the
+// V chunk goes through v_chunk<96> (kernels.h).  Plain variant only.
 //
 // QKNORM (Qwen3; D = 128 only): every q and k head is RMS-normalised over its 128 dims before the rotation, with
 // rmsnorm_kernel's rounding points: rs = rsqrtf(ss / 128 + eps), y = bf16(bf16(x * rs) * w), w = q_norm or k_norm [128].
@@ -663,6 +665,8 @@ cudaError_t silu_mul_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, in
 // element is first rounded once as bf16(acc + bias) (the fp32 add of F.linear with a bias, in model dtype; bias [(n_q +
 // 2 n_kv) * D] in qkv's q | k | v row order).  q and k are then rotated as above and written to qkv with the raw v, so
 // qkv and the caches hold exactly what opt_bias_act_kernel (no activation) followed by the plain writer leaves.
+template <int D> constexpr int ROPE_THREADS = D == 96 ? 96 : 128;  // a whole number of heads per CTA
+
 template <int D, bool QKNORM = false, bool BIAS = false>
 __global__ void __launch_bounds__(128)
 rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ positions,
@@ -672,6 +676,7 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
                     const float* __restrict__ acc, const __nv_bfloat16* __restrict__ bias) {
   static_assert(!QKNORM || D == 128, "the q / k norm variant exists for 128-dim heads");
   static_assert(!(QKNORM && BIAS), "no model has both a q / k norm and a qkv bias");
+  static_assert(D != 96 || (!QKNORM && !BIAS), "96-dim heads: plain variant only");
   griddep_launch();
   BF8 wlo, whi;  // QKNORM: this thread's 16 norm weights (static: read before the wait, as rmsnorm_kernel does)
   if constexpr (QKNORM) {
@@ -695,7 +700,7 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
   griddep_wait();
   const int t = blockIdx.x;
   constexpr int CH = D / 16;      // chunks per half of a head = threads per head
-  const int head = blockIdx.y * (128 / CH) + threadIdx.x / CH;
+  const int head = blockIdx.y * (ROPE_THREADS<D> / CH) + threadIdx.x / CH;
   const int c = threadIdx.x % CH;  // chunk of 8 pairs: dims [8c, 8c+8) and [D/2+8c, D/2+8c+8)
   const int n_heads = n_q + 2 * n_kv;
   if (head >= n_heads) return;
@@ -771,8 +776,8 @@ rope_kvwrite_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__
     const int kvh = head - n_q - n_kv;
     const int blk = slot / KV_BLOCK, off = slot % KV_BLOCK;
     BF8* vb = reinterpret_cast<BF8*>(v_cache + ((size_t)blk * n_kv + kvh) * (KV_BLOCK * D) + (size_t)off * D);
-    vb[c ^ (off & 7)] = lo;               // V layout: [token][16-byte chunk ^ (token & 7)][8]
-    vb[(CH + c) ^ (off & 7)] = hi;
+    vb[v_chunk<D>(c, off)] = lo;          // V layout: [token][16-byte chunk ^ (token & 7)][8] (D = 96: v_chunk<96>)
+    vb[v_chunk<D>(CH + c, off)] = hi;
   }
 }
 
@@ -792,6 +797,9 @@ cudaError_t rope_kvwrite_launch(__nv_bfloat16* qkv, const int32_t* positions, co
   if (head_dim == 64)
     return launch_k(rope_kvwrite_kernel<64>, dim3(T, (n_heads + 31) / 32), dim3(128), 0, stream, qkv, positions,
                     slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, none, none, 0.f, no_acc, none);
+  if (head_dim == 96)
+    return launch_k(rope_kvwrite_kernel<96>, dim3(T, (n_heads + 15) / 16), dim3(ROPE_THREADS<96>), 0, stream, qkv,
+                    positions, slot_mapping, cos_sin, k_cache, v_cache, n_q, n_kv, none, none, 0.f, no_acc, none);
   if (head_dim != 128) return cudaErrorInvalidValue;
   dim3 grid(T, (n_heads + 15) / 16);
   return launch_k(rope_kvwrite_kernel<128>, grid, dim3(128), 0, stream, qkv, positions, slot_mapping, cos_sin, k_cache,

@@ -2190,8 +2190,12 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
     // the 64-dim kernels are exercised on a single GPU without adapters; the other combinations are refused until tested
     if (cfg->tp_size > 1) return fail("head_dim 64 is supported on a single GPU only (tp_size must be 1)");
     if (cfg->max_loras > 0) return fail("head_dim 64: LoRA adapter slots are not supported (max_loras must be 0)");
+  } else if (cfg->head_dim == 96) {
+    // Phi-3-mini: on the same terms as 64
+    if (cfg->tp_size > 1) return fail("head_dim 96 is supported on a single GPU only (tp_size must be 1)");
+    if (cfg->max_loras > 0) return fail("head_dim 96: LoRA adapter slots are not supported (max_loras must be 0)");
   } else if (cfg->head_dim != HEAD_DIM) {
-    return fail("head_dim must be 128 or 64");
+    return fail("head_dim must be 128, 96 or 64");
   }
   if (cfg->n_kv_heads <= 0 || cfg->n_q_heads % cfg->n_kv_heads != 0) return fail("n_q_heads must be a multiple of n_kv_heads");
   const int G = cfg->n_q_heads / cfg->n_kv_heads;
@@ -2201,6 +2205,8 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
   if (cfg->arch == TGIS_ARCH_LLAMA && cfg->head_dim == 64 && G == 3)
     return fail("head_dim 64: GQA group size must be 1, 2, 4 or 8, or 5, 6 or 7 (group 3 is not instantiated for "
                 "64-dim heads)");
+  if (cfg->arch == TGIS_ARCH_LLAMA && cfg->head_dim == 96 && G != 1 && G != 2 && G != 4 && G != 8)
+    return fail("head_dim 96: GQA group size must be 1, 2, 4 or 8 (the groups instantiated for 96-dim heads)");
   if (cfg->hidden % 64 || cfg->ffn % 64) return fail("hidden/ffn must be multiples of 64");
   if (cfg->vocab < 1) return fail("vocab must be positive");
   if (cfg->hidden > 8192) return fail("hidden > 8192 unsupported");
@@ -2251,7 +2257,8 @@ int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, fl
                      logit_scale == 1.f;
   if (e->opt && !llama) return fail("model scalars (Granite) apply to the Llama layer stack only, not OPT");
   if (e->kv_head_dim != HEAD_DIM && !llama)
-    return fail("model scalars (Granite) need head_dim 128: Granite with 64-dim heads is not supported yet");
+    return fail("model scalars (Granite) need head_dim 128: Granite with " + std::to_string(e->kv_head_dim) +
+                "-dim heads is not supported yet");
   // the tensor-parallel exchange kernels (ar_add_rmsnorm / ar2_add_rmsnorm) and the NCCL path's norm do not implement
   // the residual multiplier
   if (e->tp > 1 && residual_multiplier != 1.f)
@@ -2307,6 +2314,7 @@ int tgis_engine_set_qkv_bias(tgis_engine* e, int32_t on) {
   if (e->opt) return fail("qkv bias (Qwen2) applies to the Llama layer stack only: OPT has its own bias path");
   if (e->tp > 1) return fail("qkv bias (Qwen2) is supported on a single GPU only (tp_size must be 1)");
   if (e->qk_norm_w.p) return fail("qkv bias (Qwen2) and q/k norm (Qwen3) cannot be combined");
+  if (e->kv_head_dim != HEAD_DIM && e->kv_head_dim != 64) return fail("qkv bias (Qwen2) needs head_dim 128 or 64");
   if (e->qkv_bias_w.p) return 0;
   try {
     CK(cudaSetDevice(e->cfg.device));

@@ -176,8 +176,22 @@ cudaError_t gather_rows_launch(const __nv_bfloat16* x, const int32_t* rows, __nv
 // two layouts at half the width, K [8 chunks][BLOCK][8] and V [BLOCK][8 chunks ^ (tok&7)][8], 4 KiB per tile; qkv rows are
 // (n_q + 2 n_kv) * 64 and cos_sin rows cos(32) | sin(32).  Any other head_dim, or a (head_dim, group size) pair that is not
 // instantiated, returns cudaErrorInvalidValue.  The GEMM's fused RoPE epilogue (GemmRope) and opt.cu are 128 only.
+// 96-dim heads (Phi-3-mini): K [12 chunks][BLOCK][8] and V [BLOCK][12 chunks, permuted by v_chunk][8], 6 KiB per tile;
+// qkv rows are (n_q + 2 n_kv) * 96 and cos_sin rows cos(48) | sin(48).
 constexpr int KV_BLOCK = 32;
 constexpr int HEAD_DIM = 128;
+
+// Physical 16-byte chunk of logical chunk c of token tok in a V tile row of D / 8 chunks.  D = 128 and 64: c ^ (tok & 7).
+// D = 96 (12 chunks): the xor would carry chunks 8..11 to 15 (into the next token's row), so chunks 0..7 keep the xor and
+// chunks 8..11 are xor-ed among themselves by (tok >> 1) & 3.  A 192-byte row puts physical chunk p of token t in 16-byte
+// bank group (4 (t & 1) + p) mod 8; for one logical chunk, the 8 rows of an ldmatrix matrix (8 consecutive tokens from
+// a multiple of 8) then land in 8 distinct bank groups: c < 8 gives (c ^ t) ^ 4 (t & 1), c >= 8 gives
+// 4 (t & 1) + ((c - 8) ^ ((t >> 1) & 3)), each a bijection of t & 7.  The writer and both readers index through this.
+template <int D>
+__device__ __forceinline__ int v_chunk(int c, int tok) {
+  if constexpr (D == 96) return c < 8 ? c ^ (tok & 7) : 8 + ((c - 8) ^ ((tok >> 1) & 3));
+  else return c ^ (tok & 7);
+}
 
 // neox RoPE on q,k in-place inside qkv[T, (nq+2nkv)*128] and scatter of k,v into the paged cache.
 // cos_sin: [max_pos][128] bf16 = cos(64) | sin(64)   (vllm: rotary_embedding/base.py cache.to(dtype))

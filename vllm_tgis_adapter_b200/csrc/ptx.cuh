@@ -269,6 +269,11 @@ __device__ __forceinline__ uint32_t dsmem_addr(uint32_t local_smem_addr, uint32_
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(local_smem_addr), "r"(cta_rank));
   return r;
 }
+__device__ __forceinline__ float2 ld_dsmem_f2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared::cluster.v2.f32 {%0,%1}, [%2];\n" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
 __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];\n"

@@ -358,7 +358,7 @@ int tgis_k_attention_window(int32_t head_dim, const void* qkv_dev, const void* k
                             int32_t bt_stride, void* out_dev, int32_t n_q, int32_t n_kv, float scale, int32_t mode,
                             int32_t window) {
   if (mode < 0 || mode > 2) return kfail("mode must be 0 (existing prefill kernel), 1 (split-context) or 2 (selection)");
-  if (head_dim != 64 && head_dim != HEAD_DIM) return kfail("head_dim must be 64 or 128");
+  if (head_dim != 64 && head_dim != 96 && head_dim != HEAD_DIM) return kfail("head_dim must be 64, 96 or 128");
   if (window < 0) return kfail("window must be >= 0 (0: none)");
   AttnCall call;
   call.head_dim = head_dim;
@@ -487,7 +487,7 @@ int tgis_k_attention_bench_window(int32_t head_dim, const void* qkv_dev, const v
                                   int32_t n_q, int32_t n_kv, float scale, int32_t n_layers, int64_t layer_stride_bytes,
                                   int32_t iters, float* us_out, int32_t window) {
   if (n_kv <= 0 || n_q % n_kv) return kfail("bad head counts");
-  if (head_dim != 64 && head_dim != HEAD_DIM) return kfail("head_dim must be 64 or 128");
+  if (head_dim != 64 && head_dim != 96 && head_dim != HEAD_DIM) return kfail("head_dim must be 64, 96 or 128");
   if (window < 0) return kfail("window must be >= 0 (0: none)");
   const int G = n_q / n_kv;
   const int qkv_ld = (n_q + 2 * n_kv) * head_dim, out_ld = n_q * head_dim;

@@ -32,7 +32,11 @@ class ModelConfig:
     the keys p - sliding_window < k <= p (tgis_engine_set_sliding_window; single GPU).
 
     Qwen2 / Qwen2.5 (Qwen2ForCausalLM) is arch "llama" with qkv_bias set: a bias on the q, k and v projections, added to
-    the fp32 accumulators before the one rounding to bf16 (tgis_engine_set_qkv_bias; head_dim 128 or 64, single GPU)."""
+    the fp32 accumulators before the one rounding to bf16 (tgis_engine_set_qkv_bias; head_dim 128 or 64, single GPU).
+
+    Phi-3 / Phi-3.5 / Phi-4 (Phi3ForCausalLM) is arch "llama", with head_dim 96 for Phi-3-mini / Phi-3.5-mini (single
+    GPU, no LoRA slots), LongRoPE for the 128k variants (rope_long_factor / rope_short_factor) and the model-wide
+    sliding_window of the 4k variants.  Its fused qkv_proj / gate_up_proj tensors are split on the host (loader.py)."""
 
     n_layers: int        # num_hidden_layers
     hidden: int          # hidden_size
@@ -57,10 +61,21 @@ class ModelConfig:
     qk_norm: bool = False               # Qwen3: per-head RMSNorm of q and k (self_attn.q_norm / k_norm)
     sliding_window: int | None = None   # Mistral: keys per query, itself included, in every layer; None = all
     qkv_bias: bool = False              # Qwen2: self_attn.{q,k,v}_proj.bias
+    # LongRoPE (Phi-3 128k, rope_type "longrope"): per-frequency rescale factors [head_dim / 2], long and short, with
+    # rope_original_max_pos as original_max_position_embeddings; empty = no LongRoPE (rope.py)
+    rope_long_factor: tuple[float, ...] = ()
+    rope_short_factor: tuple[float, ...] = ()
+    rope_max_position_embeddings: int = 0   # LongRoPE: max_position_embeddings (the mscale's numerator)
+    fused_projections: bool = False     # Phi-3: checkpoints hold self_attn.qkv_proj and mlp.gate_up_proj (loader.py)
+
+    @property
+    def rope_longrope(self) -> bool:
+        return bool(self.rope_long_factor)
 
     @property
     def rope_scaled(self) -> bool:
-        return self.rope_scaling_factor not in (0.0, 1.0)
+        """the rotary table is not the engine's built-in unscaled one (llama3 scaling or LongRoPE)"""
+        return self.rope_scaling_factor not in (0.0, 1.0) or self.rope_longrope
 
     @property
     def is_granite(self) -> bool:
@@ -149,6 +164,21 @@ PRESETS: dict[str, ModelConfig] = {
                               rope_theta=1000000.0, rms_eps=1e-6, max_model_len=8192, qkv_bias=True),
     "qwen2.5-14b": ModelConfig(n_layers=48, hidden=5120, n_q_heads=40, n_kv_heads=8, ffn=13824, vocab=152064,
                                rope_theta=1000000.0, rms_eps=1e-5, max_model_len=8192, qkv_bias=True),
+    # Phi-3: a CPU-oracle-sized stack with 96-dim heads, GQA group 1 and an odd vocabulary, and the
+    # Phi-3-mini-4k, Phi-3-medium-4k and Phi-4 shapes.  Those three are the published microsoft/Phi-3-mini-4k-instruct,
+    # Phi-3-medium-4k-instruct and phi-4 config.json values as recalled, not checked against the files when these
+    # presets were written.  The 4k checkpoints' config.json sets sliding_window 2047, which the loader maps; the presets
+    # leave it out (only the Mistral presets carry a window), which changes nothing below 2047 tokens.  Phi-4's
+    # sliding_window is uncertain (recalled as null, i.e. none).
+    "phi3-tiny": ModelConfig(n_layers=2, hidden=384, n_q_heads=4, n_kv_heads=4, ffn=512, vocab=1021, head_dim=96,
+                             rope_theta=10000.0, rms_eps=1e-5, max_model_len=2048, fused_projections=True),
+    "phi3-mini-4k": ModelConfig(n_layers=32, hidden=3072, n_q_heads=32, n_kv_heads=32, ffn=8192, vocab=32064,
+                                head_dim=96, rope_theta=10000.0, rms_eps=1e-5, max_model_len=4096,
+                                fused_projections=True),
+    "phi3-medium-4k": ModelConfig(n_layers=40, hidden=5120, n_q_heads=40, n_kv_heads=10, ffn=17920, vocab=32064,
+                                  rope_theta=10000.0, rms_eps=1e-5, max_model_len=4096, fused_projections=True),
+    "phi-4": ModelConfig(n_layers=40, hidden=5120, n_q_heads=40, n_kv_heads=10, ffn=17920, vocab=100352,
+                         rope_theta=250000.0, rms_eps=1e-5, max_model_len=16384, fused_projections=True),
 }
 
 
@@ -244,6 +274,9 @@ class NativeEngine:
         if model.sliding_window and tp_size > 1:
             raise EngineError("sliding-window attention (Mistral) is not supported with tensor parallelism: it is "
                               "implemented on a single GPU only (use tensor_parallel_size 1)")
+        if model.fused_projections and tp_size > 1:
+            raise EngineError("Phi-3 is not supported with tensor parallelism: it is implemented on a single GPU only "
+                              "(use tensor_parallel_size 1)")
         if model.qkv_bias and tp_size > 1:
             raise EngineError("Qwen2 (qkv_bias) is not supported with tensor parallelism: the qkv bias is implemented on a "
                               "single GPU only (use tensor_parallel_size 1)")

@@ -30,6 +30,8 @@ def model_config_from_hf(path: Path, max_model_len: int | None) -> ModelConfig:
         return _qwen3_model_config(cfg, max_model_len)
     if cfg.get("model_type") == "mistral" or "MistralForCausalLM" in archs:
         return _mistral_model_config(cfg, max_model_len)
+    if cfg.get("model_type") == "phi3" or "Phi3ForCausalLM" in archs:
+        return _phi3_model_config(cfg, max_model_len)
     if cfg.get("model_type") == "qwen2" or "Qwen2ForCausalLM" in archs:
         if cfg.get("attention_bias") is False:
             # Qwen2's q / k / v projections always carry a bias (transformers and vLLM hard-code bias=True; Qwen2Config
@@ -214,6 +216,81 @@ def _qwen2_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
                        tie_word_embeddings=bool(cfg.get("tie_word_embeddings", False)), qkv_bias=True, **scaling)
 
 
+def _phi3_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
+    """microsoft Phi-3 / Phi-3.5 / Phi-4 Phi3ForCausalLM config.json -> the Llama stack (vLLM's Phi3ForCausalLM is a plain
+    subclass of LlamaForCausalLM), with head_dim 96, 128 or 64, rope_type "longrope" (legacy spellings "su" and "yarn",
+    as transformers' Phi3Config normalises them) and a model-wide sliding window (null: none).  The checkpoint's fused
+    qkv_proj / gate_up_proj tensors are split at load (split_fused).  Variants the engine would serve wrongly are refused,
+    each with its reason."""
+    hidden, heads = cfg["hidden_size"], cfg["num_attention_heads"]
+    head_dim = cfg.get("head_dim") or hidden // heads
+    window = cfg.get("sliding_window")
+    rope = cfg.get("rope_scaling") or cfg.get("rope_parameters") or {}   # transformers' Phi3Config: rope_scaling first
+    kind = rope.get("rope_type") or rope.get("type") or "default"
+    problems = []
+    partial = rope.get("partial_rotary_factor", cfg.get("partial_rotary_factor", 1.0))
+    if partial != 1.0:
+        problems.append(f"partial_rotary_factor {partial} (only full-width rotary embeddings are implemented)")
+    for key in ("short_mscale", "long_mscale", "attention_factor"):
+        if rope.get(key) is not None:
+            problems.append(f"rope {key} {rope[key]} (only the default LongRoPE scale sqrt(1 + ln s / ln original) is "
+                            "implemented)")
+    kinds = sorted(set(cfg.get("layer_types") or []))
+    if len(kinds) > 1:
+        problems.append(f"layer_types mixing {kinds} (per-layer windows are not implemented: one window serves every "
+                        "layer)")
+    if window is not None and (not isinstance(window, int) or isinstance(window, bool) or window < 0):
+        problems.append(f"sliding_window {window!r} (a non-negative integer or null)")
+    if head_dim not in (64, 96, 128):
+        problems.append(f"head_dim {head_dim} (the attention kernels exist for 64, 96 and 128)")
+    if kind not in ("default", "longrope", "su", "yarn"):
+        problems.append(f"rope scaling type {kind!r} (only 'default' and 'longrope' are implemented)")
+    if problems:
+        raise ValueError("unsupported Phi-3 variant: " + "; ".join(problems))
+    theta = float(rope.get("rope_theta") or cfg.get("rope_theta") or 10000.0)
+    derived = cfg.get("max_position_embeddings", 4096)
+    if max_model_len is not None and max_model_len > derived:
+        raise ValueError(f"max_model_len {max_model_len} exceeds the model's max_position_embeddings {derived}")
+    scaling = {}
+    if kind != "default":
+        orig = rope.get("original_max_position_embeddings") or cfg.get("original_max_position_embeddings")
+        long_f, short_f = rope.get("long_factor"), rope.get("short_factor")
+        if not orig or not long_f or not short_f:
+            raise ValueError("rope scaling type 'longrope' needs long_factor, short_factor and "
+                             "original_max_position_embeddings")
+        if len(long_f) != head_dim // 2 or len(short_f) != head_dim // 2:
+            raise ValueError(f"longrope long_factor / short_factor must have head_dim / 2 = {head_dim // 2} entries, got "
+                             f"{len(long_f)} / {len(short_f)}")
+        scaling = dict(rope_long_factor=tuple(float(x) for x in long_f),
+                       rope_short_factor=tuple(float(x) for x in short_f), rope_original_max_pos=int(orig),
+                       rope_max_position_embeddings=int(derived))
+    return ModelConfig(n_layers=cfg["num_hidden_layers"], hidden=hidden, n_q_heads=heads,
+                       n_kv_heads=cfg.get("num_key_value_heads") or heads, ffn=cfg["intermediate_size"],
+                       vocab=cfg["vocab_size"], head_dim=head_dim, rope_theta=theta,
+                       rms_eps=float(cfg.get("rms_norm_eps", 1e-5)), max_model_len=max_model_len or min(derived, 8192),
+                       tie_word_embeddings=bool(cfg.get("tie_word_embeddings", False)), sliding_window=window or None,
+                       fused_projections=True, **scaling)
+
+
+def split_fused(name: str, t, mc: ModelConfig) -> list:
+    """[(name, tensor)] to load for one checkpoint tensor: Phi-3's self_attn.qkv_proj.weight as its q | k | v rows and
+    mlp.gate_up_proj.weight as gate (rows [0, ffn)) | up (rows [ffn, 2 ffn)) under the separate projections' names
+    (HF Phi3MLP's chunk order, vLLM's merged column order); every other tensor as it is"""
+    if name.endswith("self_attn.qkv_proj.weight"):
+        base = name[: -len("qkv_proj.weight")]
+        q, kv = mc.n_q_heads * mc.head_dim, mc.n_kv_heads * mc.head_dim
+        if t.shape[0] != q + 2 * kv:
+            raise ValueError(f"{name}: {t.shape[0]} rows, expected (n_q + 2 n_kv) * head_dim = {q + 2 * kv}")
+        return [(base + "q_proj.weight", t[:q]), (base + "k_proj.weight", t[q:q + kv]),
+                (base + "v_proj.weight", t[q + kv:])]
+    if name.endswith("mlp.gate_up_proj.weight"):
+        base = name[: -len("gate_up_proj.weight")]
+        if t.shape[0] != 2 * mc.ffn:
+            raise ValueError(f"{name}: {t.shape[0]} rows, expected 2 * intermediate_size = {2 * mc.ffn}")
+        return [(base + "gate_proj.weight", t[:mc.ffn]), (base + "up_proj.weight", t[mc.ffn:])]
+    return [(name, t)]
+
+
 def _opt_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
     """facebook/opt-* config.json -> ModelConfig(arch="opt").  The variants vLLM's OPT model handles with extra modules
     (opt-350m: post-LayerNorm + project_in/out) are refused rather than silently mis-served."""
@@ -284,12 +361,18 @@ def load_synthetic_weights(eng: NativeEngine, mc: ModelConfig, seed: int, device
     eng.load_weight("model.norm.weight", ones)
     for i in range(mc.n_layers):
         p = f"model.layers.{i}."
-        eng.load_weight(p + "self_attn.q_proj.weight", rnd(q_dim, mc.hidden))
-        eng.load_weight(p + "self_attn.k_proj.weight", rnd(kv_dim, mc.hidden))
-        eng.load_weight(p + "self_attn.v_proj.weight", rnd(kv_dim, mc.hidden))
+        if mc.fused_projections:   # Phi-3: the checkpoint's fused tensors, through the loader's split
+            for n, t in split_fused(p + "self_attn.qkv_proj.weight", rnd(q_dim + 2 * kv_dim, mc.hidden), mc):
+                eng.load_weight(n, t)
+            for n, t in split_fused(p + "mlp.gate_up_proj.weight", rnd(2 * mc.ffn, mc.hidden), mc):
+                eng.load_weight(n, t)
+        else:
+            eng.load_weight(p + "self_attn.q_proj.weight", rnd(q_dim, mc.hidden))
+            eng.load_weight(p + "self_attn.k_proj.weight", rnd(kv_dim, mc.hidden))
+            eng.load_weight(p + "self_attn.v_proj.weight", rnd(kv_dim, mc.hidden))
+            eng.load_weight(p + "mlp.gate_proj.weight", rnd(mc.ffn, mc.hidden))
+            eng.load_weight(p + "mlp.up_proj.weight", rnd(mc.ffn, mc.hidden))
         eng.load_weight(p + "self_attn.o_proj.weight", rnd(mc.hidden, q_dim))
-        eng.load_weight(p + "mlp.gate_proj.weight", rnd(mc.ffn, mc.hidden))
-        eng.load_weight(p + "mlp.up_proj.weight", rnd(mc.ffn, mc.hidden))
         eng.load_weight(p + "mlp.down_proj.weight", rnd(mc.hidden, mc.ffn))
         eng.load_weight(p + "input_layernorm.weight", ones)
         eng.load_weight(p + "post_attention_layernorm.weight", ones)
@@ -321,7 +404,8 @@ def load_safetensors_dir(eng: NativeEngine, path: Path) -> None:
             for name in sf.keys():  # noqa: SIM118
                 if name.endswith("rotary_emb.inv_freq"):
                     continue
-                eng.load_weight(name, sf.get_tensor(name))
+                for n, t in split_fused(name, sf.get_tensor(name), eng.model):
+                    eng.load_weight(n, t)
 
 
 def _resolve_model(args):
@@ -380,6 +464,8 @@ def build_engine(args) -> AsyncTGISEngine:
         raise ValueError(f"Qwen3 (per-head q/k norm) is supported on a single GPU only: tensor_parallel_size {tp}")
     if tp > 1 and mc.sliding_window:
         raise ValueError(f"Mistral (sliding-window attention) is supported on a single GPU only: tensor_parallel_size {tp}")
+    if tp > 1 and mc.fused_projections:
+        raise ValueError(f"Phi-3 is supported on a single GPU only: tensor_parallel_size {tp}")
     if tp > 1 and mc.qkv_bias:
         raise ValueError(f"Qwen2 (qkv bias) is supported on a single GPU only: tensor_parallel_size {tp}")
     if tp > 1:
