@@ -58,6 +58,11 @@ typedef struct tgis_engine tgis_engine;
  *          leaves every dot product unchanged.  Single GPU, no LoRA slots. */
 #define TGIS_ARCH_LLAMA 0
 #define TGIS_ARCH_OPT 1
+/* GPT_BIGCODE: GPTBigCodeForCausalLM (StarCoder, SantaCoder, Granite-20B/34B-Code): OPT's layer stack with learned positions
+ *   from 0 (no offset), GELU-tanh (gelu_pytorch_tanh) between c_fc and c_proj, and one kv head shared by every query head
+ *   (multi_query: n_kv_heads = 1, groups up to 64) or multi-head attention (n_kv_heads = n_q_heads).  head_dim 128,
+ *   hidden = n_q_heads * 128, single GPU, no LoRA slots.  lm_head.weight is optional (tied to transformer.wte). */
+#define TGIS_ARCH_GPT_BIGCODE 2
 
 /* Model + runtime configuration (bf16 decoder-only transformer; see TGIS_ARCH_*). */
 typedef struct tgis_config {
@@ -95,7 +100,7 @@ typedef struct tgis_config {
    * projections of every layer.  Single GPU only (tp_size == 1). */
   int32_t max_loras;
   int32_t max_lora_rank;
-  int32_t arch;               /* TGIS_ARCH_LLAMA / TGIS_ARCH_OPT */
+  int32_t arch;               /* TGIS_ARCH_LLAMA / TGIS_ARCH_OPT / TGIS_ARCH_GPT_BIGCODE */
   int32_t reserved0;
 } tgis_config;
 
@@ -201,7 +206,9 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out);
 /* name: HF Llama parameter name ("model.layers.3.self_attn.q_proj.weight", "lm_head.weight", ...) or
  * "tgis.rope_cos_sin" ([max_model_len,128] bf16 = cos|sin); arch OPT: HF OPT parameter names
  * ("model.decoder.layers.3.self_attn.q_proj.bias", "model.decoder.embed_positions.weight" with >= max_model_len + 2 rows,
- * ...; a 1-D tensor is passed as rows = n, cols = 1).  ptr may be host or device memory (cudaMemcpyDefault);
+ * ...; a 1-D tensor is passed as rows = n, cols = 1); arch GPT_BIGCODE: HF GPTBigCode names ("transformer.wte.weight",
+ * "transformer.wpe.weight" with >= max_model_len rows, "transformer.h.3.attn.c_attn.weight" = q | k | v rows, ...).
+ * ptr may be host or device memory (cudaMemcpyDefault);
  * dtype 0 = bf16.  rows/cols describe the full (unsharded) tensor. */
 int tgis_engine_load_weight(tgis_engine* e, const char* name, const void* ptr, int64_t rows, int64_t cols, int32_t dtype);
 /* Granite (GraniteForCausalLM: the Llama layer stack plus four scalars of its config.json; vllm

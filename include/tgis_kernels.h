@@ -40,11 +40,13 @@ int tgis_k_silu_mul(const void* gate_up_dev, void* act_dev, int32_t T, int32_t f
 /* OPT (csrc/opt.cu; vllm model_executor/models/opt.py:61-70,148-197 = torch.nn.LayerNorm / F.linear(x, W, b) / ReLU):
  * tgis_k_opt_layernorm: acc_dev != NULL: residual = bf16(residual + bf16(acc + acc_bias)) first (acc fp32 [T, hidden], the
  *   row-"producer" GEMM's accumulators); out = bf16((residual - mean) * rstd * w + b).  residual is bf16 [T, hidden].
- * tgis_k_opt_bias_act: out[T, N] = bf16(act(acc[T, N] + bias[N])), act = ReLU (relu != 0) or identity.
+ * tgis_k_opt_bias_act: out[T, N] = bf16(act(acc[T, N] + bias[N])), act = identity (0), ReLU (1) or GELU-tanh (2:
+ *   GPTBigCode's gelu_pytorch_tanh, out = bf16(gelu_tanh(bf16(acc + bias))) with torch's CUDA formula in fp32); any other
+ *   act fails.
  * tgis_k_opt_embed: out[t] = bf16(tok_table[tok[t]] + pos_table[pos[t] + offset]); tok / pos are int32 DEVICE arrays. */
 int tgis_k_opt_layernorm(const void* acc_dev, const void* acc_bias_dev, void* residual_dev, const void* w_dev,
                          const void* b_dev, void* out_dev, int32_t T, int32_t hidden, float eps);
-int tgis_k_opt_bias_act(const void* acc_dev, const void* bias_dev, void* out_dev, int32_t T, int32_t N, int32_t relu);
+int tgis_k_opt_bias_act(const void* acc_dev, const void* bias_dev, void* out_dev, int32_t T, int32_t N, int32_t act);
 int tgis_k_opt_embed(const void* tok_dev, const void* pos_dev, const void* tok_table_dev, const void* pos_table_dev,
                      void* out_dev, int32_t T, int32_t hidden, int32_t vocab, int32_t n_pos_rows, int32_t offset);
 int tgis_k_rope_kv(void* qkv_dev, const int32_t* positions_host, const int32_t* slot_mapping_host,

@@ -15,7 +15,8 @@
 //
 // decode  (q_len = 1): grid (seq x split, kv_head); split-KV in fixed 128-token chunks (batch-invariant numerics);
 //                      one warp per 32-token block; the G = n_q/n_kv query heads of the group share every K/V byte;
-//                      last-arriving split combines partials in split order (deterministic).
+//                      last-arriving split combines partials in split order (deterministic).  G = 9..64 (D = 128):
+//                      head octets of <= 8 query heads, each its own work unit.
 // prefill (q_len >= 1): grid (16-query tile, kv_head); one warp per query head of the group; mma.sync m16n8k16 with
 //                      online softmax; KV blocks double-buffered through smem by TMA bulk copies.
 //                      Split-context variant (prefix-cache hits: a short suffix over a long cached context): a cluster of
@@ -116,9 +117,17 @@ __global__ void __launch_bounds__(DEC_THREADS, TGIS_DEC_MINB)
 attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv_bfloat16* __restrict__ k_cache,
                    const __nv_bfloat16* __restrict__ v_cache, const DecItem* __restrict__ items,
                    int max_splits, float* __restrict__ part_o, float* __restrict__ part_ml,
-                   __nv_bfloat16* __restrict__ out, int out_ld, int n_kv, float scale, int prefetch_old) {
+                   __nv_bfloat16* __restrict__ out, int out_ld, int n_kv, float scale, int prefetch_old,
+                   int group) {
   static_assert(G <= 8, "query heads of a group are rows 0..7 of the MMA tile");
   constexpr int DEC_RING = tgis::DEC_RING<D>, DEC_WARP_SMEM = tgis::DEC_WARP_SMEM<D>;
+  // G = 0: a group of `group` = 9..64 query heads, cut into head octets of at most 8 (the last one may be partial: its
+  // missing heads are zero columns).  A work unit is (kv head, octet), octets of one kv head adjacent; the octets of a
+  // (sequence, split) each stream its K / V tiles, the later ones from L2.  G = 1..8: one octet, unit = kv head.
+  constexpr bool OCT = G == 0;
+  const int grp = OCT ? group : G;                  // query heads per kv head
+  const int n_oct = OCT ? (group + 7) >> 3 : 1;     // octets per kv head
+  const int n_u = n_kv * n_oct;                     // work units per (sequence, split)
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint8_t* ring = smem + warp * DEC_WARP_SMEM;
@@ -135,7 +144,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
   griddep_launch();
   // ---- item list: host-written for this step, not produced by a preceding kernel -> readable before griddep_wait
   const int4* it4 = reinterpret_cast<const int4*>(items);  // record e = it4[2e] (q_row, kv_len, seq_split, -), it4[2e+1] (blocks)
-  const int n_flat = it4[0].x * n_kv;
+  const int n_flat = it4[0].x * n_u;
   const int n_slots = gridDim.x * DEC_WARPS;
   const int gw = warp * gridDim.x + blockIdx.x;  // consecutive items land on different SMs
   // The host lists the items longest first; round k hands item k*n_slots + (k even ? gw : n_slots-1-gw) to warp gw
@@ -143,8 +152,8 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
   auto item_of_round = [&](int k) { return k * n_slots + ((k & 1) ? n_slots - 1 - gw : gw); };
   int f = gw;
   if (f >= n_flat) return;
-  auto item_at = [&](int ff) { return __ldg(&it4[2 * (1 + ff / n_kv)]); };
-  auto blocks_at = [&](int ff) { return __ldg(&it4[2 * (1 + ff / n_kv) + 1]); };
+  auto item_at = [&](int ff) { return __ldg(&it4[2 * (1 + ff / n_u)]); };
+  auto blocks_at = [&](int ff) { return __ldg(&it4[2 * (1 + ff / n_u) + 1]); };
   auto n_blk_of = [&](const int4& it) {
     const int n_tok = min(DEC_TOK, it.y - (it.z >> 16) * DEC_TOK);
     return (n_tok + KV_BLOCK - 1) / KV_BLOCK;
@@ -157,7 +166,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
   int4 c_it = item_at(f);
   int4 c_nxt = c_it;
   // ---- issue cursor: runs DEC_RING tiles ahead of consumption, across item boundaries
-  int i_f = f, i_kvh = f % n_kv, i_jb = blk0_of(c_it), i_nblk = n_blk_of(c_it), i_kv = 0, i_buf = 0;
+  int i_f = f, i_kvh = f % n_u / n_oct, i_jb = blk0_of(c_it), i_nblk = n_blk_of(c_it), i_kv = 0, i_buf = 0;
   int4 i_nxt = c_it, i_blks = blocks_at(f), i_blks_nxt = i_blks;  // block ids of the item being issued / the next one
   int4 i_cur = c_it;                                                // record of the item being issued
   int i_k = 0, c_k = 0;  // round of the issue cursor / of the consumer
@@ -182,7 +191,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
     if (++i_jb == i_nblk) {  // next item of this warp; its record was requested one item ago
       i_f = item_of_round(++i_k);
       if (i_f >= n_flat) return;
-      i_kvh = i_f % n_kv;
+      i_kvh = i_f % n_u / n_oct;
       i_jb = blk0_of(i_nxt);
       i_nblk = n_blk_of(i_nxt);
       i_cur = i_nxt;
@@ -193,10 +202,12 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
       }
     }
   };
-  auto issue_q = [&](const int4& it, int kvh) {
+  auto issue_q = [&](const int4& it, int u) {
     if (lane == 0) {
-      mbar_arrive_expect_tx(q_bar, G * D * 2);
-      bulk_load_1d(q_s, qkv + (size_t)it.x * qkv_ld + (size_t)kvh * G * D, G * D * 2, q_bar);
+      const int kvh = u / n_oct, h0 = (u - kvh * n_oct) * 8;  // the unit's kv head and first head in the group
+      const int nh = OCT ? min(8, grp - h0) : G;
+      mbar_arrive_expect_tx(q_bar, nh * D * 2);
+      bulk_load_1d(q_s, qkv + (size_t)it.x * qkv_ld + (size_t)kvh * grp * D + (size_t)h0 * D, nh * D * 2, q_bar);
     }
   };
 
@@ -214,7 +225,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
   }
   griddep_wait();  // q and the newest cache slot come from the preceding kernels
   STL_WAITED();
-  issue_q(c_it, f % n_kv);
+  issue_q(c_it, f % n_u);
   for (int i = n_pre; i < DEC_RING; ++i) issue_tile();
 
   const int hr = lane >> 2, t4 = lane & 3;
@@ -224,7 +235,9 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
   int c_buf = 0, c_ph = 0, q_ph = 0;
 
   for (; f < n_flat; f = item_of_round(++c_k)) {
-    const int kvh = f % n_kv;
+    const int u = f % n_u, kvh = u / n_oct;
+    const int h0 = (u - kvh * n_oct) * 8;        // first head of the octet in the group (0 without octets)
+    const int nh = OCT ? min(8, grp - h0) : G;   // heads of the octet
     const int seq = c_it.z & 0xffff, split = c_it.z >> 16;
     const int kv_len = c_it.y;
     const int n_splits = (kv_len + DEC_TOK - 1) / DEC_TOK;
@@ -235,15 +248,15 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
     const int f_next = item_of_round(c_k + 1);
     const bool has_next = f_next < n_flat;
     if (has_next) c_nxt = item_at(f_next);
-    // ---- Q^T as B fragments: n = head (lane/4), 8 k-steps of 16 dims; heads >= G are zero columns
+    // ---- Q^T as B fragments: n = head (lane/4), 8 k-steps of 16 dims; heads >= nh are zero columns
     mbar_wait(q_bar, q_ph);
     q_ph ^= 1;
     uint32_t qb[D / 16][2];
 #pragma unroll
     for (int ks = 0; ks < D / 16; ++ks) {
       const uint8_t* qp = q_s + (hr * D + ks * 16 + t4 * 2) * 2;
-      qb[ks][0] = hr < G ? *reinterpret_cast<const uint32_t*>(qp) : 0u;
-      qb[ks][1] = hr < G ? *reinterpret_cast<const uint32_t*>(qp + 16) : 0u;
+      qb[ks][0] = hr < nh ? *reinterpret_cast<const uint32_t*>(qp) : 0u;
+      qb[ks][1] = hr < nh ? *reinterpret_cast<const uint32_t*>(qp + 16) : 0u;
     }
     // this thread's accumulators: heads 2*t4 + {0,1} (e & 1), dims md*16 + hr + {0,8} (e >> 1)
     float ot[D / 16][4];
@@ -273,7 +286,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
       if (++c_buf == DEC_RING) { c_buf = 0; c_ph ^= 1; }
       if (jb == jb0) {  // q_s was copied to registers above; by now the next item's record has arrived
         __syncwarp();
-        if (has_next) issue_q(c_nxt, f_next % n_kv);
+        if (has_next) issue_q(c_nxt, f_next % n_u);
       }
       // ---- online softmax; st[mt][e]: token mt*16 + hr + (e>>1)*8, head 2*t4 + (e&1)
       // tokens [first, valid) of the block are visible: first > 0 only in the block holding lo
@@ -357,11 +370,11 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
 
     // ---- item epilogue: with one visible split the kernel writes the row itself
     if (n_splits - c_it.w / DEC_TOK == 1) {
-      __nv_bfloat16* o_dst = out + (size_t)c_it.x * out_ld + (size_t)(kvh * G + 2 * t4) * D + hr;
+      __nv_bfloat16* o_dst = out + (size_t)c_it.x * out_ld + (size_t)(kvh * grp + h0 + 2 * t4) * D + hr;
       const float inv[2] = {1.f / l_r[0], 1.f / l_r[1]};
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        if (2 * t4 + (e & 1) < G) {
+        if (2 * t4 + (e & 1) < nh) {
 #pragma unroll
           for (int md = 0; md < D / 16; ++md)
             o_dst[(e & 1) * D + md * 16 + (e >> 1) * 8] = __float2bfloat16_rn(ot[md][e] * inv[e & 1]);
@@ -370,10 +383,10 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
     } else {
       // store the partial (m in the exp2 domain); attn_merge_kernel combines the splits in split order
       const size_t pbase = (size_t)(seq * n_kv + kvh) * max_splits;
-      float* po = part_o + ((pbase + split) * G + 2 * t4) * D + hr;
+      float* po = part_o + ((pbase + split) * grp + h0 + 2 * t4) * D + hr;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        if (2 * t4 + (e & 1) < G) {
+        if (2 * t4 + (e & 1) < nh) {
 #pragma unroll
           for (int md = 0; md < D / 16; ++md) po[(e & 1) * D + md * 16 + (e >> 1) * 8] = ot[md][e];
         }
@@ -381,8 +394,9 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
       if (hr == 0) {
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh)
-          if (2 * t4 + hh < G)
-            *reinterpret_cast<float2*>(part_ml + ((pbase + split) * G + 2 * t4 + hh) * 2) = make_float2(m_r[hh], l_r[hh]);
+          if (2 * t4 + hh < nh)
+            *reinterpret_cast<float2*>(part_ml + ((pbase + split) * grp + h0 + 2 * t4 + hh) * 2) =
+                make_float2(m_r[hh], l_r[hh]);
       }
     }
     c_it = c_nxt;
@@ -393,15 +407,20 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv
 // Split merge: one CTA per (decode sequence, kv head) with more than one visible split, thread = dim.  Reads the
 // partials of the visible splits (from the one holding lo = max(0, kv_len - window); window 0: all) in split order
 // (deterministic), writes the normalised bf16 rows.  The partials stay indexed by absolute split.
+// G = 0 (a group of `group` = 9..64 heads): one CTA per (decode sequence, kv head, head octet), as in the streaming kernel.
 template <int D, int G>
 __global__ void __launch_bounds__(D)
 attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ seq_ids, int max_splits,
                   const float* __restrict__ part_o, const float* __restrict__ part_ml,
-                  __nv_bfloat16* __restrict__ out, int out_ld, int n_kv, int window) {
-  __shared__ float ml_s[64 * G * 2];
+                  __nv_bfloat16* __restrict__ out, int out_ld, int n_kv, int window, int group) {
+  constexpr bool OCT = G == 0;
+  constexpr int GO = OCT ? 8 : G;  // heads of this CTA (an octet's missing heads are computed on zeros, not written)
+  __shared__ float ml_s[64 * GO * 2];
   STL_ENTER(4);
   griddep_launch();
-  const int sidx = blockIdx.x, kvh = blockIdx.y, d = threadIdx.x;
+  const int grp = OCT ? group : G, n_oct = OCT ? (group + 7) >> 3 : 1;
+  const int sidx = blockIdx.x, kvh = blockIdx.y / n_oct, d = threadIdx.x;
+  const int h0 = (blockIdx.y - kvh * n_oct) * 8, nh = OCT ? min(8, grp - h0) : G;
   const AttnSeq sq = seqs[seq_ids ? seq_ids[sidx] : sidx];  // host-written
   const int n_splits = (sq.kv_len + DEC_TOK - 1) / DEC_TOK;
   const int s0 = window > 0 ? max(0, sq.kv_len - window) / DEC_TOK : 0;  // first visible split
@@ -409,18 +428,29 @@ attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ 
   griddep_wait();
   STL_WAITED();
   const size_t pbase = (size_t)(sidx * n_kv + kvh) * max_splits;
-  float m_f[G], l_f[G], o_f[G];
+  // (m, l) pairs of splits [c0, c0 + nc) -> ml_s [split][GO heads][2]
+  auto load_ml = [&](int c0, int nc) {
+    if constexpr (OCT) {
+      for (int i = d; i < nc * GO * 2; i += D) {
+        const int sp = i / (GO * 2), r = i % (GO * 2);
+        ml_s[i] = r < nh * 2 ? __ldcg(&part_ml[((pbase + c0 + sp) * grp + h0) * 2 + r]) : 0.f;
+      }
+    } else {
+      for (int i = d; i < nc * G * 2; i += D) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
+    }
+  };
+  float m_f[GO], l_f[GO], o_f[GO];
 #pragma unroll
-  for (int g = 0; g < G; ++g) m_f[g] = -INFINITY, l_f[g] = 0.f, o_f[g] = 0.f;
+  for (int g = 0; g < GO; ++g) m_f[g] = -INFINITY, l_f[g] = 0.f, o_f[g] = 0.f;
   // pass 1: row maxima (the (m, l) pairs go through shared memory in chunks of 64 splits)
   for (int c0 = s0; c0 < n_splits; c0 += 64) {
     const int nc = min(64, n_splits - c0);
     __syncthreads();
-    for (int i = d; i < nc * G * 2; i += D) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
+    load_ml(c0, nc);
     __syncthreads();
     for (int sp = 0; sp < nc; ++sp)
 #pragma unroll
-      for (int g = 0; g < G; ++g) m_f[g] = fmaxf(m_f[g], ml_s[(sp * G + g) * 2]);
+      for (int g = 0; g < GO; ++g) m_f[g] = fmaxf(m_f[g], ml_s[(sp * GO + g) * 2]);
   }
   // pass 2: weighted sums in split order, SPB splits of loads in flight per thread
   constexpr int SPB = 4;
@@ -428,32 +458,33 @@ attn_merge_kernel(const AttnSeq* __restrict__ seqs, const int32_t* __restrict__ 
     const int nc = min(64, n_splits - c0);
     if (n_splits - s0 > 64) {
       __syncthreads();
-      for (int i = d; i < nc * G * 2; i += D) ml_s[i] = __ldcg(&part_ml[(pbase + c0) * G * 2 + i]);
+      load_ml(c0, nc);
       __syncthreads();
     }
     for (int sp0 = 0; sp0 < nc; sp0 += SPB) {
-      float ov[SPB][G];
+      float ov[SPB][GO];
 #pragma unroll
       for (int j = 0; j < SPB; ++j)
 #pragma unroll
-        for (int g = 0; g < G; ++g)
-          ov[j][g] = (sp0 + j < nc) ? __ldcg(&part_o[((pbase + c0 + sp0 + j) * G + g) * D + d]) : 0.f;
+        for (int g = 0; g < GO; ++g)
+          ov[j][g] = (sp0 + j < nc && g < nh) ? __ldcg(&part_o[((pbase + c0 + sp0 + j) * grp + h0 + g) * D + d]) : 0.f;
 #pragma unroll
       for (int j = 0; j < SPB; ++j) {
         if (sp0 + j < nc) {
 #pragma unroll
-          for (int g = 0; g < G; ++g) {
-            const float fs = exp2f(ml_s[((sp0 + j) * G + g) * 2] - m_f[g]);
-            l_f[g] += ml_s[((sp0 + j) * G + g) * 2 + 1] * fs;
+          for (int g = 0; g < GO; ++g) {
+            const float fs = exp2f(ml_s[((sp0 + j) * GO + g) * 2] - m_f[g]);
+            l_f[g] += ml_s[((sp0 + j) * GO + g) * 2 + 1] * fs;
             o_f[g] += ov[j][g] * fs;
           }
         }
       }
     }
   }
-  __nv_bfloat16* o_dst = out + (size_t)sq.q_start * out_ld + (size_t)kvh * G * D;
+  __nv_bfloat16* o_dst = out + (size_t)sq.q_start * out_ld + (size_t)kvh * grp * D + (size_t)h0 * D;
 #pragma unroll
-  for (int g = 0; g < G; ++g) o_dst[g * D + d] = __float2bfloat16_rn(o_f[g] / l_f[g]);
+  for (int g = 0; g < GO; ++g)
+    if (g < nh) o_dst[g * D + d] = __float2bfloat16_rn(o_f[g] / l_f[g]);
   STL_EXIT();
 }
 
@@ -462,7 +493,7 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
                                    const __nv_bfloat16* v_cache, const DecItem* items, int max_entries,
                                    const AttnSeq* seqs, const int32_t* seq_ids, int n_seqs, int max_splits,
                                    float* part_o, float* part_ml, __nv_bfloat16* out, int out_ld, int n_kv,
-                                   float scale, int num_sms, cudaStream_t stream, int window) {
+                                   float scale, int num_sms, cudaStream_t stream, int window, int group) {
   static bool attr = false;
   if (!attr) {
     cudaError_t e =
@@ -470,15 +501,17 @@ static cudaError_t decode_launch_g(const __nv_bfloat16* qkv, int qkv_ld, const _
     if (e != cudaSuccess) return e;
     attr = true;
   }
-  const long long max_flat = (long long)max_entries * n_kv;
+  const int n_oct = G == 0 ? (group + 7) / 8 : 1;  // work units per kv head
+  const long long max_flat = (long long)max_entries * n_kv * n_oct;
   const int grid = (int)std::min<long long>((long long)TGIS_DEC_MINB * num_sms, (max_flat + DEC_WARPS - 1) / DEC_WARPS);
   const char* env_pre = getenv("TGIS_ATTN_PREFETCH");  // 0: no cache reads before the grid-dependency wait
   const int prefetch_old = (env_pre && env_pre[0] == '0') ? 0 : 1;
   cudaError_t e = launch_k(attn_decode_kernel<D, G>, dim3(grid), dim3(DEC_THREADS), DEC_SMEM<D>, stream, qkv, qkv_ld,
-                           k_cache, v_cache, items, max_splits, part_o, part_ml, out, out_ld, n_kv, scale, prefetch_old);
+                           k_cache, v_cache, items, max_splits, part_o, part_ml, out, out_ld, n_kv, scale, prefetch_old,
+                           group);
   if (e != cudaSuccess || max_splits <= 1) return e;
-  return launch_k(attn_merge_kernel<D, G>, dim3(n_seqs, n_kv), dim3(D), 0, stream, seqs, seq_ids, max_splits,
-                  (const float*)part_o, (const float*)part_ml, out, out_ld, n_kv, window);
+  return launch_k(attn_merge_kernel<D, G>, dim3(n_seqs, n_kv * n_oct), dim3(D), 0, stream, seqs, seq_ids, max_splits,
+                  (const float*)part_o, (const float*)part_ml, out, out_ld, n_kv, window, group);
 }
 
 cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
@@ -492,8 +525,12 @@ cudaError_t attn_decode_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_
 #define TGIS_DEC(DD, GG)                                                                                      \
   case GG:                                                                                                    \
     return decode_launch_g<DD, GG>(qkv, qkv_ld, k_cache, v_cache, items, max_entries, seqs, seq_ids, n_seqs, \
-                                   max_splits, part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream, window)
+                                   max_splits, part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream, window, GG)
   if (head_dim == 128) {
+    // groups of 9..64 (multi-query GPTBigCode: 16..48; StarCoder2: 12): head octets, one instantiation for all of them
+    if (G > 8 && G <= 64)
+      return decode_launch_g<128, 0>(qkv, qkv_ld, k_cache, v_cache, items, max_entries, seqs, seq_ids, n_seqs,
+                                     max_splits, part_o, part_ml, out, out_ld, n_kv, scale, num_sms, stream, window, G);
     switch (G) {
       TGIS_DEC(128, 1);
       TGIS_DEC(128, 2);
@@ -533,13 +570,16 @@ template <int D> constexpr int PF_SPLIT_SMEM_MAX = PF_QROWS * D * 4 * 8;  // G =
 
 // grid (n_tiles, n_kv) / SPLIT: (n_tiles * PF_CLUSTER, n_kv) in clusters of PF_CLUSTER; blockDim = 32 * G (warp = query
 // head inside the GQA group).
+// CHUNKS (groups of 9..64): the group is cut into n_ch = gridDim.y / n_kv chunks of blockDim / 32 <= 8 heads, grid y =
+// (kv head, chunk); each chunk streams the tile's K / V on its own.  Warps past the group's last head (G = 22: 3 chunks
+// of 8) run on its last head's queries and store nothing.
 // SPLIT (split-context prefill): the PF_CLUSTER CTAs of a cluster share one (tile, kv head); CTA rank r streams the r-th
 // contiguous near-equal share of the tile's causal block range with the same per-block arithmetic, leaves its (o, m, l)
 // partial in its own shared memory (the KV stages once they are drained; dynamic shared memory, G * 8 KiB when that is
 // more), and after a cluster barrier merges the partials of rows [r * 16 / PF_CLUSTER, ...) from every rank through
 // distributed shared memory, in rank order, in fp32.  No global workspace and no atomics: the same bits on every run,
 // and the split points depend only on the tile's own block range.
-template <int D, bool SPLIT>
+template <int D, bool SPLIT, bool CHUNKS>
 __global__ void __launch_bounds__(256)
 attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __nv_bfloat16* __restrict__ k_cache,
                     const __nv_bfloat16* __restrict__ v_cache, const AttnSeq* __restrict__ seqs,
@@ -553,7 +593,10 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   griddep_launch();
   griddep_wait();
   const int crank = SPLIT ? (int)cluster_ctarank() : 0;
-  const int tile = SPLIT ? blockIdx.x / PF_CLUSTER : blockIdx.x, kvh = blockIdx.y;
+  const int n_ch = CHUNKS ? gridDim.y / n_kv : 1;
+  const int tile = SPLIT ? blockIdx.x / PF_CLUSTER : blockIdx.x, kvh = CHUNKS ? blockIdx.y / n_ch : blockIdx.y;
+  // first head of this CTA's chunk inside the group (0 without chunks)
+  const int hq0 = CHUNKS ? (blockIdx.y - kvh * n_ch) * (blockDim.x >> 5) : 0;
   const AttnSeq sq = seqs[tile_seq[tile]];
   const int q0 = tile_q0[tile];                      // first query (index within this step's q_len)
   const int n_rows = min(PF_QROWS, sq.q_len - q0);   // valid query rows in the tile
@@ -568,7 +611,8 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
   const int jb1 = SPLIT ? blk_lo + (crank + 1) * (n_blk - blk_lo) / PF_CLUSTER : n_blk;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int head = kvh * G + warp;
+  const bool live = !CHUNKS || hq0 + warp < G;  // the warp's head exists (its results are stored)
+  const int head = CHUNKS ? kvh * G + min(hq0 + warp, G - 1) : kvh * G + warp;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars[0], 1);
@@ -765,9 +809,9 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
       }
     }
     cluster_sync_all();  // no CTA leaves while a peer may still read its shared memory
-    if (row < n_rows) {
+    if (row < n_rows && (!CHUNKS || hq0 + hd < G)) {
       const float inv = 1.f / l_f;
-      __nv_bfloat16* dst = out + (size_t)(sq.q_start + q0 + row) * out_ld + (size_t)(kvh * G + hd) * D + d0;
+      __nv_bfloat16* dst = out + (size_t)(sq.q_start + q0 + row) * out_ld + (size_t)(kvh * G + hq0 + hd) * D + d0;
       if constexpr (D == 128) {
         uint4 pk;
         pk.x = pack_bf16x2(acc[0] * inv, acc[1] * inv);
@@ -789,7 +833,7 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_ld, const __n
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int row = g + r * 8;
-    if (row < n_rows) {
+    if (row < n_rows && live) {
       const float inv = 1.f / l_r[r];
       __nv_bfloat16* dst = out + (size_t)(sq.q_start + q0 + row) * out_ld + (size_t)head * D;
 #pragma unroll
@@ -807,19 +851,26 @@ cudaError_t attn_prefill_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv
   if (n_tiles <= 0) return cudaSuccess;
   if (n_q % n_kv != 0 || window < 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
-  if (G > 8 || (head_dim != 128 && head_dim != 64 && head_dim != 96)) return cudaErrorInvalidValue;
+  if (G > 8) {  // head chunks of at most 8 warps, 128-dim heads only
+    if (head_dim != 128 || G > 64) return cudaErrorInvalidValue;
+    const int n_ch = (G + 7) / 8, hc = (G + n_ch - 1) / n_ch;
+    return launch_k(attn_prefill_kernel<128, false, true>, dim3(n_tiles, n_kv * n_ch), dim3(32 * hc), 0, stream, qkv,
+                    qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G,
+                    scale, window);
+  }
+  if (head_dim != 128 && head_dim != 64 && head_dim != 96) return cudaErrorInvalidValue;
   dim3 grid(n_tiles, n_kv);
   if (head_dim == 96)
-    return launch_k(attn_prefill_kernel<96, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
-                    tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
+    return launch_k(attn_prefill_kernel<96, false, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache,
+                    seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
   if (head_dim == 64)
-    return launch_k(attn_prefill_kernel<64, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
-                    tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
-  return launch_k(attn_prefill_kernel<128, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache, seqs,
-                  tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
+    return launch_k(attn_prefill_kernel<64, false, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache,
+                    seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
+  return launch_k(attn_prefill_kernel<128, false, false>, grid, dim3(32 * G), 0, stream, qkv, qkv_ld, k_cache, v_cache,
+                  seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv, G, scale, window);
 }
 
-template <int D>
+template <int D, bool CHUNKS>
 static cudaError_t prefill_split_launch_d(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
                                           const __nv_bfloat16* v_cache, const AttnSeq* seqs, const int32_t* tile_seq,
                                           const int32_t* tile_q0, int n_tiles, const int32_t* block_table,
@@ -832,16 +883,18 @@ static cudaError_t prefill_split_launch_d(const __nv_bfloat16* qkv, int qkv_ld, 
   if (e != cudaSuccess) return e;
   const uint64_t bit = dev < 64 ? 1ull << dev : 0ull;
   if (!(attr_set.load(std::memory_order_acquire) & bit)) {
-    e = cudaFuncSetAttribute(attn_prefill_kernel<D, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    e = cudaFuncSetAttribute(attn_prefill_kernel<D, true, CHUNKS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              PF_SPLIT_SMEM_MAX<D>);
     if (e != cudaSuccess) return e;
     attr_set.fetch_or(bit, std::memory_order_release);
   }
-  const int smem = std::max(2 * 2 * TILE_BYTES<D>, G * PF_QROWS * D * 4);
-  dim3 grid(n_tiles * PF_CLUSTER, n_kv);
-  return launch_k_cluster(attn_prefill_kernel<D, true>, grid, dim3(32 * G), (size_t)smem, stream, PF_CLUSTER, qkv,
-                          qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld, n_kv,
-                          G, scale, window);
+  // heads per CTA: the group, or (CHUNKS) its even share of ceil(G / 8) chunks
+  const int n_ch = (G + 7) / 8, hc = (G + n_ch - 1) / n_ch;
+  const int smem = std::max(2 * 2 * TILE_BYTES<D>, hc * PF_QROWS * D * 4);
+  dim3 grid(n_tiles * PF_CLUSTER, n_kv * n_ch);
+  return launch_k_cluster(attn_prefill_kernel<D, true, CHUNKS>, grid, dim3(32 * hc), (size_t)smem, stream, PF_CLUSTER,
+                          qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, block_table, bt_stride, out, out_ld,
+                          n_kv, G, scale, window);
 }
 
 cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, const __nv_bfloat16* k_cache,
@@ -852,15 +905,19 @@ cudaError_t attn_prefill_split_launch(const __nv_bfloat16* qkv, int qkv_ld, cons
   if (n_tiles <= 0) return cudaSuccess;
   if (n_q % n_kv != 0 || window < 0) return cudaErrorInvalidValue;
   const int G = n_q / n_kv;
-  if (G > 8) return cudaErrorInvalidValue;
+  if (G > 8) {
+    if (head_dim != 128 || G > 64) return cudaErrorInvalidValue;
+    return prefill_split_launch_d<128, true>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
+                                             bt_stride, out, out_ld, n_kv, G, scale, stream, window);
+  }
   if (head_dim == 128)
-    return prefill_split_launch_d<128>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
+    return prefill_split_launch_d<128, false>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
                                        bt_stride, out, out_ld, n_kv, G, scale, stream, window);
   if (head_dim == 64)
-    return prefill_split_launch_d<64>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
+    return prefill_split_launch_d<64, false>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
                                       bt_stride, out, out_ld, n_kv, G, scale, stream, window);
   if (head_dim == 96)
-    return prefill_split_launch_d<96>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
+    return prefill_split_launch_d<96, false>(qkv, qkv_ld, k_cache, v_cache, seqs, tile_seq, tile_q0, n_tiles, block_table,
                                       bt_stride, out, out_ld, n_kv, G, scale, stream, window);
   return cudaErrorInvalidValue;
 }

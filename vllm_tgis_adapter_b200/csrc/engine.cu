@@ -250,8 +250,10 @@ struct tgis_engine {
   DevBuf<bf16> qkv_bias_w;
   std::vector<uint8_t> qkv_bias_loaded;
   // OPT (opt.cu): learned positions [max_model_len + 2, hidden], final LayerNorm bias; model head dim (64 or 128: every
-  // head is zero-padded to the 128-dim attention tiles at load time); fp32 GEMM accumulators of the biased projections
-  bool opt = false;
+  // head is zero-padded to the 128-dim attention tiles at load time); fp32 GEMM accumulators of the biased projections.
+  // GPTBigCode runs the same layer stack (opt is set too): positions [max_model_len, hidden] without OPT's offset of 2,
+  // GELU-tanh instead of ReLU, 128-dim heads and one kv head (multi_query) or n_q.
+  bool opt = false, bigcode = false;
   bf16 *pos_embed = nullptr, *final_norm_b = nullptr;
   // model_head_dim: the checkpoint's head size (the softmax scale); kv_head_dim: the head size of the qkv rows, the rotary
   // table and the KV tiles, i.e. of the kernels that run.  They differ for OPT only (64-dim heads zero-padded to 128).
@@ -471,11 +473,12 @@ struct tgis_engine {
     Fl = c.ffn / tp;
     Vl = c.vocab / tp;
     Vpad = (c.vocab + 7) / 8 * 8;  // == vocab under tensor parallelism (tgis_engine_create)
-    opt = c.arch == TGIS_ARCH_OPT;
+    bigcode = c.arch == TGIS_ARCH_GPT_BIGCODE;
+    opt = c.arch == TGIS_ARCH_OPT || bigcode;
     model_head_dim = c.head_dim;
     kv_head_dim = opt ? HEAD_DIM : c.head_dim;
     attn_scale = 1.0f / std::sqrt((float)model_head_dim);  // zero-padded head dims add nothing to q . k
-    pos_rows = opt ? c.max_model_len + 2 : 0;
+    pos_rows = bigcode ? c.max_model_len : opt ? c.max_model_len + 2 : 0;
     q_dim = nq * kv_head_dim;
     qkv_dim = (nq + 2 * nkv) * kv_head_dim;
     bt_stride = (c.max_model_len + KV_BLOCK - 1) / KV_BLOCK;
@@ -956,7 +959,67 @@ struct tgis_engine {
     return fail("unknown layer weight " + full_name);
   }
 
+  // GPTBigCode checkpoints (HF names, "transformer." prefix).  Single GPU.  Every projection is an nn.Linear [out, in]
+  // of 128-dim heads.  c_attn's rows are q | k | v (wqkv's layout) with multi_query; multi-head checkpoints hold them
+  // head by head, [head][q | k | v] (transformers views the output as (heads, 3 * head_dim)), and are regrouped here.
+  // Every other tensor is one contiguous copy.
+  int load_weight_bigcode(const std::string& name, const void* ptr, int64_t rows, int64_t cols) {
+    const tgis_config& c = cfg;
+    const int64_t H = c.hidden, F = c.ffn, V = c.vocab;
+    bf16* dst = nullptr;
+    int64_t n = 0;       // elements
+    int64_t c_attn = 0;  // c_attn's row width (H: weight, 1: bias), 0 for every other tensor
+    std::string key;
+    if (name == "lm_head.weight") {
+      dst = lm_head, n = V * H;
+    } else if (name.rfind("transformer.", 0) == 0) {
+      key = name.substr(12);
+      if (key == "wte.weight") dst = embed, n = V * H;
+      // the checkpoint's table has n_positions rows: the engine keeps the max_model_len rows it can reach
+      else if (key == "wpe.weight") dst = pos_embed, n = (int64_t)pos_rows * H;
+      else if (key == "ln_f.weight") dst = final_norm, n = H;
+      else if (key == "ln_f.bias") dst = final_norm_b, n = H;
+      else if (key.rfind("h.", 0) == 0 && key.find('.', 2) != std::string::npos) {
+        const size_t dot = key.find('.', 2);
+        const int li = atoi(key.substr(2, dot - 2).c_str());
+        if (li < 0 || li >= c.n_layers) return fail("layer index out of range in " + name);
+        LayerW& l = layers[li];
+        const std::string sub = key.substr(dot + 1);
+        if (sub == "ln_1.weight") dst = l.ln1, n = H;
+        else if (sub == "ln_1.bias") dst = l.ln1_b, n = H;
+        else if (sub == "attn.c_attn.weight") dst = l.wqkv, n = (int64_t)qkv_dim * H, c_attn = H;
+        else if (sub == "attn.c_attn.bias") dst = l.b_qkv, n = qkv_dim, c_attn = 1;
+        else if (sub == "attn.c_proj.weight") dst = l.wo, n = H * q_dim;
+        else if (sub == "attn.c_proj.bias") dst = l.b_o, n = H;
+        else if (sub == "ln_2.weight") dst = l.ln2, n = H;
+        else if (sub == "ln_2.bias") dst = l.ln2_b, n = H;
+        else if (sub == "mlp.c_fc.weight") dst = l.wgu, n = F * H;
+        else if (sub == "mlp.c_fc.bias") dst = l.b_fc1, n = F;
+        else if (sub == "mlp.c_proj.weight") dst = l.wd, n = H * F;
+        else if (sub == "mlp.c_proj.bias") dst = l.b_fc2, n = H;
+      }
+    }
+    if (!dst) return fail("unknown weight " + name);
+    const bool ok = dst == pos_embed ? cols == H && rows >= pos_rows : rows * cols == n;
+    if (!ok) return fail("shape mismatch for " + name + ": got " + std::to_string(rows) + "x" + std::to_string(cols));
+    cudaError_t e = cudaSuccess;
+    if (c_attn && nkv > 1) {
+      // multi-head c_attn: per head 3 groups of 128 rows (q, k, v) -> the q, k and v blocks of wqkv
+      const size_t w = (size_t)c_attn * HEAD_DIM * sizeof(bf16);  // bytes of one head's rows of one projection
+      for (int j = 0; j < 3 && e == cudaSuccess; ++j)
+        e = cudaMemcpy2D(reinterpret_cast<uint8_t*>(dst) + j * nkv * w, w, static_cast<const uint8_t*>(ptr) + j * w, 3 * w, w,
+                         nkv, cudaMemcpyDefault);
+    } else {
+      e = cudaMemcpy(dst, ptr, (size_t)n * sizeof(bf16), cudaMemcpyDefault);
+    }
+    if (e != cudaSuccess) return fail(std::string("cudaMemcpy(weight) failed: ") + cudaGetErrorString(e));
+    if (dst == lm_head) lm_head_loaded = true;
+    else opt_loaded.insert(key);
+    return 0;
+  }
+
   int load_weight(const std::string& name, const void* ptr, int64_t rows, int64_t cols) {
+    if (bigcode) return load_weight_bigcode(name, ptr, rows, cols);
     if (opt) return load_weight_opt(name, ptr, rows, cols);
     const tgis_config& c = cfg;
     const int64_t H = c.hidden, F = c.ffn, V = c.vocab;
@@ -1104,7 +1167,12 @@ struct tgis_engine {
   }
 
   void finalize_weights() {
-    if (opt) {
+    if (bigcode) {
+      const size_t expected = 4 + (size_t)12 * cfg.n_layers;
+      if (opt_loaded.size() < expected)
+        throw CudaError("GPTBigCode checkpoint incomplete: " + std::to_string(opt_loaded.size()) + " of " +
+                        std::to_string(expected) + " tensors loaded (wte, wpe, ln_f.{weight,bias} and 12 per layer)");
+    } else if (opt) {
       // an OPT checkpoint with a tensor missing must not come up healthy on zeros (the reference's engine fails the load)
       const size_t expected = 4 + (size_t)16 * cfg.n_layers;
       if (opt_loaded.size() < expected)
@@ -1267,7 +1335,7 @@ struct tgis_engine {
         gemm(xm_xn, l.m_qkv, xn.p, l.wqkv, qb ? (void*)y32.p : (void*)qkv.p, T, qkv_dim, H, qb ? 1 : 0, 0,
              rope_fused ? &rp : nullptr);
         if (qb && lora) {
-          CK(opt_bias_act_launch(y32.p, qkv_dim, qb, qkv.p, qkv_dim, T, qkv_dim, /*relu=*/0, num_sms, stream));
+          CK(opt_bias_act_launch(y32.p, qkv_dim, qb, qkv.p, qkv_dim, T, qkv_dim, ACT_NONE, num_sms, stream));
           ++n_launches;
         }
         if (lora) {
@@ -1371,6 +1439,9 @@ struct tgis_engine {
   // attention kernels run unchanged on zero-padded 128-dim heads with the model's softmax scale.  Per layer:
   //   LN1 [+ previous fc2 bias/residual] -> qkv GEMM -> bias + KV scatter -> attention -> out_proj GEMM ->
   //   LN2 + out_proj bias/residual -> fc1 GEMM -> bias + ReLU -> fc2 GEMM;  final LayerNorm after the last layer.
+  // GPTBigCode (vllm model_executor/models/gpt_bigcode.py) is the same stack with positions from 0 (wpe has no offset),
+  // GELU-tanh after c_fc, and n_kv = 1 (multi_query) or n_q: the writer, the item list and the attention kernels take
+  // any n_q = G * n_kv, G up to 64.
   void opt_layers(int T, int n_dec, int n_tiles, int max_dec_kv, int S, int R) {
     const tgis_config& c = cfg;
     const int H = c.hidden, F = Fl, V = c.vocab;
@@ -1378,7 +1449,7 @@ struct tgis_engine {
     const int32_t* d_pos = ds<int32_t>(off_pos);
     const AttnSeq* d_seqs = ds<AttnSeq>(off_seqs);
     const int32_t* d_bt = ds<int32_t>(off_bt);
-    CK(opt_embed_launch(d_tok, d_pos, embed, pos_embed, resid.p, T, H, V, pos_rows, /*offset=*/2, stream));
+    CK(opt_embed_launch(d_tok, d_pos, embed, pos_embed, resid.p, T, H, V, pos_rows, /*offset=*/bigcode ? 0 : 2, stream));
     ++n_launches;
     for (int li = 0; li < c.n_layers; ++li) {
       LayerW& l = layers[li];
@@ -1402,7 +1473,7 @@ struct tgis_engine {
       gemm(xm_attn, l.m_o, attn_out.p, l.wo, y32.p, T, H, q_dim, /*out_f32=*/1);
       CK(opt_layernorm_launch(y32.p, l.b_o, resid.p, l.ln2, l.ln2_b, xn.p, T, H, c.rms_eps, stream));
       gemm(xm_xn, l.m_gu, xn.p, l.wgu, y32.p, T, F, H, /*out_f32=*/1);
-      CK(opt_bias_act_launch(y32.p, F, l.b_fc1, act.p, F, T, F, /*relu=*/1, num_sms, stream));
+      CK(opt_bias_act_launch(y32.p, F, l.b_fc1, act.p, F, T, F, bigcode ? ACT_GELU_TANH : ACT_RELU, num_sms, stream));
       gemm(xm_act, l.m_d, act.p, l.wd, y32.p, T, H, F, /*out_f32=*/1);
       n_launches += 2;
     }
@@ -2179,8 +2250,19 @@ int tgis_abi_version(void) { return TGIS_ABI_VERSION; }
 int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
   if (!cfg || !out) return fail("null argument");
   if (cfg->abi_version != TGIS_ABI_VERSION) return fail("ABI version mismatch");
-  if (cfg->arch != TGIS_ARCH_LLAMA && cfg->arch != TGIS_ARCH_OPT) return fail("unknown arch");
-  if (cfg->arch == TGIS_ARCH_OPT) {
+  if (cfg->arch != TGIS_ARCH_LLAMA && cfg->arch != TGIS_ARCH_OPT && cfg->arch != TGIS_ARCH_GPT_BIGCODE)
+    return fail("unknown arch");
+  const bool bigcode = cfg->arch == TGIS_ARCH_GPT_BIGCODE;
+  if (bigcode) {
+    if (cfg->head_dim != HEAD_DIM) return fail("GPTBigCode: head_dim must be 128");
+    if (cfg->hidden != cfg->n_q_heads * HEAD_DIM) return fail("GPTBigCode: hidden must be n_q_heads * 128");
+    if (cfg->n_kv_heads != 1 && cfg->n_kv_heads != cfg->n_q_heads)
+      return fail("GPTBigCode: n_kv_heads must be 1 (multi_query) or n_q_heads (multi-head attention)");
+    if (cfg->n_q_heads / cfg->n_kv_heads > 64)
+      return fail("GPTBigCode: at most 64 query heads per kv head (the attention kernels' largest group)");
+    if (cfg->tp_size > 1) return fail("GPTBigCode runs on a single GPU only (tp_size must be 1)");
+    if (cfg->max_loras > 0) return fail("GPTBigCode: LoRA adapter slots are not supported (max_loras must be 0)");
+  } else if (cfg->arch == TGIS_ARCH_OPT) {
     if (cfg->head_dim != 64 && cfg->head_dim != HEAD_DIM) return fail("OPT: head_dim must be 64 or 128");
     if (cfg->n_q_heads != cfg->n_kv_heads) return fail("OPT: n_kv_heads must equal n_q_heads (multi-head attention)");
     if (cfg->hidden != cfg->n_q_heads * cfg->head_dim) return fail("OPT: hidden must be n_q_heads * head_dim");
@@ -2201,7 +2283,9 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
   const int G = cfg->n_q_heads / cfg->n_kv_heads;
   // decode attention is instantiated for every group of 1..8 at 128-dim heads and for all but 3 at 64-dim heads (the
   // query heads of a group share one 8-wide MMA tile, hence the upper bound)
-  if (G < 1 || G > 8) return fail("GQA group size must be 1 to 8 (n_q_heads / n_kv_heads)");
+  // GPTBigCode: groups of 9..64 run on head octets (attention.cu); Llama and OPT keep 1..8 until each has its own parity
+  // test above 8
+  if (G < 1 || (G > 8 && !bigcode)) return fail("GQA group size must be 1 to 8 (n_q_heads / n_kv_heads)");
   if (cfg->arch == TGIS_ARCH_LLAMA && cfg->head_dim == 64 && G == 3)
     return fail("head_dim 64: GQA group size must be 1, 2, 4 or 8, or 5, 6 or 7 (group 3 is not instantiated for "
                 "64-dim heads)");

@@ -156,9 +156,11 @@ cudaError_t opt_embed_launch(const int32_t* token_ids, const int32_t* positions,
 cudaError_t opt_layernorm_launch(const float* acc, const __nv_bfloat16* acc_bias, __nv_bfloat16* residual,
                                  const __nv_bfloat16* w, const __nv_bfloat16* b, __nv_bfloat16* out, int T, int hidden,
                                  float eps, cudaStream_t stream);
-// out[t, n] = bf16(act(acc[t, n] + bias[n])), act = ReLU or identity
+// out[t, n] = bf16(act(acc[t, n] + bias[n])); act ACT_GELU_TANH (GPTBigCode's gelu_pytorch_tanh) rounds the biased
+// projection first: out = bf16(gelu_tanh(bf16(acc + bias))).  Another act is cudaErrorInvalidValue.
+constexpr int ACT_NONE = 0, ACT_RELU = 1, ACT_GELU_TANH = 2;
 cudaError_t opt_bias_act_launch(const float* acc, int ld_acc, const __nv_bfloat16* bias, __nv_bfloat16* out, int ld_out,
-                                int T, int N, int relu, int num_sms, cudaStream_t stream);
+                                int T, int N, int act, int num_sms, cudaStream_t stream);
 // qkv epilogue: q_out[t, head, :] = bf16(acc + bias) for the q heads; k / v heads go straight into the paged cache
 // (slot_mapping[t] < 0: not cached).  acc fp32 [T, (n_q + 2 n_kv) * 128], q_out bf16 with the same row stride.
 cudaError_t opt_qkv_bias_kvwrite_launch(const float* acc, const __nv_bfloat16* bias, __nv_bfloat16* q_out,

@@ -146,8 +146,10 @@ opt_layernorm_kernel(const float* __restrict__ acc, const __nv_bfloat16* __restr
   }
 }
 
-// out[t, n] = bf16(act(acc[t, n] + bias[n])), 8 columns per thread, grid-stride over T * N / 8 vectors
-template <bool RELU>
+// out[t, n] = bf16(act(acc[t, n] + bias[n])), 8 columns per thread, grid-stride over T * N / 8 vectors.
+// ACT_GELU_TANH rounds twice, as vLLM and transformers do (the projection's bf16 output, then the activation's):
+// out = bf16(gelu_tanh(bf16(acc + bias))), with torch's CUDA formula in fp32 (aten GeluKernel.cu, approximate="tanh").
+template <int ACT>
 __global__ void __launch_bounds__(256)
 opt_bias_act_kernel(const float* __restrict__ acc, int ld_acc, const __nv_bfloat16* __restrict__ bias,
                     __nv_bfloat16* __restrict__ out, int ld_out, int T, int N) {
@@ -165,7 +167,13 @@ opt_bias_act_kernel(const float* __restrict__ acc, int ld_acc, const __nv_bfloat
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       float y = av[e] + __bfloat162float(bb.v[e]);
-      if (RELU) y = fmaxf(y, 0.f);
+      if (ACT == ACT_RELU) y = fmaxf(y, 0.f);
+      if (ACT == ACT_GELU_TANH) {
+        constexpr float kBeta = 0.7978845608028654f, kKappa = 0.044715f;  // sqrt(2 / pi)
+        const float x = bf16_round(y);
+        const float x_cube = x * x * x;
+        y = 0.5f * x * (1.f + tanhf(kBeta * (x + kKappa * x_cube)));
+      }
       o.v[e] = __float2bfloat16_rn(y);
     }
     reinterpret_cast<B8*>(out + (size_t)t * ld_out)[c] = o;
@@ -260,14 +268,18 @@ cudaError_t opt_layernorm_launch(const float* acc, const __nv_bfloat16* acc_bias
 }
 
 cudaError_t opt_bias_act_launch(const float* acc, int ld_acc, const __nv_bfloat16* bias, __nv_bfloat16* out, int ld_out,
-                                int T, int N, int relu, int num_sms, cudaStream_t stream) {
+                                int T, int N, int act, int num_sms, cudaStream_t stream) {
   if (T <= 0) return cudaSuccess;
   if (N % 8 != 0 || ld_acc % 8 != 0 || ld_out % 8 != 0) return cudaErrorInvalidValue;
   const long total = (long)T * (N / 8);
   const int grid = (int)std::min<long>((total + 255) / 256, (long)num_sms * 8);
-  if (relu)
-    return launch_k(opt_bias_act_kernel<true>, dim3(grid), dim3(256), 0, stream, acc, ld_acc, bias, out, ld_out, T, N);
-  return launch_k(opt_bias_act_kernel<false>, dim3(grid), dim3(256), 0, stream, acc, ld_acc, bias, out, ld_out, T, N);
+  if (act == ACT_RELU)
+    return launch_k(opt_bias_act_kernel<ACT_RELU>, dim3(grid), dim3(256), 0, stream, acc, ld_acc, bias, out, ld_out, T, N);
+  if (act == ACT_GELU_TANH)
+    return launch_k(opt_bias_act_kernel<ACT_GELU_TANH>, dim3(grid), dim3(256), 0, stream, acc, ld_acc, bias, out, ld_out,
+                    T, N);
+  if (act != ACT_NONE) return cudaErrorInvalidValue;
+  return launch_k(opt_bias_act_kernel<ACT_NONE>, dim3(grid), dim3(256), 0, stream, acc, ld_acc, bias, out, ld_out, T, N);
 }
 
 }  // namespace tgis

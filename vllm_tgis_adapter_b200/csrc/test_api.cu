@@ -156,8 +156,8 @@ int tgis_k_opt_layernorm(const void* acc_dev, const void* acc_bias_dev, void* re
   return 0;
 }
 
-int tgis_k_opt_bias_act(const void* acc_dev, const void* bias_dev, void* out_dev, int32_t T, int32_t N, int32_t relu) {
-  KCK(opt_bias_act_launch((const float*)acc_dev, N, (const bf16*)bias_dev, (bf16*)out_dev, N, T, N, relu, test_num_sms(), 0));
+int tgis_k_opt_bias_act(const void* acc_dev, const void* bias_dev, void* out_dev, int32_t T, int32_t N, int32_t act) {
+  KCK(opt_bias_act_launch((const float*)acc_dev, N, (const bf16*)bias_dev, (bf16*)out_dev, N, T, N, act, test_num_sms(), 0));
   KCK(cudaDeviceSynchronize());
   return 0;
 }

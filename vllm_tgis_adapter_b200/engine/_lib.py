@@ -11,7 +11,7 @@ import os
 from pathlib import Path
 
 ABI_VERSION = 8
-ARCH_LLAMA, ARCH_OPT = 0, 1
+ARCH_LLAMA, ARCH_OPT, ARCH_GPT_BIGCODE = 0, 1, 2
 MAX_REQUEST_ID = 96
 MAX_TOPN = 12
 MAX_STOP_TOKEN_IDS = 8

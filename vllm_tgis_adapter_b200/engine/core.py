@@ -36,7 +36,11 @@ class ModelConfig:
 
     Phi-3 / Phi-3.5 / Phi-4 (Phi3ForCausalLM) is arch "llama", with head_dim 96 for Phi-3-mini / Phi-3.5-mini (single
     GPU, no LoRA slots), LongRoPE for the 128k variants (rope_long_factor / rope_short_factor) and the model-wide
-    sliding_window of the 4k variants.  Its fused qkv_proj / gate_up_proj tensors are split on the host (loader.py)."""
+    sliding_window of the 4k variants.  Its fused qkv_proj / gate_up_proj tensors are split on the host (loader.py).
+
+    GPTBigCode (GPTBigCodeForCausalLM: StarCoder, SantaCoder, Granite-20B/34B-Code) is arch "gpt_bigcode": OPT's layer
+    stack with positions from 0, GELU-tanh, head_dim 128 and n_kv_heads 1 (multi_query, up to 64 query heads) or n_q_heads
+    (single GPU, no LoRA slots)."""
 
     n_layers: int        # num_hidden_layers
     hidden: int          # hidden_size
@@ -179,6 +183,22 @@ PRESETS: dict[str, ModelConfig] = {
                                   rope_theta=10000.0, rms_eps=1e-5, max_model_len=4096, fused_projections=True),
     "phi-4": ModelConfig(n_layers=40, hidden=5120, n_q_heads=40, n_kv_heads=10, ffn=17920, vocab=100352,
                          rope_theta=250000.0, rms_eps=1e-5, max_model_len=16384, fused_projections=True),
+    # GPTBigCode: two CPU-oracle-sized stacks, multi-query with 12 heads (a partial last head octet: 8 + 4) and multi-head,
+    # with an odd vocabulary, and the StarCoderBase-1B, StarCoder-15B, Granite-20B-Code and Granite-34B-Code shapes.
+    # Those four are the published bigcode/starcoderbase-1b, bigcode/starcoder, ibm-granite/granite-20b-code-base and
+    # granite-34b-code-base config.json values as recalled, not checked against the files when these presets were written.
+    "gpt-bigcode-tiny": ModelConfig(n_layers=2, hidden=1536, n_q_heads=12, n_kv_heads=1, ffn=2048, vocab=1021,
+                                    rms_eps=1e-5, max_model_len=2048, arch="gpt_bigcode", tie_word_embeddings=True),
+    "gpt-bigcode-tiny-mha": ModelConfig(n_layers=2, hidden=512, n_q_heads=4, n_kv_heads=4, ffn=1024, vocab=1021,
+                                        rms_eps=1e-5, max_model_len=2048, arch="gpt_bigcode", tie_word_embeddings=True),
+    "starcoderbase-1b": ModelConfig(n_layers=24, hidden=2048, n_q_heads=16, n_kv_heads=1, ffn=8192, vocab=49152,
+                                    rms_eps=1e-5, max_model_len=8192, arch="gpt_bigcode", tie_word_embeddings=True),
+    "starcoder-15b": ModelConfig(n_layers=40, hidden=6144, n_q_heads=48, n_kv_heads=1, ffn=24576, vocab=49152,
+                                 rms_eps=1e-5, max_model_len=8192, arch="gpt_bigcode", tie_word_embeddings=True),
+    "granite-20b-code": ModelConfig(n_layers=52, hidden=6144, n_q_heads=48, n_kv_heads=1, ffn=24576, vocab=49152,
+                                    rms_eps=1e-5, max_model_len=8192, arch="gpt_bigcode", tie_word_embeddings=True),
+    "granite-34b-code": ModelConfig(n_layers=88, hidden=6144, n_q_heads=48, n_kv_heads=1, ffn=24576, vocab=49152,
+                                    rms_eps=1e-5, max_model_len=8192, arch="gpt_bigcode", tie_word_embeddings=True),
 }
 
 
@@ -280,11 +300,16 @@ class NativeEngine:
         if model.qkv_bias and tp_size > 1:
             raise EngineError("Qwen2 (qkv_bias) is not supported with tensor parallelism: the qkv bias is implemented on a "
                               "single GPU only (use tensor_parallel_size 1)")
-        if model.arch not in ("llama", "opt"):
+        if model.arch == "gpt_bigcode" and tp_size > 1:
+            raise EngineError("GPTBigCode is not supported with tensor parallelism: it is implemented on a single GPU only "
+                              "(use tensor_parallel_size 1)")
+        if model.arch == "gpt_bigcode" and max_loras:
+            raise EngineError("GPTBigCode is not supported with LoRA adapters (--enable-lora)")
+        if model.arch not in ("llama", "opt", "gpt_bigcode"):
             raise EngineError(f"unknown architecture {model.arch!r}")
         if model.arch == "llama" and model.head_dim != 128 and model.is_granite:
             raise EngineError(f"Granite with head_dim {model.head_dim} is not supported yet (Granite needs head_dim 128)")
-        cfg.arch = _lib.ARCH_OPT if model.arch == "opt" else _lib.ARCH_LLAMA
+        cfg.arch = {"opt": _lib.ARCH_OPT, "gpt_bigcode": _lib.ARCH_GPT_BIGCODE}.get(model.arch, _lib.ARCH_LLAMA)
         self.max_loras, self.max_lora_rank = int(max_loras), int(max_lora_rank)
         self._h = C.c_void_p()
         if self.lib.tgis_engine_create(C.byref(cfg), C.byref(self._h)) != 0:

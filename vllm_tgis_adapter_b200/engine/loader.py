@@ -24,6 +24,8 @@ def model_config_from_hf(path: Path, max_model_len: int | None) -> ModelConfig:
     archs = cfg.get("architectures") or []
     if cfg.get("model_type") == "opt" or any("OPT" in a for a in archs):
         return _opt_model_config(cfg, max_model_len)
+    if cfg.get("model_type") == "gpt_bigcode" or "GPTBigCodeForCausalLM" in archs:
+        return _gpt_bigcode_model_config(cfg, max_model_len)
     if cfg.get("model_type") == "granite" or "GraniteForCausalLM" in archs:
         return _granite_model_config(cfg, max_model_len)
     if cfg.get("model_type") == "qwen3" or "Qwen3ForCausalLM" in archs:
@@ -319,6 +321,39 @@ def _opt_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
                        max_model_len=max_model_len or derived, arch="opt")
 
 
+def _gpt_bigcode_model_config(cfg: dict, max_model_len: int | None) -> ModelConfig:
+    """bigcode / ibm-granite GPTBigCodeForCausalLM config.json -> ModelConfig(arch="gpt_bigcode"), read as vLLM's
+    gpt_bigcode.py reads it: n_inner None is 4 n_embd, multi_query is one kv head, n_positions bounds max_model_len and
+    is its default.  Variants the engine would serve wrongly are refused, each with its reason."""
+    hidden, heads = cfg.get("n_embd", 768), cfg.get("n_head", 12)
+    head_dim = hidden // heads
+    problems = []
+    act = cfg.get("activation_function", "gelu_pytorch_tanh")
+    if act != "gelu_pytorch_tanh":
+        problems.append(f"activation_function {act!r} (only gelu_pytorch_tanh is implemented)")
+    if cfg.get("scale_attn_weights", True) is False:
+        problems.append("scale_attn_weights false (the attention kernels scale the scores by 1 / sqrt(head_dim))")
+    if head_dim != 128 or hidden != heads * head_dim:
+        problems.append(f"head_dim {hidden} / {heads} (the GPTBigCode attention path needs 128-dim heads)")
+    if problems:
+        raise ValueError("unsupported GPTBigCode variant: " + "; ".join(problems))
+    derived = cfg.get("n_positions", 1024)
+    if max_model_len is not None and max_model_len > derived:
+        raise ValueError(f"max_model_len {max_model_len} exceeds the model's n_positions {derived}")
+    return ModelConfig(n_layers=cfg.get("n_layer", 12), hidden=hidden, n_q_heads=heads,
+                       n_kv_heads=1 if cfg.get("multi_query", True) else heads,
+                       ffn=cfg.get("n_inner") or 4 * hidden, vocab=cfg.get("vocab_size", 50257), head_dim=head_dim,
+                       rms_eps=float(cfg.get("layer_norm_epsilon", 1e-5)), max_model_len=max_model_len or derived,
+                       arch="gpt_bigcode", tie_word_embeddings=bool(cfg.get("tie_word_embeddings", True)))
+
+
+def skip_tensor(name: str) -> bool:
+    """checkpoint tensors that are not weights: rotary inverse frequencies, and GPTBigCode's causal-mask buffers
+    (.attn.bias / .attn.masked_bias, which older checkpoints saved; vLLM skips them too).  c_attn.bias is a weight, and
+    no other architecture here names a tensor "attn.bias" (theirs are self_attn.*_proj.bias)."""
+    return name.endswith(("rotary_emb.inv_freq", ".attn.bias", ".attn.masked_bias"))
+
+
 def load_synthetic_weights(eng: NativeEngine, mc: ModelConfig, seed: int, device: int) -> None:
     import torch
 
@@ -349,6 +384,34 @@ def load_synthetic_weights(eng: NativeEngine, mc: ModelConfig, seed: int, device
             eng.load_weight(p + "fc2.weight", rnd(H, mc.ffn))
             eng.load_weight(p + "fc2.bias", vec(H))
             for ln in ("self_attn_layer_norm", "final_layer_norm"):
+                eng.load_weight(p + ln + ".weight", vec(H, 0.05, 1.0))
+                eng.load_weight(p + ln + ".bias", vec(H))
+        return
+
+    if mc.arch == "gpt_bigcode":
+        # HF GPTBigCode parameter names, LayerNorms and biases as for OPT above; c_attn is q | k | v rows
+        H, kv_dim = mc.hidden, mc.n_kv_heads * mc.head_dim
+
+        def vec(n, s=0.02, base=0.0):
+            return (base + torch.randn(n, generator=gen, device=f"cuda:{device}", dtype=torch.float32) * s).to(torch.bfloat16)
+
+        eng.load_weight("transformer.wte.weight", rnd(mc.vocab, H))
+        eng.load_weight("transformer.wpe.weight", rnd(mc.max_model_len, H))
+        eng.load_weight("transformer.ln_f.weight", vec(H, 0.05, 1.0))
+        eng.load_weight("transformer.ln_f.bias", vec(H))
+        if not mc.tie_word_embeddings:
+            eng.load_weight("lm_head.weight", rnd(mc.vocab, H))
+        for i in range(mc.n_layers):
+            p = f"transformer.h.{i}."
+            eng.load_weight(p + "attn.c_attn.weight", rnd(H + 2 * kv_dim, H))
+            eng.load_weight(p + "attn.c_attn.bias", vec(H + 2 * kv_dim))
+            eng.load_weight(p + "attn.c_proj.weight", rnd(H, H))
+            eng.load_weight(p + "attn.c_proj.bias", vec(H))
+            eng.load_weight(p + "mlp.c_fc.weight", rnd(mc.ffn, H))
+            eng.load_weight(p + "mlp.c_fc.bias", vec(mc.ffn))
+            eng.load_weight(p + "mlp.c_proj.weight", rnd(H, mc.ffn))
+            eng.load_weight(p + "mlp.c_proj.bias", vec(H))
+            for ln in ("ln_1", "ln_2"):
                 eng.load_weight(p + ln + ".weight", vec(H, 0.05, 1.0))
                 eng.load_weight(p + ln + ".bias", vec(H))
         return
@@ -397,12 +460,13 @@ def load_safetensors_dir(eng: NativeEngine, path: Path) -> None:
 
         for f in bins:
             for name, t in torch.load(str(f), map_location="cpu", weights_only=True).items():
-                eng.load_weight(name, t)
+                if not skip_tensor(name):
+                    eng.load_weight(name, t)
         return
     for f in files:
         with safe_open(str(f), framework="pt", device="cpu") as sf:
             for name in sf.keys():  # noqa: SIM118
-                if name.endswith("rotary_emb.inv_freq"):
+                if skip_tensor(name):
                     continue
                 for n, t in split_fused(name, sf.get_tensor(name), eng.model):
                     eng.load_weight(n, t)
@@ -435,7 +499,7 @@ def _make_native_engine(args, mc: ModelConfig, path, device: int, **tp_kw) -> Na
         load_safetensors_dir(eng, path)      # full tensors: a tensor-parallel engine keeps its rank's shard
     else:
         load_synthetic_weights(eng, mc, args.seed, device)
-    if mc.arch != "opt":   # OPT has learned positions (part of the checkpoint), no rotary table
+    if mc.arch == "llama":   # OPT and GPTBigCode have learned positions (part of the checkpoint), no rotary table
         eng.load_weight("tgis.rope_cos_sin", rope_cos_sin(mc))
     return eng
 
@@ -468,6 +532,10 @@ def build_engine(args) -> AsyncTGISEngine:
         raise ValueError(f"Phi-3 is supported on a single GPU only: tensor_parallel_size {tp}")
     if tp > 1 and mc.qkv_bias:
         raise ValueError(f"Qwen2 (qkv bias) is supported on a single GPU only: tensor_parallel_size {tp}")
+    if tp > 1 and mc.arch == "gpt_bigcode":
+        raise ValueError(f"GPTBigCode is supported on a single GPU only: tensor_parallel_size {tp}")
+    if mc.arch == "gpt_bigcode" and getattr(args, "enable_lora", False):
+        raise ValueError("GPTBigCode is not supported with LoRA adapters: drop --enable-lora")
     if tp > 1:
         import multiprocessing as mp
         import os
