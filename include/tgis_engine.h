@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define TGIS_ABI_VERSION 8
+#define TGIS_ABI_VERSION 9
 #define TGIS_MAX_REQUEST_ID 96
 #define TGIS_MAX_TOPN 12 /* reference forces max_logprobs >= 11: tgis_utils/args.py:214-216 */
 #define TGIS_MAX_STOP_TOKEN_IDS 8
@@ -53,7 +53,7 @@ typedef struct tgis_engine tgis_engine;
  *          do_layer_norm_before = true, word_embed_proj_dim == hidden -- facebook/opt-125m, which BASELINE configs[0]
  *          names (and the reference's tests/test_hub.py:17).  The reference's integration tests start the server without
  *          --model (tests/conftest.py:83-91), so they run vLLM's default model, which in vLLM 0.22 is Qwen/Qwen3-0.6B:
- *          TGIS_ARCH_LLAMA with tgis_engine_set_qk_norm.  64-dim heads (head_dim = 64) run on the
+ *          TGIS_ARCH_LLAMA with tgis_config.qk_norm.  64-dim heads (head_dim = 64) run on the
  *          128-dim attention tiles: the engine zero-pads every head's q/k/v rows and out_proj columns at load time, which
  *          leaves every dot product unchanged.  Single GPU, no LoRA slots. */
 #define TGIS_ARCH_LLAMA 0
@@ -101,7 +101,52 @@ typedef struct tgis_config {
   int32_t max_loras;
   int32_t max_lora_rank;
   int32_t arch;               /* TGIS_ARCH_LLAMA / TGIS_ARCH_OPT / TGIS_ARCH_GPT_BIGCODE */
-  int32_t reserved0;
+  /* The fields below describe the Llama layer stack's model variants; zero everywhere is the Llama stack, bit for bit.
+   * TGIS_ARCH_OPT and TGIS_ARCH_GPT_BIGCODE refuse any other value.
+   *
+   * Granite (GraniteForCausalLM: four scalars of its config.json; vllm model_executor/models/granite.py).  0 = the
+   * default in brackets; negative or non-finite values are refused.  Anything but the defaults needs head_dim 128
+   * (Granite with 64- or 96-dim heads is not supported yet), and residual_multiplier needs tp_size 1.
+   *   embedding_multiplier  h = bf16(embed[token] * m) after the lookup (1)
+   *   residual_multiplier   r = bf16(r + bf16(x * m)) after o_proj and after down_proj (1)
+   *   attention_multiplier  the softmax scale (1 / sqrt(head_dim))
+   *   logit_scale           1 / logits_scaling: the sampler sees bf16(logit * s) (1) */
+  float embedding_multiplier;
+  float residual_multiplier;
+  float attention_multiplier;
+  float logit_scale;
+  /* Qwen3 (Qwen3ForCausalLM: an RMSNorm over each q head and each k head after the qkv projection, before RoPE; vllm
+   * model_executor/models/qwen3.py).  qk_norm != 0 allocates the per-layer vectors (2 x n_layers x 128 bf16, outside the
+   * weight arena) and makes "model.layers.{i}.self_attn.q_norm.weight" and ".k_norm.weight" (rows = 128, cols = 1) legal
+   * weight names; tgis_engine_start then fails, naming the layer, unless every layer has both.  The norm uses rms_eps and
+   * rmsnorm's rounding points: y = bf16(bf16(x * rsqrt(mean(x^2) + eps)) * w).  head_dim 128 on a single GPU only. */
+  int32_t qk_norm;
+  /* Qwen2 / Qwen2.5 (Qwen2ForCausalLM: a bias on the q, k and v projections and nowhere else; vllm
+   * model_executor/models/qwen2.py).  qkv_bias != 0 allocates the per-layer vectors (n_layers x (n_q + 2 n_kv) x head_dim
+   * bf16, outside the weight arena) and fp32 scratch for the qkv projection, and makes
+   * "model.layers.{i}.self_attn.{q,k,v}_proj.bias" (rows = n_q x head_dim or n_kv x head_dim, cols = 1) legal weight
+   * names; tgis_engine_start then fails, naming the layer and tensor, unless every layer has all three.  The projection is
+   * rounded once after the fp32 bias add, y = bf16(x . W^T + b) (F.linear with a bias in bf16); LoRA deltas are added to
+   * that biased output, then RoPE runs.  head_dim 128 or 64 on a single GPU, not together with qk_norm. */
+  int32_t qkv_bias;
+  /* Sliding-window attention in every layer (Mistral: config.json sliding_window; vLLM applies a model-wide window to each
+   * layer).  The query at position p attends to the keys at positions p - window < k <= p, window keys including itself;
+   * 0 attends to the whole context, < 0 is refused.  Decode, prefill, chunked prefill, prompt logprobs, the split-context
+   * prefill of prefix-cache hits and CUDA-graph replays all apply it.  KV blocks stay allocated for the whole sequence.
+   * Single GPU only. */
+  int32_t sliding_window;
+  /* Scaled rotary embeddings (config.json rope_scaling / rope_parameters, e.g. rope_type llama3 or longrope): the host
+   * computes the scaled table and loads it as the weight "tgis.rope_cos_sin" ([max_model_len][head_dim] = cos | sin).
+   * != 0: tgis_engine_start fails unless that table was loaded, instead of serving the built-in unscaled one. */
+  int32_t rope_table_from_host;
+  /* Automatic prefix caching (vLLM's enable_prefix_caching; default off here, on in vLLM).  A full 32-token KV block that
+   * a completed step wrote is keyed by (its parent's key, its 32 token ids, LoRA slot + the slot's generation, bumped by
+   * every clear / weight load of the slot); a new request reuses the blocks of its longest cached prefix, leaving at least
+   * one prompt token to compute.  Unreferenced cached blocks are evicted least recently used first;
+   * tgis_status.free_blocks counts them as free.  Requests with prompt_logprobs > 0 do not read the cache.  With caching
+   * on, prefill sequences of at most 128 query rows over at least 1024 earlier tokens run on the split-context attention
+   * kernel.  Any architecture. */
+  int32_t enable_prefix_caching;
 } tgis_config;
 
 /* What the adapter's proto->SamplingParams mapping (grpc_server.py:508-628) hands to the engine. */
@@ -202,6 +247,10 @@ typedef struct tgis_status {
 const char* tgis_last_error(void);
 int tgis_abi_version(void);
 
+/* Whether the engine can serve cfg: 0, or < 0 with tgis_last_error() naming the refused field and the reason.  Touches no
+ * device, so a host can check a configuration before it sets up any GPU or spawns tensor-parallel ranks.
+ * tgis_engine_create runs the same check first. */
+int tgis_config_check(const tgis_config* cfg);
 int tgis_engine_create(const tgis_config* cfg, tgis_engine** out);
 /* name: HF Llama parameter name ("model.layers.3.self_attn.q_proj.weight", "lm_head.weight", ...) or
  * "tgis.rope_cos_sin" ([max_model_len,128] bf16 = cos|sin); arch OPT: HF OPT parameter names
@@ -211,53 +260,6 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out);
  * ptr may be host or device memory (cudaMemcpyDefault);
  * dtype 0 = bf16.  rows/cols describe the full (unsharded) tensor. */
 int tgis_engine_load_weight(tgis_engine* e, const char* name, const void* ptr, int64_t rows, int64_t cols, int32_t dtype);
-/* Granite (GraniteForCausalLM: the Llama layer stack plus four scalars of its config.json; vllm
- * model_executor/models/granite.py).  Valid only between tgis_engine_create and tgis_engine_start, TGIS_ARCH_LLAMA only.
- *   embedding_multiplier  h = bf16(embed[token] * m) after the lookup
- *   residual_multiplier   r = bf16(r + bf16(x * m)) after o_proj and after down_proj; tp_size must be 1 unless m == 1
- *   attention_multiplier  the softmax scale (0: 1 / sqrt(head_dim))
- *   logit_scale           1 / logits_scaling: the sampler sees bf16(logit * s)
- * The defaults 1, 1, 0, 1 are the Llama stack, bit for bit.  An engine created with head_dim 64 accepts only the
- * defaults (Granite with 64-dim heads is not supported yet). */
-int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, float residual_multiplier,
-                                  float attention_multiplier, float logit_scale);
-/* Scaled rotary embeddings (config.json rope_scaling / rope_parameters, e.g. rope_type llama3): the host computes the
- * scaled table and loads it as the weight "tgis.rope_cos_sin" ([max_model_len][head_dim] = cos | sin).  After this call
- * tgis_engine_start fails unless that table was loaded, instead of serving the built-in unscaled one.  Valid only between
- * tgis_engine_create and tgis_engine_start, TGIS_ARCH_LLAMA only. */
-int tgis_engine_require_rope_table(tgis_engine* e);
-/* Qwen3 (Qwen3ForCausalLM: the Llama layer stack plus an RMSNorm over each q head and each k head after the qkv
- * projection, before RoPE; vllm model_executor/models/qwen3.py).  on != 0 allocates the per-layer vectors (2 x n_layers
- * x 128 bf16, outside the weight arena) and makes "model.layers.{i}.self_attn.q_norm.weight" and ".k_norm.weight"
- * (rows = 128, cols = 1) legal weight names; tgis_engine_start then fails, naming the layer, unless every layer has both.
- * The norm uses tgis_config.rms_eps and rmsnorm's rounding points: y = bf16(bf16(x * rsqrt(mean(x^2) + eps)) * w).
- * TGIS_ARCH_LLAMA with head_dim 128 on a single GPU only.  Valid only between tgis_engine_create and tgis_engine_start;
- * on = 0 turns it off again. */
-int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on);
-/* Qwen2 / Qwen2.5 (Qwen2ForCausalLM: the Llama layer stack with a bias on the q, k and v projections and nowhere else;
- * vllm model_executor/models/qwen2.py).  on != 0 allocates the per-layer vectors (n_layers x (n_q + 2 n_kv) x head_dim
- * bf16, outside the weight arena) and fp32 scratch for the qkv projection, and makes
- * "model.layers.{i}.self_attn.{q,k,v}_proj.bias" (rows = n_q x head_dim or n_kv x head_dim, cols = 1) legal weight
- * names; tgis_engine_start then fails, naming the layer and tensor, unless every layer has all three.  The projection is
- * rounded once after the fp32 bias add, y = bf16(x . W^T + b) (F.linear with a bias in bf16); LoRA deltas are added to
- * that biased output, then RoPE runs.  TGIS_ARCH_LLAMA (head_dim 128 or 64) on a single GPU, not together with
- * tgis_engine_set_qk_norm.  Valid only between tgis_engine_create and tgis_engine_start; on = 0 turns it off again. */
-int tgis_engine_set_qkv_bias(tgis_engine* e, int32_t on);
-/* Sliding-window attention in every layer (Mistral: config.json sliding_window; vLLM applies a model-wide window to each
- * layer).  The query at position p attends to the keys at positions p - window < k <= p, window keys including itself;
- * window = 0 (the default) attends to the whole context.  Decode, prefill, chunked prefill, prompt logprobs, the
- * split-context prefill of prefix-cache hits and CUDA-graph replays all apply it.  KV blocks stay allocated for the whole
- * sequence.  Refused: window < 0, TGIS_ARCH_OPT and tp_size > 1.  Valid only between tgis_engine_create and
- * tgis_engine_start. */
-int tgis_engine_set_sliding_window(tgis_engine* e, int32_t window);
-/* Automatic prefix caching (vLLM's enable_prefix_caching; default off here, on in vLLM).  Valid only between
- * tgis_engine_create and tgis_engine_start.  A full 32-token KV block that a completed step wrote is keyed by (its
- * parent's key, its 32 token ids, LoRA slot + the slot's generation, bumped by every clear / weight load of the slot);
- * a new request reuses the blocks of its longest cached prefix, leaving at least one prompt token to compute.
- * Unreferenced cached blocks are evicted least recently used first; tgis_status.free_blocks counts them as free.
- * Requests with prompt_logprobs > 0 do not read the cache.  With caching on, prefill sequences of at most 128 query
- * rows over at least 1024 earlier tokens run on the split-context attention kernel. */
-int tgis_engine_set_prefix_caching(tgis_engine* e, int32_t on);
 /* cumulative tokens looked up / found in the cache (vllm:prefix_cache_queries / _hits: as in vLLM, the lookups of a
  * preempted request's recompute are not counted) and the keyed blocks right now */
 int tgis_engine_prefix_cache_stats(tgis_engine* e, int64_t* queried_tokens, int64_t* hit_tokens, int32_t* cached_blocks);

@@ -23,13 +23,35 @@ def test_library_exports_every_declared_symbol():
     assert lib.tgis_abi_version() == _lib.ABI_VERSION
 
 
+def test_the_model_is_described_by_the_config_and_only_run_time_switches_are_setters():
+    """Everything fixed for an engine's lifetime is a tgis_config field; the calls that change an engine after
+    tgis_engine_create are the run-time switches only"""
+    import subprocess
+
+    switches = {"tgis_engine_set_mask_provider", "tgis_engine_set_profiling"}
+    assert {s for s in _declared("tgis_engine.h") if s.startswith("tgis_engine_set_")} == switches
+    assert {s for s in _lib.ENGINE_SYMBOLS if s.startswith("tgis_engine_set_")} == switches
+    lib = _lib.load_library()
+    nm = subprocess.run(["nm", "-D", "--defined-only", str(_lib.library_path())], capture_output=True, text=True,
+                        check=True).stdout
+    exported = set(re.findall(r" T (tgis_\w+)$", nm, flags=re.M))
+    assert {s for s in exported if s.startswith("tgis_engine_set_")} == switches
+    assert exported >= set(_lib.ENGINE_SYMBOLS) and lib.tgis_abi_version() == 9
+
+
+def test_config_mirror_has_the_header_fields_in_order():
+    text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / "tgis_engine.h").read_text(), flags=re.S)
+    body = re.search(r"typedef struct tgis_config \{(.*?)\} tgis_config;", text, flags=re.S).group(1)
+    assert re.findall(r"(\w+)(?:\[\w+\])?;", body) == [name for name, _ in _lib.TgisConfig._fields_]
+
+
 def test_struct_layouts_match_the_header_sizes():
     lib = _lib.load_library()
     assert lib.tgis_k_sizeof_sample_row() == 64
     assert lib.tgis_k_sizeof_sample_out() == 112
     assert lib.tgis_k_kv_block() == 32
     assert C.sizeof(_lib.TgisSamplingParams) == 120   # static_assert in csrc/engine.cu
-    assert C.sizeof(_lib.TgisConfig) == 304           # static_assert in csrc/engine.cu (ABI v7: + arch)
+    assert C.sizeof(_lib.TgisConfig) == 336           # static_assert in csrc/engine.cu (ABI v9: + model variants)
     # id, 5 ints, 2 arrays, 4 ints, pad, 4 doubles, prompt_pos + reserved
     assert C.sizeof(_lib.TgisStepOutput) == 96 + 4 * 5 + 48 + 48 + 4 * 4 + 4 + 32 + 8
 

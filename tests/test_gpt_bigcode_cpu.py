@@ -2,7 +2,6 @@
 tiny stacks), the refusals, the skipped mask buffers, the test oracle against transformers' GPTBigCodeForCausalLM
 (tests/golden/gpt_bigcode_hf_*.json, scripts/gen_gpt_bigcode_golden.py: teacher-forced logits past one decode split and
 two KV-cache decode steps), and the ABI.  No GPU."""
-import argparse
 import ctypes as C
 import dataclasses
 import json
@@ -96,16 +95,16 @@ def test_loader_refuses_gpt_bigcode_variants_it_would_serve_wrongly(tmp_path, ov
 def test_loader_refuses_tensor_parallelism_and_lora():
     from vllm_tgis_adapter_b200.engine.core import PRESETS, EngineError, NativeEngine
     from vllm_tgis_adapter_b200.engine.loader import build_engine
+    from vllm_tgis_adapter_b200.tgis_utils.args import parse_args
 
-    args = argparse.Namespace(model="starcoder-15b", synthetic_weights=True, max_model_len=None, tensor_parallel_size=2)
-    with pytest.raises(ValueError, match="GPTBigCode is supported on a single GPU only: tensor_parallel_size 2"):
+    args = parse_args(["--model", "starcoder-15b", "--synthetic-weights", "--tensor-parallel-size", "2"])
+    with pytest.raises(ValueError, match=r"GPTBigCode runs on a single GPU only \(tp_size must be 1\)"):
         build_engine(args)
-    args = argparse.Namespace(model="starcoder-15b", synthetic_weights=True, max_model_len=None, tensor_parallel_size=1,
-                              enable_lora=True)
-    with pytest.raises(ValueError, match="GPTBigCode is not supported with LoRA adapters"):
+    args = parse_args(["--model", "starcoder-15b", "--synthetic-weights", "--enable-lora"])
+    with pytest.raises(ValueError, match="GPTBigCode: LoRA adapter slots are not supported"):
         build_engine(args)
-    # and below the loader: the engine wrapper refuses both before it reaches the library
-    with pytest.raises(EngineError, match="tensor parallelism"):
+    # and below the loader: the engine refuses both before it looks for a device
+    with pytest.raises(EngineError, match="GPTBigCode runs on a single GPU only"):
         NativeEngine(PRESETS["starcoder-15b"], tp_size=2, tp_rank=0, nccl_id=bytes(128))
     with pytest.raises(EngineError, match="LoRA"):
         NativeEngine(PRESETS["starcoder-15b"], max_loras=2)
@@ -213,9 +212,9 @@ def test_arch_is_mirrored_and_the_abi_is_unchanged():
     lib = _lib.load_library()
     header = (ROOT / "include" / "tgis_engine.h").read_text()
     assert re.search(r"#define TGIS_ARCH_GPT_BIGCODE 2\b", header) and _lib.ARCH_GPT_BIGCODE == 2
-    assert re.search(r"#define TGIS_ABI_VERSION 8\b", header)
-    assert _lib.ABI_VERSION == 8 and lib.tgis_abi_version() == 8
-    assert C.sizeof(_lib.TgisConfig) == 304 and C.sizeof(_lib.TgisSamplingParams) == 120
+    assert re.search(r"#define TGIS_ABI_VERSION 9\b", header)
+    assert _lib.ABI_VERSION == 9 and lib.tgis_abi_version() == 9
+    assert C.sizeof(_lib.TgisConfig) == 336 and C.sizeof(_lib.TgisSamplingParams) == 120
     # no new entry point: the architecture is a tgis_config.arch value
     decl = set(re.findall(r"\b(tgis_engine_\w+)\s*\(", re.sub(r"/\*.*?\*/", "", header, flags=re.S)))
     assert decl == {s for s in _lib.ENGINE_SYMBOLS if s.startswith("tgis_engine_")}

@@ -2,6 +2,7 @@
 its refusals, and the C ABI additions."""
 import ctypes as C
 import json
+import re
 from pathlib import Path
 
 import numpy as np
@@ -14,6 +15,7 @@ from oracle.llama_oracle import LlamaOracle
 from oracle.llama_oracle import synthetic_weights as llama_synthetic_weights
 
 GOLD = Path(__file__).parent / "golden"
+ROOT = Path(__file__).resolve().parent.parent
 
 
 def _oracle_logits(g: dict, dtype: torch.dtype) -> torch.Tensor:
@@ -139,18 +141,20 @@ def test_granite_presets_agree_with_the_oracle_configs():
 
 
 # ------------------------------------------------------------------------------------------------ C ABI
-def test_abi_v8_exports_the_model_scalars_call_and_keeps_struct_sizes():
+def test_abi_v9_carries_the_model_scalars_in_the_config():
     from vllm_tgis_adapter_b200.engine import _lib
 
     lib = _lib.load_library()
-    assert _lib.ABI_VERSION == 8 == lib.tgis_abi_version()
-    for sym in ("tgis_engine_set_model_scalars", "tgis_k_rmsnorm_mult", "tgis_k_embed", "tgis_k_sampler_scaled"):
+    assert _lib.ABI_VERSION == 9 == lib.tgis_abi_version()
+    for sym in ("tgis_k_rmsnorm_mult", "tgis_k_embed", "tgis_k_sampler_scaled"):
         assert hasattr(lib, sym), sym
-    assert C.sizeof(_lib.TgisConfig) == 304
+    fields = [f for f, _ in _lib.TgisConfig._fields_]
+    header = (ROOT / "include" / "tgis_engine.h").read_text()
+    for f in ("embedding_multiplier", "residual_multiplier", "attention_multiplier", "logit_scale"):
+        assert f in fields and re.search(rf"float {f};", header), f
+    assert C.sizeof(_lib.TgisConfig) == 336
     assert C.sizeof(_lib.TgisSamplingParams) == 120
     assert lib.tgis_k_sizeof_sample_row() == 64 and lib.tgis_k_sizeof_sample_out() == 112
-    # a null engine is an error, not a crash
-    assert lib.tgis_engine_set_model_scalars(None, 1.0, 1.0, 0.0, 1.0) != 0
 
 
 def test_granite_under_tensor_parallelism_is_refused_before_any_rank_starts():

@@ -374,19 +374,18 @@ def test_granite_tiny_graphs_and_batch_invariance():
 
 
 def test_granite_scalars_only_before_start_and_64_dim_heads_refused():
+    import dataclasses
+
     from granite_oracle import CONFIGS
-    from vllm_tgis_adapter_b200.engine import _lib
     from vllm_tgis_adapter_b200.engine.core import EngineError, NativeEngine
 
     cfg = CONFIGS["granite-tiny"]
     eng = NativeEngine(_mc(cfg), max_num_seqs=2, max_batched_tokens=64, kv_cache_bytes=16 << 20)
-    lib = eng.lib
-    assert lib.tgis_engine_set_model_scalars(eng._h, 12.0, 0.22, 0.0, 1.0) == 0
-    assert lib.tgis_engine_set_model_scalars(eng._h, 12.0, -1.0, 0.0, 1.0) != 0
     eng.start()
-    assert lib.tgis_engine_set_model_scalars(eng._h, 12.0, 0.22, 0.0, 1.0) != 0
-    assert "before tgis_engine_start" in _lib.last_error(lib)
     eng.close()
+    with pytest.raises(EngineError, match="finite and non-negative"):
+        NativeEngine(dataclasses.replace(_mc(cfg), residual_multiplier=-1.0), max_num_seqs=2, max_batched_tokens=64,
+                     kv_cache_bytes=16 << 20)
     with pytest.raises(EngineError, match="head_dim"):
         NativeEngine(_mc(cfg, head_dim=64), max_num_seqs=2, max_batched_tokens=64, kv_cache_bytes=16 << 20)
 

@@ -166,8 +166,7 @@ def test_new_symbols_are_declared_and_exported():
     from vllm_tgis_adapter_b200.engine import _lib
 
     lib = _lib.load_library()
-    new = {"tgis_engine.h": ["tgis_engine_require_rope_table"],
-           "tgis_kernels.h": ["tgis_k_rope_kv_hd", "tgis_k_attention_hd", "tgis_k_attention_split_hd",
+    new = {"tgis_kernels.h": ["tgis_k_rope_kv_hd", "tgis_k_attention_hd", "tgis_k_attention_split_hd",
                               "tgis_k_attention_bench_hd"]}
     for header, syms in new.items():
         text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / header).read_text(), flags=re.S)
@@ -175,7 +174,9 @@ def test_new_symbols_are_declared_and_exported():
             assert re.search(rf"\b{sym}\s*\(", text), (header, sym)
             assert hasattr(lib, sym), sym
             assert sym in _lib.ENGINE_SYMBOLS + _lib.KERNEL_SYMBOLS
-    # the config struct did not grow: head_dim 64 and the table requirement need no ABI change
+    # the table requirement is a tgis_config field (ABI v9), not a call of its own
     import ctypes as C
 
-    assert C.sizeof(_lib.TgisConfig) == 304 and lib.tgis_abi_version() == _lib.ABI_VERSION
+    header = (ROOT / "include" / "tgis_engine.h").read_text()
+    assert "rope_table_from_host" in [f for f, _ in _lib.TgisConfig._fields_] and "int32_t rope_table_from_host;" in header
+    assert C.sizeof(_lib.TgisConfig) == 336 and lib.tgis_abi_version() == _lib.ABI_VERSION == 9

@@ -180,19 +180,28 @@ def test_start_up_refusals():
         NativeEngine(_mc(embedding_multiplier=12.0), **kw)
     with pytest.raises(EngineError, match="GQA group size must be 1, 2, 4 or 8"):
         NativeEngine(_mc(n_q_heads=6, n_kv_heads=2, hidden=384), **kw)
-    # the C ABI refuses Granite scalars on a 64-dim engine too (NativeEngine checks first)
-    eng = NativeEngine(_mc(rope_scaling_factor=0.0), **kw)
-    from vllm_tgis_adapter_b200.engine import _lib
+    with pytest.raises(EngineError, match="head_dim"):
+        NativeEngine(_mc(rope_scaling_factor=0.0, residual_multiplier=0.22), **kw)
+    # the Llama defaults are fine, spelled 1 or 0
+    NativeEngine(_mc(rope_scaling_factor=0.0, embedding_multiplier=1.0, residual_multiplier=1.0), **kw).close()
+    import ctypes as C
 
-    assert eng.lib.tgis_engine_set_model_scalars(eng._h, 12.0, 0.22, 0.0, 1.0) != 0
-    assert "head_dim" in _lib.last_error(eng.lib)
-    assert eng.lib.tgis_engine_set_model_scalars(eng._h, 1.0, 1.0, 0.0, 1.0) == 0   # the Llama defaults are fine
+    from vllm_tgis_adapter_b200.engine.core import engine_config
+
+    cfg = engine_config(_mc(rope_scaling_factor=0.0), **kw)
+    cfg.embedding_multiplier = cfg.residual_multiplier = cfg.attention_multiplier = cfg.logit_scale = 0.0
+    eng = NativeEngine(_mc(rope_scaling_factor=0.0), **kw)
+    eng.close()
+    assert eng.lib.tgis_engine_create(C.byref(cfg), C.byref(eng._h)) == 0
     eng.close()
     # a model whose rotary table is scaled must be given it: the built-in table is the unscaled one.  NativeEngine loads the
-    # table of a scaled config itself; through the C ABI alone the requirement stands until the table arrives
+    # table of a scaled config itself; through the C ABI alone the requirement stands until the table arrives.  The
+    # wrapper is reused around an engine created from the raw config.
+    cfg.rope_table_from_host = 1
     eng = NativeEngine(_mc(rope_scaling_factor=0.0), **kw)
+    eng.close()
+    assert eng.lib.tgis_engine_create(C.byref(cfg), C.byref(eng._h)) == 0
     eng.load_weights(_weights())
-    assert eng.lib.tgis_engine_require_rope_table(eng._h) == 0
     with pytest.raises(EngineError, match="rope_cos_sin"):
         eng.start()
     with pytest.raises(EngineError, match="rope_cos_sin"):

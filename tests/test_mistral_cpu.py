@@ -2,7 +2,6 @@
 rope spellings), the refusals, the test oracle against transformers' MistralForCausalLM (tests/golden/mistral_hf_*.json,
 scripts/gen_mistral_golden.py: teacher-forced logits over a prompt longer than twice the window and a KV-cache decode
 step past it), the decode work-item list under a window, and the new C-ABI symbols.  No GPU."""
-import argparse
 import ctypes as C
 import json
 import re
@@ -150,10 +149,11 @@ def test_loader_refuses_mistral_variants_it_would_serve_wrongly(tmp_path, over, 
 
 def test_loader_refuses_mistral_under_tensor_parallelism():
     from vllm_tgis_adapter_b200.engine.loader import build_engine
+    from vllm_tgis_adapter_b200.tgis_utils.args import parse_args
 
-    args = argparse.Namespace(model="mistral-7b-v0.1", synthetic_weights=True, max_model_len=None,
-                              tensor_parallel_size=2)
-    with pytest.raises(ValueError, match="single GPU only: tensor_parallel_size 2"):
+    args = parse_args(["--model", "mistral-7b-v0.1", "--synthetic-weights", "--tensor-parallel-size", "2"])
+    reason = r"sliding-window attention is supported on a single GPU only \(tp_size must be 1\)"
+    with pytest.raises(ValueError, match=reason):
         build_engine(args)
 
 
@@ -322,20 +322,19 @@ def test_new_symbols_are_declared_and_exported_and_the_abi_is_unchanged():
     from vllm_tgis_adapter_b200.engine import _lib
 
     lib = _lib.load_library()
-    new = {"tgis_engine.h": ["tgis_engine_set_sliding_window"],
-           "tgis_kernels.h": ["tgis_k_attention_window", "tgis_k_attention_bench_window", "tgis_k_decode_items_window"]}
+    new = {"tgis_kernels.h": ["tgis_k_attention_window", "tgis_k_attention_bench_window", "tgis_k_decode_items_window"]}
     for header, syms in new.items():
         text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / header).read_text(), flags=re.S)
         for sym in syms:
             assert re.search(rf"\b{sym}\s*\(", text), (header, sym)
             assert hasattr(lib, sym), sym
             assert sym in _lib.ENGINE_SYMBOLS + _lib.KERNEL_SYMBOLS
-    # the config struct did not grow and the version did not move: the window is a call of its own
-    assert _lib.ABI_VERSION == 8 and lib.tgis_abi_version() == 8
-    assert C.sizeof(_lib.TgisConfig) == 304 and C.sizeof(_lib.TgisSamplingParams) == 120
-    assert re.search(r"#define TGIS_ABI_VERSION 8\b", (ROOT / "include" / "tgis_engine.h").read_text())
-    # the setter needs an engine, which needs a GPU: a null one is refused before anything else
-    assert lib.tgis_engine_set_sliding_window(None, 40) != 0
+    # the window is a tgis_config field (ABI v9), not a call of its own
+    header = (ROOT / "include" / "tgis_engine.h").read_text()
+    assert "sliding_window" in [f for f, _ in _lib.TgisConfig._fields_] and "int32_t sliding_window;" in header
+    assert _lib.ABI_VERSION == 9 and lib.tgis_abi_version() == 9
+    assert C.sizeof(_lib.TgisConfig) == 336 and C.sizeof(_lib.TgisSamplingParams) == 120
+    assert re.search(r"#define TGIS_ABI_VERSION 9\b", header)
 
 
 def test_the_library_holds_sm_90a_code():

@@ -217,31 +217,26 @@ class _Rec:
 
 
 def test_start_up_refusals():
-    from vllm_tgis_adapter_b200.engine import _lib
     from vllm_tgis_adapter_b200.engine.core import PRESETS, EngineError, NativeEngine
 
     kw = dict(max_num_seqs=2, max_batched_tokens=64, kv_cache_bytes=16 << 20)
-    with pytest.raises(EngineError, match="tgis_engine_set_sliding_window failed: .*not OPT"):
+    with pytest.raises(EngineError, match="tgis_engine_create failed: .*not OPT"):
         NativeEngine(dataclasses.replace(PRESETS["opt-tiny"], sliding_window=40), **kw)
     with pytest.raises(EngineError, match="single GPU only"):
         NativeEngine(_mc(), tp_size=2, tp_rank=0, nccl_id=bytes(128), shm_name="/tgis_test_unused", **kw)
-    eng = NativeEngine(_mc(sliding_window=None), **kw)
-    assert eng.lib.tgis_engine_set_sliding_window(eng._h, -1) != 0
-    assert ">= 0" in _lib.last_error(eng.lib)
-    assert eng.lib.tgis_engine_set_sliding_window(eng._h, 40) == 0
-    assert eng.lib.tgis_engine_set_sliding_window(eng._h, 0) == 0
-    eng.load_weights(_weights())
-    eng.start()
-    assert eng.lib.tgis_engine_set_sliding_window(eng._h, 40) != 0
-    assert "before tgis_engine_start" in _lib.last_error(eng.lib)
-    eng.close()
+    with pytest.raises(EngineError, match=">= 0"):
+        NativeEngine(_mc(sliding_window=-1), **kw)
+    for window in (40, 0):
+        eng = NativeEngine(_mc(sliding_window=window), **kw)
+        eng.load_weights(_weights())
+        eng.start()
+        eng.close()
 
 
 def test_window_zero_through_the_setter_equals_no_window():
     prompts = [_prompt(n, 90 + n) for n in (50, 170)]
     a = _engine(model=_mc(sliding_window=None))
-    b = _engine(model=_mc(sliding_window=None))
-    assert b.lib.tgis_engine_set_sliding_window(b._h, 0) == 0
+    b = _engine(model=_mc(sliding_window=0))
     ra, rb = _gen(a, prompts, _sp()), _gen(b, prompts, _sp())
     a.close()
     b.close()

@@ -237,8 +237,8 @@ def test_the_abi_is_unchanged():
     from vllm_tgis_adapter_b200.engine import _lib
 
     lib = _lib.load_library()
-    assert _lib.ABI_VERSION == 8 and lib.tgis_abi_version() == 8
-    assert C.sizeof(_lib.TgisConfig) == 304 and C.sizeof(_lib.TgisSamplingParams) == 120
+    assert _lib.ABI_VERSION == 9 and lib.tgis_abi_version() == 9
+    assert C.sizeof(_lib.TgisConfig) == 336 and C.sizeof(_lib.TgisSamplingParams) == 120
 
 
 def test_the_library_holds_sm_90a_code_with_96_dim_kernels():

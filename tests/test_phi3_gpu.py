@@ -188,8 +188,9 @@ def test_kv_blocks_follow_the_head_dim():
 
 
 def test_start_up_refusals():
-    from vllm_tgis_adapter_b200.engine import _lib
-    from vllm_tgis_adapter_b200.engine.core import EngineError, NativeEngine
+    import ctypes as C
+
+    from vllm_tgis_adapter_b200.engine.core import EngineError, NativeEngine, engine_config
 
     kw = dict(max_num_seqs=2, max_batched_tokens=64, kv_cache_bytes=16 << 20)
     with pytest.raises(EngineError, match="head_dim 96: GQA group size must be 1, 2, 4 or 8"):
@@ -198,16 +199,20 @@ def test_start_up_refusals():
         NativeEngine(_mc(512), max_loras=2, **kw)
     with pytest.raises(EngineError, match="single GPU only"):
         NativeEngine(_mc(512), tp_size=2, tp_rank=0, nccl_id=bytes(128), shm_name="/tgis_test_unused", **kw)
+    with pytest.raises(EngineError, match="q/k norm .*head_dim 128"):
+        NativeEngine(_mc(512, longrope=False, qk_norm=True), **kw)
+    with pytest.raises(EngineError, match="head_dim 128 or 64"):
+        NativeEngine(_mc(512, longrope=False, qkv_bias=True), **kw)
+    with pytest.raises(EngineError, match="96-dim heads"):
+        NativeEngine(_mc(512, longrope=False, embedding_multiplier=12.0), **kw)
+    NativeEngine(_mc(512, longrope=False, sliding_window=40), **kw).close()
+    # a LongRoPE engine refuses to start without its table.  NativeEngine loads it itself, so the wrapper is reused
+    # around an engine created from the raw config.
+    cfg = engine_config(_mc(512, longrope=False), **kw)
+    cfg.rope_table_from_host = 1
     eng = NativeEngine(_mc(512, longrope=False), **kw)
-    assert eng.lib.tgis_engine_set_qk_norm(eng._h, 1) != 0 and "head_dim 128" in _lib.last_error(eng.lib)
-    assert eng.lib.tgis_engine_set_qkv_bias(eng._h, 1) != 0 and "head_dim 128 or 64" in _lib.last_error(eng.lib)
-    assert eng.lib.tgis_engine_set_model_scalars(eng._h, 12.0, 1.0, 0.0, 1.0) != 0
-    assert "96-dim heads" in _lib.last_error(eng.lib)
-    assert eng.lib.tgis_engine_set_sliding_window(eng._h, 40) == 0
     eng.close()
-    # a LongRoPE engine refuses to start without its table
-    eng = NativeEngine(_mc(512, longrope=False), **kw)
-    assert eng.lib.tgis_engine_require_rope_table(eng._h) == 0
+    assert eng.lib.tgis_engine_create(C.byref(cfg), C.byref(eng._h)) == 0
     eng.load_weights(_weights())
     with pytest.raises(Exception, match="rope"):
         eng.start()

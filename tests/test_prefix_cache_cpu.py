@@ -91,11 +91,10 @@ def test_http_metrics_reads_the_stats_call():
 
 def test_new_symbols_exported_and_null_safe():
     lib = _lib.load_library()
-    for name in ("tgis_engine_set_prefix_caching", "tgis_engine_prefix_cache_stats", "tgis_k_attention_split",
-                 "tgis_k_attention_split_bench"):
+    for name in ("tgis_engine_prefix_cache_stats", "tgis_k_attention_split", "tgis_k_attention_split_bench"):
         assert hasattr(lib, name), name
-    assert lib.tgis_engine_set_prefix_caching(None, 1) != 0
-    assert "null" in _lib.last_error(lib)
+    # prefix caching is a tgis_config field (ABI v9), not a call of its own
+    assert "enable_prefix_caching" in [f for f, _ in _lib.TgisConfig._fields_]
     q, h, n = C.c_int64(-1), C.c_int64(-1), C.c_int32(-1)
     assert lib.tgis_engine_prefix_cache_stats(None, C.byref(q), C.byref(h), C.byref(n)) != 0
     assert "null" in _lib.last_error(lib)
@@ -104,6 +103,6 @@ def test_new_symbols_exported_and_null_safe():
 
 def test_abi_version_and_struct_sizes_unchanged():
     lib = _lib.load_library()
-    assert _lib.ABI_VERSION == 8 and lib.tgis_abi_version() == 8
-    assert C.sizeof(_lib.TgisConfig) == 304
+    assert _lib.ABI_VERSION == 9 and lib.tgis_abi_version() == 9
+    assert C.sizeof(_lib.TgisConfig) == 336
     assert C.sizeof(_lib.TgisStatus) == 4 * 6 + 8 * 17

@@ -2,7 +2,6 @@
 defaults where they differ from transformers', the refusals, the test oracle against transformers' Qwen2ForCausalLM
 (tests/golden/qwen2_hf_*.json, scripts/gen_qwen2_golden.py: teacher-forced logits and a KV-cache decode step), and the
 new C-ABI symbols.  No GPU."""
-import argparse
 import ctypes as C
 import json
 import re
@@ -137,9 +136,10 @@ def test_loader_refuses_qwen2_variants_it_would_serve_wrongly(tmp_path, over, re
 
 def test_loader_refuses_qwen2_under_tensor_parallelism():
     from vllm_tgis_adapter_b200.engine.loader import build_engine
+    from vllm_tgis_adapter_b200.tgis_utils.args import parse_args
 
-    args = argparse.Namespace(model="qwen2.5-7b", synthetic_weights=True, max_model_len=None, tensor_parallel_size=2)
-    with pytest.raises(ValueError, match="Qwen2 .*single GPU only: tensor_parallel_size 2"):
+    args = parse_args(["--model", "qwen2.5-7b", "--synthetic-weights", "--tensor-parallel-size", "2"])
+    with pytest.raises(ValueError, match=r"Qwen2\) is supported on a single GPU only \(tp_size must be 1\)"):
         build_engine(args)
 
 
@@ -233,14 +233,16 @@ def test_new_symbols_are_declared_and_exported_and_the_abi_is_unchanged():
     from vllm_tgis_adapter_b200.engine import _lib
 
     lib = _lib.load_library()
-    new = {"tgis_engine.h": ["tgis_engine_set_qkv_bias"], "tgis_kernels.h": ["tgis_k_rope_kv_bias"]}
+    new = {"tgis_kernels.h": ["tgis_k_rope_kv_bias"]}
     for header, syms in new.items():
         text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / header).read_text(), flags=re.S)
         for sym in syms:
             assert re.search(rf"\b{sym}\s*\(", text), (header, sym)
             assert hasattr(lib, sym), sym
             assert sym in _lib.ENGINE_SYMBOLS + _lib.KERNEL_SYMBOLS
-    # the config struct did not grow and the version did not move: the qkv bias is a call of its own
-    assert _lib.ABI_VERSION == 8 and lib.tgis_abi_version() == 8
-    assert C.sizeof(_lib.TgisConfig) == 304 and C.sizeof(_lib.TgisSamplingParams) == 120
-    assert re.search(r"#define TGIS_ABI_VERSION 8\b", (ROOT / "include" / "tgis_engine.h").read_text())
+    # the qkv bias is a tgis_config field (ABI v9), not a call of its own
+    header = (ROOT / "include" / "tgis_engine.h").read_text()
+    assert "qkv_bias" in [f for f, _ in _lib.TgisConfig._fields_] and "int32_t qkv_bias;" in header
+    assert _lib.ABI_VERSION == 9 and lib.tgis_abi_version() == 9
+    assert C.sizeof(_lib.TgisConfig) == 336 and C.sizeof(_lib.TgisSamplingParams) == 120
+    assert re.search(r"#define TGIS_ABI_VERSION 9\b", header)

@@ -1,7 +1,6 @@
 """Qwen3 on the host side: config.json mapping (the tiny, 0.6B and 8B shapes, both rope spellings), the refusals, the test
 oracle against transformers' Qwen3ForCausalLM (tests/golden/qwen3_hf_*.json, scripts/gen_qwen3_golden.py: teacher-forced
 logits and a KV-cache decode step), and the new C-ABI symbols.  No GPU."""
-import argparse
 import ctypes as C
 import json
 import re
@@ -113,9 +112,10 @@ def test_loader_refuses_qwen3_variants_it_would_serve_wrongly(tmp_path, over, re
 
 def test_loader_refuses_qwen3_under_tensor_parallelism():
     from vllm_tgis_adapter_b200.engine.loader import build_engine
+    from vllm_tgis_adapter_b200.tgis_utils.args import parse_args
 
-    args = argparse.Namespace(model="qwen3-0.6b", synthetic_weights=True, max_model_len=None, tensor_parallel_size=2)
-    with pytest.raises(ValueError, match="single GPU only: tensor_parallel_size 2"):
+    args = parse_args(["--model", "qwen3-0.6b", "--synthetic-weights", "--tensor-parallel-size", "2"])
+    with pytest.raises(ValueError, match=r"Qwen3\) is supported on a single GPU only \(tp_size must be 1\)"):
         build_engine(args)
 
 
@@ -185,14 +185,16 @@ def test_new_symbols_are_declared_and_exported_and_the_abi_is_unchanged():
     from vllm_tgis_adapter_b200.engine import _lib
 
     lib = _lib.load_library()
-    new = {"tgis_engine.h": ["tgis_engine_set_qk_norm"], "tgis_kernels.h": ["tgis_k_rope_kv_qknorm"]}
+    new = {"tgis_kernels.h": ["tgis_k_rope_kv_qknorm"]}
     for header, syms in new.items():
         text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / header).read_text(), flags=re.S)
         for sym in syms:
             assert re.search(rf"\b{sym}\s*\(", text), (header, sym)
             assert hasattr(lib, sym), sym
             assert sym in _lib.ENGINE_SYMBOLS + _lib.KERNEL_SYMBOLS
-    # the config struct did not grow and the version did not move: the q/k norm is a call of its own
-    assert _lib.ABI_VERSION == 8 and lib.tgis_abi_version() == 8
-    assert C.sizeof(_lib.TgisConfig) == 304 and C.sizeof(_lib.TgisSamplingParams) == 120
-    assert re.search(r"#define TGIS_ABI_VERSION 8\b", (ROOT / "include" / "tgis_engine.h").read_text())
+    # the q/k norm is a tgis_config field (ABI v9), not a call of its own
+    header = (ROOT / "include" / "tgis_engine.h").read_text()
+    assert "qk_norm" in [f for f, _ in _lib.TgisConfig._fields_] and "int32_t qk_norm;" in header
+    assert _lib.ABI_VERSION == 9 and lib.tgis_abi_version() == 9
+    assert C.sizeof(_lib.TgisConfig) == 336 and C.sizeof(_lib.TgisSamplingParams) == 120
+    assert re.search(r"#define TGIS_ABI_VERSION 9\b", header)

@@ -349,13 +349,12 @@ def test_lora_follows_the_oracle_and_leaves_base_requests_untouched(tmp_path):
 
 
 def test_start_up_refusals():
-    from vllm_tgis_adapter_b200.engine import _lib
     from vllm_tgis_adapter_b200.engine.core import PRESETS, EngineError, NativeEngine
 
     kw = dict(max_num_seqs=2, max_batched_tokens=64, kv_cache_bytes=16 << 20)
-    with pytest.raises(EngineError, match="tgis_engine_set_qk_norm failed: .*not OPT"):
+    with pytest.raises(EngineError, match="tgis_engine_create failed: .*not OPT"):
         NativeEngine(dataclasses.replace(PRESETS["opt-tiny"], qk_norm=True), **kw)
-    with pytest.raises(EngineError, match="tgis_engine_set_qk_norm failed: .*head_dim 128"):
+    with pytest.raises(EngineError, match="tgis_engine_create failed: .*head_dim 128"):
         NativeEngine(_mc(head_dim=64, n_q_heads=4, hidden=256), **kw)
     with pytest.raises(EngineError, match="single GPU only"):
         NativeEngine(_mc(), tp_size=2, tp_rank=0, nccl_id=bytes(128), shm_name="/tgis_test_unused", **kw)
@@ -375,18 +374,10 @@ def test_start_up_refusals():
         eng.start()
     eng.load_weight("model.layers.1.self_attn.k_norm.weight", _weights()["model.layers.1.self_attn.k_norm.weight"])
     eng.start()
-    assert eng.lib.tgis_engine_set_qk_norm(eng._h, 1) != 0
-    assert "before tgis_engine_start" in _lib.last_error(eng.lib)
     eng.close()
     # the norm weights are not names a Llama engine knows, as before
     eng = NativeEngine(_mc(qk_norm=False), **kw)
     with pytest.raises(EngineError, match="unknown layer weight model.layers.0.self_attn.q_norm.weight"):
-        eng.load_weight("model.layers.0.self_attn.q_norm.weight", torch.ones(128, dtype=torch.bfloat16))
-    # ... and through the C ABI: on, then off again
-    assert eng.lib.tgis_engine_set_qk_norm(eng._h, 1) == 0
-    eng.load_weight("model.layers.0.self_attn.q_norm.weight", torch.ones(128, dtype=torch.bfloat16))
-    assert eng.lib.tgis_engine_set_qk_norm(eng._h, 0) == 0
-    with pytest.raises(EngineError, match="unknown layer weight"):
         eng.load_weight("model.layers.0.self_attn.q_norm.weight", torch.ones(128, dtype=torch.bfloat16))
     eng.close()
 

@@ -239,12 +239,12 @@ struct tgis_engine {
   bf16 *embed = nullptr, *lm_head = nullptr, *final_norm = nullptr, *cos_sin = nullptr;
   bool lm_head_loaded = false, cos_sin_loaded = false;
   bool rope_table_required = false;  // scaled RoPE: default_rope_table() is not this model's table
-  // Qwen3 (tgis_engine_set_qk_norm): layer l's q_norm [128] at qk_norm_w + 256 l, its k_norm 128 further, in an
+  // Qwen3 (tgis_config.qk_norm): layer l's q_norm [128] at qk_norm_w + 256 l, its k_norm 128 further, in an
   // allocation of their own, so that the arena and the KV block count of every other model stay as they are;
   // qk_norm_loaded: per layer, bit 0 = q_norm, bit 1 = k_norm
   DevBuf<bf16> qk_norm_w;
   std::vector<uint8_t> qk_norm_loaded;
-  // Qwen2 (tgis_engine_set_qkv_bias): layer l's q | k | v bias [qkv_dim] at qkv_bias_w + qkv_dim l, in wqkv's row order
+  // Qwen2 (tgis_config.qkv_bias): layer l's q | k | v bias [qkv_dim] at qkv_bias_w + qkv_dim l, in wqkv's row order
   // and an allocation of its own (the qkv GEMM then writes fp32 to y32); qkv_bias_loaded: per layer, bit 0 = q, 1 = k,
   // 2 = v
   DevBuf<bf16> qkv_bias_w;
@@ -259,8 +259,8 @@ struct tgis_engine {
   // table and the KV tiles, i.e. of the kernels that run.  They differ for OPT only (64-dim heads zero-padded to 128).
   int pos_rows = 0, model_head_dim = HEAD_DIM, kv_head_dim = HEAD_DIM;
   float attn_scale = 0.f;
-  // Granite's scalars (tgis_engine_set_model_scalars; 1 = the Llama stack): embedding and residual multipliers, and the
-  // scale of the bf16 logits the sampler sees (1 / logits_scaling)
+  // Granite's scalars (tgis_config.*_multiplier and logit_scale; 1 = the Llama stack): embedding and residual
+  // multipliers, and the scale of the bf16 logits the sampler sees (1 / logits_scaling)
   float emb_mult = 1.f, res_mult = 1.f, logit_scale = 1.f;
   // rows of embed / lm_head: the vocabulary rounded up to a multiple of 8 (the padded rows are zero), so that the lm_head
   // GEMM's output rows stay 16-byte aligned for any vocabulary; the sampler is told ld = Vpad, vocab = V
@@ -274,11 +274,11 @@ struct tgis_engine {
   size_t kv_layer_elems = 0;
   int num_blocks = 0;
   std::vector<int32_t> free_blocks;
-  // prefix caching (tgis_engine_set_prefix_caching; rank 0's scheduler only): per block a reference count and, for a
+  // prefix caching (tgis_config.enable_prefix_caching; rank 0's scheduler only): per block a reference count and, for a
   // full block whose KV a completed step wrote, its cache entry.  A keyed block nobody references sits in the evictable
   // LRU (front = least recently used) and keeps its key until it is reallocated.
   bool prefix_caching = false;
-  // sliding-window attention (tgis_engine_set_sliding_window): every layer's query at position p sees the keys
+  // sliding-window attention (tgis_config.sliding_window): every layer's query at position p sees the keys
   // p - window < k <= p; 0 = the whole context.  KV blocks stay allocated for the whole sequence.
   int attn_window = 0;
   struct PcBlock {
@@ -477,7 +477,15 @@ struct tgis_engine {
     opt = c.arch == TGIS_ARCH_OPT || bigcode;
     model_head_dim = c.head_dim;
     kv_head_dim = opt ? HEAD_DIM : c.head_dim;
-    attn_scale = 1.0f / std::sqrt((float)model_head_dim);  // zero-padded head dims add nothing to q . k
+    // zero-padded head dims add nothing to q . k
+    attn_scale = c.attention_multiplier > 0.f ? c.attention_multiplier : 1.0f / std::sqrt((float)model_head_dim);
+    auto or_one = [](float m) { return m > 0.f ? m : 1.f; };
+    emb_mult = or_one(c.embedding_multiplier);
+    res_mult = or_one(c.residual_multiplier);
+    logit_scale = or_one(c.logit_scale);
+    attn_window = c.sliding_window;
+    rope_table_required = c.rope_table_from_host != 0;
+    prefix_caching = c.enable_prefix_caching != 0;
     pos_rows = bigcode ? c.max_model_len : opt ? c.max_model_len + 2 : 0;
     q_dim = nq * kv_head_dim;
     qkv_dim = (nq + 2 * nkv) * kv_head_dim;
@@ -685,6 +693,17 @@ struct tgis_engine {
     for (int i = 0; i < num_blocks; ++i) free_blocks[i] = num_blocks - 1 - i;
     free_slots.resize(S_max);
     for (int i = 0; i < S_max; ++i) free_slots[i] = S_max - 1 - i;
+    // after the KV cache: with kv_cache_bytes == 0 its size comes from the free memory, which these must not shrink
+    if (c.qk_norm) {
+      qk_norm_w.alloc((size_t)2 * L * HEAD_DIM);
+      qk_norm_loaded.assign(L, 0);
+    }
+    if (c.qkv_bias) {
+      y32.alloc(T_alloc * qkv_dim);
+      qkv_bias_w.alloc(L * qkv_dim);
+      qkv_bias_loaded.assign(L, 0);
+    }
+    if (prefix_caching) pcb.assign(num_blocks, PcBlock{});
     snapshot();
     CK(cudaStreamSynchronize(stream));
     CK(cudaDeviceSynchronize());
@@ -2244,11 +2263,11 @@ extern "C" {
 const char* tgis_last_error(void) { return g_last_error.c_str(); }
 static_assert(offsetof(tgis_sampling_params, lora_slot) == 112, "ctypes mirror: engine/_lib.py TgisSamplingParams");
 static_assert(sizeof(tgis_sampling_params) == 120, "ctypes mirror: engine/_lib.py TgisSamplingParams");
-static_assert(sizeof(tgis_config) == 304, "ctypes mirror: engine/_lib.py TgisConfig");
+static_assert(sizeof(tgis_config) == 336, "ctypes mirror: engine/_lib.py TgisConfig");
 int tgis_abi_version(void) { return TGIS_ABI_VERSION; }
 
-int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
-  if (!cfg || !out) return fail("null argument");
+int tgis_config_check(const tgis_config* cfg) {
+  if (!cfg) return fail("null argument");
   if (cfg->abi_version != TGIS_ABI_VERSION) return fail("ABI version mismatch");
   if (cfg->arch != TGIS_ARCH_LLAMA && cfg->arch != TGIS_ARCH_OPT && cfg->arch != TGIS_ARCH_GPT_BIGCODE)
     return fail("unknown arch");
@@ -2279,6 +2298,42 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
   } else if (cfg->head_dim != HEAD_DIM) {
     return fail("head_dim must be 128, 96 or 64");
   }
+  const int tpv = cfg->tp_size > 1 ? cfg->tp_size : 1;
+  // the Llama stack's model variants (0 in every field below is the Llama stack), before the shape checks: a variant
+  // that cannot run under tensor parallelism is refused as such, whatever tp_size divides
+  const bool opt = cfg->arch != TGIS_ARCH_LLAMA;
+  const float emb = cfg->embedding_multiplier, res = cfg->residual_multiplier, attn = cfg->attention_multiplier,
+              logit = cfg->logit_scale;
+  auto ok = [](float v) { return std::isfinite(v) && v >= 0.f; };
+  if (!ok(emb) || !ok(res) || !ok(attn) || !ok(logit))
+    return fail("model scalars must be finite and non-negative (0: the Llama default, 1 or 1/sqrt(head_dim))");
+  auto one = [](float v) { return v == 0.f || v == 1.f; };
+  const bool granite = !one(emb) || !one(res) || attn != 0.f || !one(logit);
+  if (opt && granite) return fail("model scalars (Granite) apply to the Llama layer stack only, not OPT");
+  if (cfg->head_dim != HEAD_DIM && granite)
+    return fail("model scalars (Granite) need head_dim 128: Granite with " + std::to_string(cfg->head_dim) +
+                "-dim heads is not supported yet");
+  // the tensor-parallel exchange kernels (ar_add_rmsnorm / ar2_add_rmsnorm) and the NCCL path's norm do not implement
+  // the residual multiplier
+  if (tpv > 1 && !one(res))
+    return fail("Granite (residual_multiplier != 1) is not supported with tensor parallelism (tp_size must be 1)");
+  if (opt && cfg->rope_table_from_host) return fail("OPT has learned positions, no rotary table");
+  if (cfg->qk_norm) {
+    if (opt) return fail("q/k norm (Qwen3) applies to the Llama layer stack only, not OPT");
+    if (cfg->head_dim != HEAD_DIM) return fail("q/k norm (Qwen3) needs head_dim 128");
+    if (tpv > 1) return fail("q/k norm (Qwen3) is supported on a single GPU only (tp_size must be 1)");
+  }
+  if (cfg->qkv_bias) {
+    if (opt) return fail("qkv bias (Qwen2) applies to the Llama layer stack only: OPT has its own bias path");
+    if (tpv > 1) return fail("qkv bias (Qwen2) is supported on a single GPU only (tp_size must be 1)");
+    if (cfg->qk_norm) return fail("qkv bias (Qwen2) and q/k norm (Qwen3) cannot be combined");
+    if (cfg->head_dim != HEAD_DIM && cfg->head_dim != 64) return fail("qkv bias (Qwen2) needs head_dim 128 or 64");
+  }
+  if (cfg->sliding_window < 0) return fail("sliding window must be >= 0 (0 = attend to the whole context)");
+  if (cfg->sliding_window > 0 && opt)
+    return fail("sliding-window attention applies to the Llama layer stack only, not OPT");
+  if (cfg->sliding_window > 0 && tpv > 1)
+    return fail("sliding-window attention is supported on a single GPU only (tp_size must be 1)");
   if (cfg->n_kv_heads <= 0 || cfg->n_q_heads % cfg->n_kv_heads != 0) return fail("n_q_heads must be a multiple of n_kv_heads");
   const int G = cfg->n_q_heads / cfg->n_kv_heads;
   // decode attention is instantiated for every group of 1..8 at 128-dim heads and for all but 3 at 64-dim heads (the
@@ -2294,11 +2349,10 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
   if (cfg->hidden % 64 || cfg->ffn % 64) return fail("hidden/ffn must be multiples of 64");
   if (cfg->vocab < 1) return fail("vocab must be positive");
   if (cfg->hidden > 8192) return fail("hidden > 8192 unsupported");
-  const int tpv = cfg->tp_size > 1 ? cfg->tp_size : 1;
   if (tpv > 16 || cfg->tp_rank < 0 || cfg->tp_rank >= tpv) return fail("bad tp_size / tp_rank");
   // (a single GPU takes any vocabulary: its lm_head is padded to a multiple of 8 rows)
   if (cfg->n_kv_heads % tpv || cfg->ffn % (64 * tpv) || (tpv > 1 && cfg->vocab % (8 * tpv)))
-    return fail("n_kv_heads, ffn/64 and vocab/8 must be divisible by tp_size");
+    return fail("tp_size does not divide n_kv_heads, ffn/64 and vocab/8");
   if (cfg->max_batched_tokens < 16 || cfg->max_num_seqs < 1 || cfg->max_model_len < 2) return fail("bad limits");
   if (cfg->max_loras < 0 || cfg->max_loras > 64) return fail("max_loras must be in [0, 64]");
   if (cfg->max_loras > 0) {
@@ -2306,6 +2360,12 @@ int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
     if (cfg->max_lora_rank < 8 || cfg->max_lora_rank > 64 || cfg->max_lora_rank % 8)
       return fail("max_lora_rank must be a multiple of 8 in [8, 64]");
   }
+  return 0;
+}
+
+int tgis_engine_create(const tgis_config* cfg, tgis_engine** out) {
+  if (!cfg || !out) return fail("null argument");
+  if (int rc = tgis_config_check(cfg)) return rc;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail("no CUDA device: the TGIS engine has no CPU fallback");
@@ -2327,108 +2387,6 @@ int tgis_engine_load_weight(tgis_engine* e, const char* name, const void* ptr, i
   if (dtype != 0) return fail("only bf16 (dtype 0) weights are supported");
   if (e->started) return fail("engine already started");
   return e->load_weight(name, ptr, rows, cols);
-}
-
-int tgis_engine_set_model_scalars(tgis_engine* e, float embedding_multiplier, float residual_multiplier,
-                                  float attention_multiplier, float logit_scale) {
-  if (!e) return fail("null engine");
-  if (e->started) return fail("model scalars must be set before tgis_engine_start");
-  auto ok = [](float v) { return std::isfinite(v) && v > 0.f; };
-  if (!ok(embedding_multiplier) || !ok(residual_multiplier) || !ok(logit_scale) ||
-      !(std::isfinite(attention_multiplier) && attention_multiplier >= 0.f))
-    return fail("model scalars must be finite and positive (attention_multiplier: 0 = 1/sqrt(head_dim))");
-  const bool llama = embedding_multiplier == 1.f && residual_multiplier == 1.f && attention_multiplier == 0.f &&
-                     logit_scale == 1.f;
-  if (e->opt && !llama) return fail("model scalars (Granite) apply to the Llama layer stack only, not OPT");
-  if (e->kv_head_dim != HEAD_DIM && !llama)
-    return fail("model scalars (Granite) need head_dim 128: Granite with " + std::to_string(e->kv_head_dim) +
-                "-dim heads is not supported yet");
-  // the tensor-parallel exchange kernels (ar_add_rmsnorm / ar2_add_rmsnorm) and the NCCL path's norm do not implement
-  // the residual multiplier
-  if (e->tp > 1 && residual_multiplier != 1.f)
-    return fail("Granite (residual_multiplier != 1) is not supported with tensor parallelism (tp_size must be 1)");
-  e->emb_mult = embedding_multiplier;
-  e->res_mult = residual_multiplier;
-  e->logit_scale = logit_scale;
-  e->attn_scale = attention_multiplier > 0.f ? attention_multiplier : 1.0f / std::sqrt((float)e->model_head_dim);
-  return 0;
-}
-
-int tgis_engine_require_rope_table(tgis_engine* e) {
-  if (!e) return fail("null engine");
-  if (e->started) return fail("the rotary table requirement must be set before tgis_engine_start");
-  if (e->opt) return fail("OPT has learned positions, no rotary table");
-  e->rope_table_required = true;
-  return 0;
-}
-
-int tgis_engine_set_qk_norm(tgis_engine* e, int32_t on) {
-  if (!e) return fail("null engine");
-  if (e->started) return fail("the q/k norm must be set before tgis_engine_start");
-  if (!on) {
-    if (e->qk_norm_w.p) cudaFree(e->qk_norm_w.p);
-    e->qk_norm_w.p = nullptr;
-    e->qk_norm_loaded.clear();
-    return 0;
-  }
-  if (e->opt) return fail("q/k norm (Qwen3) applies to the Llama layer stack only, not OPT");
-  if (e->kv_head_dim != HEAD_DIM) return fail("q/k norm (Qwen3) needs head_dim 128");
-  if (e->tp > 1) return fail("q/k norm (Qwen3) is supported on a single GPU only (tp_size must be 1)");
-  if (e->qkv_bias_w.p) return fail("qkv bias (Qwen2) and q/k norm (Qwen3) cannot be combined");
-  if (e->qk_norm_w.p) return 0;
-  try {
-    CK(cudaSetDevice(e->cfg.device));
-    e->qk_norm_w.alloc((size_t)2 * e->cfg.n_layers * HEAD_DIM);
-  } catch (const std::exception& ex) {
-    return fail(ex.what());
-  }
-  e->qk_norm_loaded.assign(e->cfg.n_layers, 0);
-  return 0;
-}
-
-int tgis_engine_set_qkv_bias(tgis_engine* e, int32_t on) {
-  if (!e) return fail("null engine");
-  if (e->started) return fail("the qkv bias must be set before tgis_engine_start");
-  if (!on) {
-    if (e->qkv_bias_w.p) cudaFree(e->qkv_bias_w.p);
-    e->qkv_bias_w.p = nullptr;
-    e->qkv_bias_loaded.clear();
-    return 0;  // (y32 stays: it is scratch)
-  }
-  if (e->opt) return fail("qkv bias (Qwen2) applies to the Llama layer stack only: OPT has its own bias path");
-  if (e->tp > 1) return fail("qkv bias (Qwen2) is supported on a single GPU only (tp_size must be 1)");
-  if (e->qk_norm_w.p) return fail("qkv bias (Qwen2) and q/k norm (Qwen3) cannot be combined");
-  if (e->kv_head_dim != HEAD_DIM && e->kv_head_dim != 64) return fail("qkv bias (Qwen2) needs head_dim 128 or 64");
-  if (e->qkv_bias_w.p) return 0;
-  try {
-    CK(cudaSetDevice(e->cfg.device));
-    if (!e->y32.p) e->y32.alloc((size_t)std::max(e->T_max, 256) * e->qkv_dim);  // the activations' T_alloc rows
-    e->qkv_bias_loaded.assign(e->cfg.n_layers, 0);
-    e->qkv_bias_w.alloc((size_t)e->cfg.n_layers * e->qkv_dim);
-  } catch (const std::exception& ex) {
-    e->qkv_bias_loaded.clear();
-    return fail(ex.what());
-  }
-  return 0;
-}
-
-int tgis_engine_set_sliding_window(tgis_engine* e, int32_t window) {
-  if (!e) return fail("null engine");
-  if (e->started) return fail("the sliding window must be set before tgis_engine_start");
-  if (window < 0) return fail("sliding window must be >= 0 (0 = attend to the whole context)");
-  if (window > 0 && e->opt) return fail("sliding-window attention applies to the Llama layer stack only, not OPT");
-  if (window > 0 && e->tp > 1)
-    return fail("sliding-window attention is supported on a single GPU only (tp_size must be 1)");
-  e->attn_window = window;
-  return 0;
-}
-
-int tgis_engine_set_prefix_caching(tgis_engine* e, int32_t on) {
-  if (!e) return fail("null engine");
-  if (e->started) return fail("prefix caching must be set before tgis_engine_start");
-  e->prefix_caching = on != 0;
-  e->pcb.assign(e->prefix_caching ? e->num_blocks : 0, tgis_engine::PcBlock{});
-  return 0;
 }
 
 int tgis_engine_prefix_cache_stats(tgis_engine* e, int64_t* queried_tokens, int64_t* hit_tokens, int32_t* cached_blocks) {

@@ -10,7 +10,7 @@ import ctypes as C
 import os
 from pathlib import Path
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 ARCH_LLAMA, ARCH_OPT, ARCH_GPT_BIGCODE = 0, 1, 2
 MAX_REQUEST_ID = 96
 MAX_TOPN = 12
@@ -28,7 +28,10 @@ class TgisConfig(C.Structure):
         ("gpu_mem_fraction", C.c_float), ("device", C.c_int32), ("tp_size", C.c_int32), ("tp_rank", C.c_int32),
         ("use_cuda_graphs", C.c_int32), ("debug_gemm_ref", C.c_int32), ("seed", C.c_uint64),
         ("nccl_id", C.c_uint8 * 128), ("shm_name", C.c_char * 64),
-        ("max_loras", C.c_int32), ("max_lora_rank", C.c_int32), ("arch", C.c_int32), ("reserved0", C.c_int32),
+        ("max_loras", C.c_int32), ("max_lora_rank", C.c_int32), ("arch", C.c_int32),
+        ("embedding_multiplier", C.c_float), ("residual_multiplier", C.c_float), ("attention_multiplier", C.c_float),
+        ("logit_scale", C.c_float), ("qk_norm", C.c_int32), ("qkv_bias", C.c_int32), ("sliding_window", C.c_int32),
+        ("rope_table_from_host", C.c_int32), ("enable_prefix_caching", C.c_int32),
     ]
 
 
@@ -69,8 +72,8 @@ class TgisStatus(C.Structure):
 
 # Every symbol include/tgis_engine.h and include/tgis_kernels.h declare (tests/test_abi_cpu.py checks the export list)
 ENGINE_SYMBOLS = [
-    "tgis_last_error", "tgis_abi_version", "tgis_engine_create", "tgis_engine_load_weight", "tgis_engine_set_model_scalars",
-    "tgis_engine_require_rope_table", "tgis_engine_set_qk_norm", "tgis_engine_set_qkv_bias", "tgis_engine_set_sliding_window", "tgis_engine_set_prefix_caching", "tgis_engine_prefix_cache_stats", "tgis_engine_start",
+    "tgis_last_error", "tgis_abi_version", "tgis_config_check", "tgis_engine_create", "tgis_engine_load_weight",
+    "tgis_engine_prefix_cache_stats", "tgis_engine_start",
     "tgis_engine_add_request", "tgis_engine_abort", "tgis_engine_set_mask_provider", "tgis_engine_load_adapter_weight", "tgis_engine_clear_adapter", "tgis_engine_poll", "tgis_engine_status",
     "tgis_engine_max_model_len", "tgis_engine_set_profiling", "tgis_nccl_unique_id", "tgis_engine_worker_run", "tgis_engine_shutdown", "tgis_engine_destroy", "tgis_engine_run_until_idle",
 ]
@@ -114,14 +117,9 @@ def load_library() -> C.CDLL:
     vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
     lib.tgis_last_error.restype = C.c_char_p
     lib.tgis_k_last_error.restype = C.c_char_p
+    lib.tgis_config_check.argtypes = [C.POINTER(TgisConfig)]
     lib.tgis_engine_create.argtypes = [C.POINTER(TgisConfig), C.POINTER(vp)]
     lib.tgis_engine_load_weight.argtypes = [vp, C.c_char_p, vp, i64, i64, i32]
-    lib.tgis_engine_set_model_scalars.argtypes = [vp, f32, f32, f32, f32]
-    lib.tgis_engine_require_rope_table.argtypes = [vp]
-    lib.tgis_engine_set_qk_norm.argtypes = [vp, i32]
-    lib.tgis_engine_set_qkv_bias.argtypes = [vp, i32]
-    lib.tgis_engine_set_sliding_window.argtypes = [vp, i32]
-    lib.tgis_engine_set_prefix_caching.argtypes = [vp, i32]
     lib.tgis_engine_prefix_cache_stats.argtypes = [vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i32)]
     lib.tgis_engine_start.argtypes = [vp]
     lib.tgis_engine_add_request.argtypes = [vp, C.c_char_p, C.POINTER(i32), i32, C.POINTER(TgisSamplingParams)]

@@ -20,19 +20,19 @@ class ModelConfig:
     rms_eps carries the LayerNorm epsilon, rope_theta unused) -- include/tgis_engine.h TGIS_ARCH_*.
 
     Granite (GraniteForCausalLM) is arch "llama" with the four scalars of its config.json set; their defaults are the
-    Llama stack (tgis_engine_set_model_scalars).
+    Llama stack (tgis_config.embedding_multiplier ...).
 
     arch "llama" takes head_dim 128 or 64 (Llama-3.2-1B; single GPU, no LoRA slots, no Granite scalars), and the
     rope_type "llama3" frequency scaling of Llama-3.1 / 3.2 (rope_scaling_factor > 1; loader.rope_cos_sin).
 
     Qwen3 (Qwen3ForCausalLM) is arch "llama" with qk_norm set: an RMSNorm over each q and k head before RoPE, with the
-    per-layer weights self_attn.q_norm / k_norm (tgis_engine_set_qk_norm; head_dim 128, single GPU).
+    per-layer weights self_attn.q_norm / k_norm (tgis_config.qk_norm; head_dim 128, single GPU).
 
     Mistral (MistralForCausalLM) is arch "llama" with sliding_window set: every layer's query at position p attends to
-    the keys p - sliding_window < k <= p (tgis_engine_set_sliding_window; single GPU).
+    the keys p - sliding_window < k <= p (tgis_config.sliding_window; single GPU).
 
     Qwen2 / Qwen2.5 (Qwen2ForCausalLM) is arch "llama" with qkv_bias set: a bias on the q, k and v projections, added to
-    the fp32 accumulators before the one rounding to bf16 (tgis_engine_set_qkv_bias; head_dim 128 or 64, single GPU).
+    the fp32 accumulators before the one rounding to bf16 (tgis_config.qkv_bias; head_dim 128 or 64, single GPU).
 
     Phi-3 / Phi-3.5 / Phi-4 (Phi3ForCausalLM) is arch "llama", with head_dim 96 for Phi-3-mini / Phi-3.5-mini (single
     GPU, no LoRA slots), LongRoPE for the 128k variants (rope_long_factor / rope_short_factor) and the model-wide
@@ -254,6 +254,48 @@ def make_sampling_params(*, greedy: bool = True, temperature: float = 1.0, top_k
     return sp
 
 
+def engine_config(model: ModelConfig, *, max_num_seqs: int = 64, max_batched_tokens: int = 2048,
+                  kv_cache_bytes: int = 0, gpu_mem_fraction: float = 0.85, device: int = 0, seed: int = 0,
+                  debug_gemm_ref: bool = False, use_cuda_graphs: bool | None = None, tp_size: int = 1, tp_rank: int = 0,
+                  nccl_id: bytes | None = None, shm_name: str = "", max_loras: int = 0, max_lora_rank: int = 16,
+                  enable_prefix_caching: bool = False) -> TgisConfig:
+    """The engine's whole configuration: the model plus NativeEngine's runtime options.  config_error() says whether the
+    library can serve it."""
+    if model.arch not in ("llama", "opt", "gpt_bigcode"):
+        raise EngineError(f"unknown architecture {model.arch!r}")
+    if use_cuda_graphs is None:   # default on; TGIS_CUDA_GRAPHS=0 turns decode-step graph replay off
+        import os
+
+        use_cuda_graphs = os.environ.get("TGIS_CUDA_GRAPHS", "1") != "0"
+    cfg = TgisConfig()
+    cfg.abi_version = _lib.ABI_VERSION
+    cfg.n_layers, cfg.hidden, cfg.n_q_heads, cfg.n_kv_heads = model.n_layers, model.hidden, model.n_q_heads, model.n_kv_heads
+    cfg.head_dim, cfg.ffn, cfg.vocab = model.head_dim, model.ffn, model.vocab
+    cfg.rope_theta, cfg.rms_eps, cfg.max_model_len = model.rope_theta, model.rms_eps, model.max_model_len
+    cfg.max_num_seqs, cfg.max_batched_tokens = max_num_seqs, max_batched_tokens
+    cfg.kv_cache_bytes, cfg.gpu_mem_fraction = kv_cache_bytes, gpu_mem_fraction
+    cfg.device, cfg.tp_size, cfg.tp_rank = device, tp_size, tp_rank
+    if nccl_id is not None:
+        cfg.nccl_id[:] = nccl_id
+    cfg.shm_name = shm_name.encode()
+    cfg.use_cuda_graphs, cfg.debug_gemm_ref, cfg.seed = int(use_cuda_graphs), 1 if debug_gemm_ref else 0, seed
+    cfg.max_loras, cfg.max_lora_rank = int(max_loras), int(max_lora_rank) if max_loras else 0
+    cfg.arch = {"opt": _lib.ARCH_OPT, "gpt_bigcode": _lib.ARCH_GPT_BIGCODE}.get(model.arch, _lib.ARCH_LLAMA)
+    cfg.embedding_multiplier, cfg.residual_multiplier = model.embedding_multiplier, model.residual_multiplier
+    cfg.attention_multiplier, cfg.logit_scale = model.attention_multiplier, 1.0 / model.logits_scaling
+    cfg.qk_norm, cfg.qkv_bias, cfg.sliding_window = int(model.qk_norm), int(model.qkv_bias), int(model.sliding_window or 0)
+    # the engine's built-in rotary table is the unscaled one: a scaled model's start needs the host's table
+    cfg.rope_table_from_host = int(model.arch == "llama" and model.rope_scaled)
+    cfg.enable_prefix_caching = int(enable_prefix_caching)
+    return cfg
+
+
+def config_error(cfg: TgisConfig) -> str | None:
+    """The library's reason for refusing cfg (tgis_config_check), or None when it can serve it.  Touches no GPU."""
+    lib = _lib.load_library()
+    return _lib.last_error(lib) if lib.tgis_config_check(C.byref(cfg)) != 0 else None
+
+
 class NativeEngine:
     """Owns one `tgis_engine*`."""
 
@@ -264,89 +306,25 @@ class NativeEngine:
                  enable_prefix_caching: bool = False):
         self.lib = _lib.load_library()
         self.model = model
-        if use_cuda_graphs is None:   # default on; TGIS_CUDA_GRAPHS=0 turns decode-step graph replay off
-            import os
-
-            use_cuda_graphs = os.environ.get("TGIS_CUDA_GRAPHS", "1") != "0"
-        cfg = TgisConfig()
-        cfg.abi_version = _lib.ABI_VERSION
-        cfg.n_layers, cfg.hidden, cfg.n_q_heads, cfg.n_kv_heads = model.n_layers, model.hidden, model.n_q_heads, model.n_kv_heads
-        cfg.head_dim, cfg.ffn, cfg.vocab = model.head_dim, model.ffn, model.vocab
-        cfg.rope_theta, cfg.rms_eps, cfg.max_model_len = model.rope_theta, model.rms_eps, model.max_model_len
-        cfg.max_num_seqs, cfg.max_batched_tokens = max_num_seqs, max_batched_tokens
-        cfg.kv_cache_bytes, cfg.gpu_mem_fraction = kv_cache_bytes, gpu_mem_fraction
-        cfg.device, cfg.tp_size, cfg.tp_rank = device, tp_size, tp_rank
         if tp_size > 1:
             import torch  # noqa: F401  (load torch's NCCL before the engine dlopens libnccl.so.2)
 
             if nccl_id is None or len(nccl_id) != 128:
                 raise EngineError("tensor parallelism needs the 128-byte NCCL unique id of rank 0")
-            C.memmove(cfg.nccl_id, nccl_id, 128)
-            cfg.shm_name = shm_name.encode()
-        cfg.use_cuda_graphs, cfg.debug_gemm_ref, cfg.seed = int(use_cuda_graphs), 1 if debug_gemm_ref else 0, seed
-        cfg.max_loras, cfg.max_lora_rank = int(max_loras), int(max_lora_rank) if max_loras else 0
-        if model.residual_multiplier != 1.0 and tp_size > 1:
-            raise EngineError("Granite (residual_multiplier != 1) is not supported with tensor parallelism: the "
-                              "row-parallel exchange kernels do not implement the multiplier (use tensor_parallel_size 1)")
-        if model.qk_norm and tp_size > 1:
-            raise EngineError("Qwen3 (qk_norm) is not supported with tensor parallelism: the q/k norm is implemented on a "
-                              "single GPU only (use tensor_parallel_size 1)")
-        if model.sliding_window and tp_size > 1:
-            raise EngineError("sliding-window attention (Mistral) is not supported with tensor parallelism: it is "
-                              "implemented on a single GPU only (use tensor_parallel_size 1)")
-        if model.fused_projections and tp_size > 1:
-            raise EngineError("Phi-3 is not supported with tensor parallelism: it is implemented on a single GPU only "
-                              "(use tensor_parallel_size 1)")
-        if model.qkv_bias and tp_size > 1:
-            raise EngineError("Qwen2 (qkv_bias) is not supported with tensor parallelism: the qkv bias is implemented on a "
-                              "single GPU only (use tensor_parallel_size 1)")
-        if model.arch == "gpt_bigcode" and tp_size > 1:
-            raise EngineError("GPTBigCode is not supported with tensor parallelism: it is implemented on a single GPU only "
-                              "(use tensor_parallel_size 1)")
-        if model.arch == "gpt_bigcode" and max_loras:
-            raise EngineError("GPTBigCode is not supported with LoRA adapters (--enable-lora)")
-        if model.arch not in ("llama", "opt", "gpt_bigcode"):
-            raise EngineError(f"unknown architecture {model.arch!r}")
-        if model.arch == "llama" and model.head_dim != 128 and model.is_granite:
-            raise EngineError(f"Granite with head_dim {model.head_dim} is not supported yet (Granite needs head_dim 128)")
-        cfg.arch = {"opt": _lib.ARCH_OPT, "gpt_bigcode": _lib.ARCH_GPT_BIGCODE}.get(model.arch, _lib.ARCH_LLAMA)
+        cfg = engine_config(model, max_num_seqs=max_num_seqs, max_batched_tokens=max_batched_tokens,
+                            kv_cache_bytes=kv_cache_bytes, gpu_mem_fraction=gpu_mem_fraction, device=device, seed=seed,
+                            debug_gemm_ref=debug_gemm_ref, use_cuda_graphs=use_cuda_graphs, tp_size=tp_size,
+                            tp_rank=tp_rank, nccl_id=nccl_id, shm_name=shm_name, max_loras=max_loras,
+                            max_lora_rank=max_lora_rank, enable_prefix_caching=enable_prefix_caching)
         self.max_loras, self.max_lora_rank = int(max_loras), int(max_lora_rank)
+        self.enable_prefix_caching = bool(enable_prefix_caching)
         self._h = C.c_void_p()
         if self.lib.tgis_engine_create(C.byref(cfg), C.byref(self._h)) != 0:
             raise EngineError(f"tgis_engine_create failed: {_lib.last_error(self.lib)}")
-        if model.is_granite and self.lib.tgis_engine_set_model_scalars(
-                self._h, model.embedding_multiplier, model.residual_multiplier, model.attention_multiplier,
-                1.0 / model.logits_scaling) != 0:
-            msg = _lib.last_error(self.lib)
-            self.close()
-            raise EngineError(f"tgis_engine_set_model_scalars failed: {msg}")
-        if model.arch == "llama" and model.rope_scaled:
-            # the engine's built-in rotary table is the unscaled one: mark the table as required (start fails without it)
-            # and load the scaled one here, so that every way of building an engine gets it
-            if self.lib.tgis_engine_require_rope_table(self._h) != 0:
-                msg = _lib.last_error(self.lib)
-                self.close()
-                raise EngineError(f"tgis_engine_require_rope_table failed: {msg}")
+        if cfg.rope_table_from_host:   # loaded here, so that every way of building an engine gets it
             from .rope import rope_cos_sin
 
             self.load_weight("tgis.rope_cos_sin", rope_cos_sin(model))
-        if model.qk_norm and self.lib.tgis_engine_set_qk_norm(self._h, 1) != 0:
-            msg = _lib.last_error(self.lib)
-            self.close()
-            raise EngineError(f"tgis_engine_set_qk_norm failed: {msg}")
-        if model.qkv_bias and self.lib.tgis_engine_set_qkv_bias(self._h, 1) != 0:
-            msg = _lib.last_error(self.lib)
-            self.close()
-            raise EngineError(f"tgis_engine_set_qkv_bias failed: {msg}")
-        if model.sliding_window and self.lib.tgis_engine_set_sliding_window(self._h, int(model.sliding_window)) != 0:
-            msg = _lib.last_error(self.lib)
-            self.close()
-            raise EngineError(f"tgis_engine_set_sliding_window failed: {msg}")
-        self.enable_prefix_caching = bool(enable_prefix_caching)
-        if self.enable_prefix_caching and self.lib.tgis_engine_set_prefix_caching(self._h, 1) != 0:
-            msg = _lib.last_error(self.lib)
-            self.close()
-            raise EngineError(f"tgis_engine_set_prefix_caching failed: {msg}")
         self._poll_buf = (TgisStepOutput * 512)()
 
     # -- weights ------------------------------------------------------------------------------------------------

@@ -12,7 +12,7 @@ import logging
 from pathlib import Path
 
 from .async_engine import AsyncTGISEngine
-from .core import PRESETS, ModelConfig, NativeEngine
+from .core import PRESETS, ModelConfig, NativeEngine, config_error, engine_config
 from .rope import rope_cos_sin, rope_inv_freq  # noqa: F401  (the table every Llama engine is given: rope.py)
 from .tokenizer import load_tokenizer
 
@@ -489,12 +489,17 @@ def _resolve_model(args):
     raise ValueError(f"model path {args.model} does not exist (no network access: hub ids cannot be resolved)")
 
 
+def _engine_options(args, device: int, **tp_kw) -> dict:
+    """NativeEngine's keyword arguments (engine_config's options) from the server's arguments"""
+    return dict(max_num_seqs=args.max_num_seqs, max_batched_tokens=args.max_num_batched_tokens,
+                gpu_mem_fraction=args.gpu_memory_utilization, device=device, seed=args.seed,
+                max_loras=args.max_loras if getattr(args, "enable_lora", False) else 0,
+                max_lora_rank=getattr(args, "max_lora_rank", 16),
+                enable_prefix_caching=bool(getattr(args, "enable_prefix_caching", False)), **tp_kw)
+
+
 def _make_native_engine(args, mc: ModelConfig, path, device: int, **tp_kw) -> NativeEngine:
-    eng = NativeEngine(mc, max_num_seqs=args.max_num_seqs, max_batched_tokens=args.max_num_batched_tokens,
-                       gpu_mem_fraction=args.gpu_memory_utilization, device=device, seed=args.seed,
-                       max_loras=args.max_loras if getattr(args, "enable_lora", False) else 0,
-                       max_lora_rank=getattr(args, "max_lora_rank", 16),
-                       enable_prefix_caching=bool(getattr(args, "enable_prefix_caching", False)), **tp_kw)
+    eng = NativeEngine(mc, **_engine_options(args, device, **tp_kw))
     if path is not None:
         load_safetensors_dir(eng, path)      # full tensors: a tensor-parallel engine keeps its rank's shard
     else:
@@ -524,26 +529,19 @@ def build_engine(args) -> AsyncTGISEngine:
     tp = args.tensor_parallel_size or 1
     mc, path = _resolve_model(args)
     tp_kw = {}
-    if tp > 1 and mc.qk_norm:
-        raise ValueError(f"Qwen3 (per-head q/k norm) is supported on a single GPU only: tensor_parallel_size {tp}")
-    if tp > 1 and mc.sliding_window:
-        raise ValueError(f"Mistral (sliding-window attention) is supported on a single GPU only: tensor_parallel_size {tp}")
+    # Phi-3's fused projections are split on the host into full tensors, which no rank shards
     if tp > 1 and mc.fused_projections:
         raise ValueError(f"Phi-3 is supported on a single GPU only: tensor_parallel_size {tp}")
-    if tp > 1 and mc.qkv_bias:
-        raise ValueError(f"Qwen2 (qkv bias) is supported on a single GPU only: tensor_parallel_size {tp}")
-    if tp > 1 and mc.arch == "gpt_bigcode":
-        raise ValueError(f"GPTBigCode is supported on a single GPU only: tensor_parallel_size {tp}")
-    if mc.arch == "gpt_bigcode" and getattr(args, "enable_lora", False):
-        raise ValueError("GPTBigCode is not supported with LoRA adapters: drop --enable-lora")
+    # every other refusal is the library's, made here before any rank is spawned or device touched
+    err = config_error(engine_config(mc, **_engine_options(args, args.device, tp_size=tp)))
+    if err:
+        raise ValueError(err)
     if tp > 1:
         import multiprocessing as mp
         import os
 
         import torch  # noqa: F401
 
-        if mc.n_kv_heads % tp or mc.ffn % tp or mc.vocab % tp:
-            raise ValueError(f"tensor_parallel_size {tp} does not divide kv heads / ffn / vocab of {mc}")
         nccl_id = NativeEngine.nccl_unique_id()
         shm_name = f"/tgis_tp_{os.getpid()}"
         ctx = mp.get_context("spawn")
