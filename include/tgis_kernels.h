@@ -213,6 +213,13 @@ int tgis_k_sampler_scaled(const void* logits_dev, int32_t logits_bf16, int32_t l
  * y[t, col0 + n] = bf16(y + bf16(B_s[n, :] . bf16(A_s x[t]))) */
 int tgis_k_lora(const void* x_dev, int32_t ldx, const int32_t* tok_slot_dev, const void* a_dev, const void* b_dev, int32_t K,
                 int32_t N, int32_t Rm, int32_t col0, void* y_dev, int32_t ldy, int32_t T);
+/* a group of n_mods (<= 3) modules over the same x, as the engine's qkv group: module m has a_devs[m], b_devs[m] and
+   dims[5 m ..] = {K, N, Rm, col0, v_off}; its rank vector sits at v_off within the v_ld floats per token of the shrink
+   buffer.  tok_row_dev (nullable): the rows in the order the kernels walk them in 8-token tiles, as the engine groups
+   them by adapter slot */
+int tgis_k_lora_group(const void* x_dev, int32_t ldx, const int32_t* tok_slot_dev, const int32_t* tok_row_dev, int32_t n_mods,
+                      const void* const* a_devs, const void* const* b_devs, const int32_t* dims, int32_t v_ld, void* y_dev,
+                      int32_t ldy, int32_t T);
 /* same kernels, col0 = 0, timed: iters launches of each, average device microseconds per launch */
 int tgis_k_lora_bench(const void* x_dev, int32_t ldx, const int32_t* tok_slot_dev, const void* a_dev, const void* b_dev,
                       int32_t K, int32_t N, int32_t Rm, void* y_dev, int32_t ldy, int32_t T, int32_t iters,

@@ -42,6 +42,18 @@ def two_layer(name: str):
     return dataclasses.replace(PRESETS[name], n_layers=2)
 
 
+def lora_capable(mc) -> bool:
+    """csrc/engine.cu tgis_config_check: LoRA adapter slots are served by the Llama layer stack with 128-dim heads on one
+    GPU (tests/test_lora_real_dims_cpu.py holds this against the library for every real preset)"""
+    return mc.arch == "llama" and mc.head_dim == 128
+
+
+# the real presets that serve LoRA adapters: tests/test_lora_real_dims_gpu.py runs each with adapters against its
+# family's oracle.  FUSED_ROPE comes first, so LORA_FUSED_ROPE is a prefix as well.
+LORA_REAL_DIMS = [n for n in REAL_DIMS + ["llama3-8b"] if lora_capable(two_layer(n))]
+LORA_FUSED_ROPE = [n for n in LORA_REAL_DIMS if n in FUSED_ROPE]
+
+
 @dataclasses.dataclass
 class Family:
     name: str

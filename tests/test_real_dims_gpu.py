@@ -138,13 +138,23 @@ def _as_tuples(outs):
     return [[(r.new_token, r.logprob, r.rank, tuple(r.topn)) for r in recs] for recs in outs]
 
 
-def check_greedy(ora, prompts, outs, n_new=N_NEW, n_top=3, where=""):
+def _step(ora, work, lora, **kw):
+    """ora.step, with per-sequence adapters when `lora` is given (the GPTBigCode oracle takes none)"""
+    return ora.step(work, **kw) if lora is None else ora.step(work, lora=lora, **kw)
+
+
+def check_greedy(ora, prompts, outs, n_new=N_NEW, n_top=3, where="", lora=None):
     """teacher-forced on the engine's tokens, every sequence stepping together after its own prefill.  Every request
     asks for min_tokens = max_tokens, so the engine never picks EOS: the greedy choice is the argmax over the other
-    tokens, while logprobs and ranks are those of the whole distribution."""
+    tokens, while logprobs and ranks are those of the whole distribution.  lora: per prompt None or the adapter its
+    request ran under (LlamaOracle.step's `lora`); a request under a non-zero adapter may also use the 1 % exception for
+    its logprob and top-n values, at up to 4 ulps."""
     assert [len(r) for r in outs] == [n_new] * len(prompts), where
     seqs = [ora.new_seq() for _ in prompts]
-    logits = torch.cat([ora.step([(s, p)]) for s, p in zip(seqs, prompts)])
+    # (the all-zero adapter adds nothing: its requests keep the plain bars)
+    adapted = [ad is not None and any(bool(b.any()) for _, b in ad.values()) for ad in (lora or [None] * len(prompts))]
+    logits = torch.cat([_step(ora, [(s, p)], None if lora is None else [lora[i]])
+                        for i, (s, p) in enumerate(zip(seqs, prompts))])
     flips = steps = wide = 0
     for j in range(n_new):
         for i, recs in enumerate(outs):
@@ -165,15 +175,23 @@ def check_greedy(ora, prompts, outs, n_new=N_NEW, n_top=3, where=""):
                 flips += 1
             elif margin > RACE * u and abs(float(row[EOS] - row[r.new_token])) > RACE * u:
                 assert r.rank == 1 + int(row[EOS] > row[r.new_token]), (at, "rank", r.rank)
-            assert abs(r.logprob - float(lp[r.new_token])) <= 3 * u, (at, "logprob", r.logprob, float(lp[r.new_token]))
+            err = abs(r.logprob - float(lp[r.new_token]))
+            if adapted[i] and 3 * u < err <= WIDE_RACE * u + u:
+                wide += 1   # an adapted projection adds two bf16 roundings of fp32 sums (rank vector, delta)
+            else:
+                assert err <= 3 * u, (at, "logprob", r.logprob, float(lp[r.new_token]))
             assert len(r.topn) == n_top, at
             floor = float(torch.topk(lp, n_top).values[-1])
             for tid, tlp in r.topn:
-                assert abs(tlp - float(lp[tid])) <= 3 * u, (at, "top-n", tid, tlp, float(lp[tid]))
+                err = abs(tlp - float(lp[tid]))
+                if adapted[i] and 3 * u < err <= WIDE_RACE * u + u:
+                    wide += tid != r.new_token   # (the sampled token's value was counted above)
+                else:
+                    assert err <= 3 * u, (at, "top-n", tid, tlp, float(lp[tid]))
                 assert float(lp[tid]) >= floor - WIDE_RACE * u, (at, "top-n id", tid)
                 wide += float(lp[tid]) < floor - RACE * u
         if j + 1 < n_new:
-            logits = ora.step([(s, [recs[j].new_token]) for s, recs in zip(seqs, outs)])
+            logits = _step(ora, [(s, [recs[j].new_token]) for s, recs in zip(seqs, outs)], lora)
     assert flips <= steps // 10, (where, flips, steps)
     assert wide <= max(1, steps // 100), (where, "2-3 ulp events", wide, steps)
 
@@ -215,14 +233,15 @@ def test_prompt_logprobs_match_the_oracle(stack):
     check_prompt_logprobs(stack.oracle(), p, recs, where=stack.name)
 
 
-def check_prompt_logprobs(ora, p, recs, where=""):
+def check_prompt_logprobs(ora, p, recs, where="", lora=None):
     """tests/test_mistral_gpu.py's prompt-logprob bars at every position: the logprob within 3 ulps of the row's top
-    logit, the rank inside the band of tokens within 3 ulps of it, the top-1 value within 3 ulps"""
+    logit, the rank inside the band of tokens within 3 ulps of it, the top-1 value within 3 ulps.  lora: the adapter
+    the request ran under, or None"""
     prec = sorted([r for r in recs if r.prompt_pos >= 1], key=lambda r: r.prompt_pos)
     assert [r.prompt_pos for r in prec] == list(range(1, len(p)))
     assert [r.token_id for r in prec] == p[1:]
     assert all(len(r.topn) == 3 for r in prec)
-    logits = ora.step([(ora.new_seq(), p)], want_all_logits=True)[:-1]
+    logits = _step(ora, [(ora.new_seq(), p)], None if lora is None else [lora], want_all_logits=True)[:-1]
     lp = torch.log_softmax(logits, -1)
     top = logits.max(-1).values.abs().clamp_min(1e-6)
     u = torch.exp2(torch.floor(torch.log2(top)) - 7)

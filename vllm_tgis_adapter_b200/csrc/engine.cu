@@ -337,7 +337,7 @@ struct tgis_engine {
   uint8_t* h_stage = nullptr;
   DevBuf<uint8_t> d_stage;
   size_t off_tok = 0, off_pos = 0, off_slotmap = 0, off_tokslot = 0, off_seqs = 0, off_decids = 0, off_tileseq = 0,
-         off_tileq0 = 0, off_samplesrc = 0, off_rows = 0, off_epoch = 0, off_bt = 0, off_toklora = 0, stage_bytes = 0;
+         off_tileq0 = 0, off_samplesrc = 0, off_rows = 0, off_epoch = 0, off_bt = 0, off_toklora = 0, off_lorarow = 0, stage_bytes = 0;
 
   // host state
   std::mutex mu;
@@ -629,6 +629,7 @@ struct tgis_engine {
     off_slotmap = place(4 * (size_t)T_max);
     off_tokslot = place(4 * (size_t)T_max);
     off_toklora = place(4 * (size_t)T_max);  // adapter slot of every token (0: base model)
+    off_lorarow = place(4 * (size_t)T_max);  // LoRA steps: the token rows grouped by adapter slot (lora.cu's tile order)
     off_seqs = place(sizeof(AttnSeq) * (size_t)S_max);
     off_decids = place(4 * (size_t)S_max);
     off_tileseq = place(4 * (size_t)tiles_max);
@@ -1320,10 +1321,11 @@ struct tgis_engine {
     // add), so the fused epilogues are switched off for the step and the deltas land between the GEMM and its consumer
     const bool lora = (samp_complex & 4) != 0 && max_loras > 0;
     const int32_t* d_toklora = ds<int32_t>(off_toklora);
+    const int32_t* d_lorarow = ds<int32_t>(off_lorarow);
     const int LR = lora_R, kvd = nkv * kv_head_dim;
     auto lora_apply = [&](const LoraGroup& g, const bf16* x, int ldx, bf16* y, int ldy) {
-      CK(lora_shrink_launch(x, ldx, d_toklora, g, lora_v.p, T, stream));
-      CK(lora_expand_launch(lora_v.p, d_toklora, g, y, ldy, T, stream));
+      CK(lora_shrink_launch(x, ldx, d_toklora, d_lorarow, g, lora_v.p, T, stream));
+      CK(lora_expand_launch(lora_v.p, d_toklora, d_lorarow, g, y, ldy, T, stream));
       n_launches += 2;
     };
     if (lora) ++lora_steps;
@@ -1761,6 +1763,17 @@ struct tgis_engine {
       tileseq[n_tiles] = ctile_seq[i];
       tileq0[n_tiles++] = ctile_q0[i];
     }
+    if (samp_complex & 4) {
+      // LoRA: lora.cu walks the tokens in 8-token tiles in this order -- rows grouped by adapter slot (a counting sort,
+      // stable), so that tokens sharing an adapter share tiles and its A / B rows are read once per tile.  The rows
+      // themselves stay in place: every other kernel of the step sees the same batch as without adapters, and a GEMM's
+      // result for a row can depend on the row's place in the batch (the split tiles of stream-K schedules).
+      int32_t* lorarow = hs<int32_t>(off_lorarow);
+      std::vector<int> first(max_loras + 2, 0);
+      for (int t = 0; t < T; ++t) ++first[toklora[t] + 1];
+      for (int s = 1; s <= max_loras + 1; ++s) first[s] += first[s - 1];
+      for (int t = 0; t < T; ++t) lorarow[first[toklora[t]]++] = t;
+    }
     // ---- ship metadata + run the layer stack (one CUDA graph launch for a pure-decode step when enabled)
     // decode work items: (sequence, DECODE_SPLIT-token split) entries; the copy covers the worst case for this
     // (S, max_splits) so that its size is a function of the CUDA-graph key
@@ -2155,16 +2168,8 @@ struct tgis_engine {
       return false;
     }
 
-    // LoRA: sequences that share an adapter sit next to each other in the step, so that lora.cu's 8-token tiles are
-    // same-adapter tiles (A / B rows read once per tile) instead of falling back to one pass per token.  Every kernel's
-    // result for a token is independent of its neighbours, and post-processing below walks the same order.
-    if (max_loras > 0) {
-      bool any_lora = false;
-      for (const Sched& s : batch) any_lora |= s.r->sp.lora_slot > 0;
-      if (any_lora)
-        std::stable_sort(batch.begin(), batch.end(),
-                         [](const Sched& a, const Sched& b) { return a.r->sp.lora_slot < b.r->sp.lora_slot; });
-    }
+    // (LoRA steps keep this order too: lora.cu groups the tokens by adapter through a row order of its own, see
+    // run_batch, because moving a base-model row to another place in the batch can change its GEMM results)
 
     // ---- run
     run_batch(batch);

@@ -139,10 +139,13 @@ struct LoraGroup {
   int n_mods;
   int v_ld;                // floats per token in the shrink buffer
 };
-cudaError_t lora_shrink_launch(const __nv_bfloat16* x, int ldx, const int32_t* tok_slot, const LoraGroup& g, float* v, int T,
-                               cudaStream_t stream);
-cudaError_t lora_expand_launch(const float* v, const int32_t* tok_slot, const LoraGroup& g, __nv_bfloat16* y, int ldy, int T,
-                               cudaStream_t stream);
+// tok_slot[row]: the adapter slot of each row (0: none); tok_row[p] (nullable: p): the row at position p of the order the
+// kernels walk in 8-token tiles -- the engine lists the rows grouped by slot, so that the tiles are same-adapter tiles
+// while the rows stay where every other kernel of the step has them
+cudaError_t lora_shrink_launch(const __nv_bfloat16* x, int ldx, const int32_t* tok_slot, const int32_t* tok_row,
+                               const LoraGroup& g, float* v, int T, cudaStream_t stream);
+cudaError_t lora_expand_launch(const float* v, const int32_t* tok_slot, const int32_t* tok_row, const LoraGroup& g,
+                               __nv_bfloat16* y, int ldy, int T, cudaStream_t stream);
 // act[t, j] = bf16(silu(gate_up[t, 2j])) * gate_up[t, 2j + 1]  (the interleaved gate_up layout the fused GEMM epilogue reads)
 cudaError_t silu_mul_interleaved_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, int T, int ffn,
                                         cudaStream_t stream);

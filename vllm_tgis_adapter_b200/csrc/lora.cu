@@ -56,6 +56,10 @@ __device__ __forceinline__ float dot8(const F8& a, const F8& b) {
 constexpr int LORA_TT = 8;  // tokens per tile
 constexpr int LORA_MAX_RM = 128;
 
+// the row of y / x that tile position p serves: tok_row lists the step's rows grouped by adapter slot (nullptr: the rows
+// in order).  Shrink sums live at the position, not the row, between the two kernels.
+__device__ __forceinline__ int lora_row(const int32_t* __restrict__ tok_row, int p) { return tok_row ? tok_row[p] : p; }
+
 __device__ __forceinline__ F8 cvt8(const uint4& r) {
   const uint32_t w[4] = {r.x, r.y, r.z, r.w};
   F8 o;
@@ -74,8 +78,8 @@ __device__ __forceinline__ F8 cvt8(const uint4& r) {
 // 16 CTAs re-read the same 64 KB of x).  Partial sums meet in shared memory and are added in warp order: deterministic.
 constexpr int LORA_RPC = 4;
 __global__ void __launch_bounds__(256)
-lora_shrink_kernel(const __nv_bfloat16* __restrict__ x, int ldx, const int32_t* __restrict__ tok_slot, LoraGroup g,
-                   float* __restrict__ v, int T) {
+lora_shrink_kernel(const __nv_bfloat16* __restrict__ x, int ldx, const int32_t* __restrict__ tok_slot,
+                   const int32_t* __restrict__ tok_row, LoraGroup g, float* __restrict__ v, int T) {
   __shared__ float part[8][LORA_RPC][LORA_TT];
   griddep_launch();
   griddep_wait();
@@ -92,7 +96,7 @@ lora_shrink_kernel(const __nv_bfloat16* __restrict__ x, int ldx, const int32_t* 
   bool any = false, uniform = true;
 #pragma unroll
   for (int j = 0; j < LORA_TT; ++j) {
-    const int sj = (j < nt) ? tok_slot[t0 + j] : 0;
+    const int sj = (j < nt) ? tok_slot[lora_row(tok_row, t0 + j)] : 0;
     if (j == 0) slot0 = sj;
     any |= sj > 0;
     uniform &= (j >= nt) || sj == slot0;
@@ -113,7 +117,7 @@ lora_shrink_kernel(const __nv_bfloat16* __restrict__ x, int ldx, const int32_t* 
 #pragma unroll
       for (int q = 0; q < LORA_RPC; ++q) ar[q] = a0[(size_t)q * nvec + kv];
 #pragma unroll
-      for (int j = 0; j < LORA_TT; ++j) xr[j] = xq[(size_t)(t0 + (j < nt ? j : 0)) * ldq + kv];
+      for (int j = 0; j < LORA_TT; ++j) xr[j] = xq[(size_t)lora_row(tok_row, t0 + (j < nt ? j : 0)) * ldq + kv];
 #pragma unroll
       for (int j = 0; j < LORA_TT; ++j) {
         const F8 xf = cvt8(xr[j]);
@@ -124,10 +128,11 @@ lora_shrink_kernel(const __nv_bfloat16* __restrict__ x, int ldx, const int32_t* 
   } else {
 #pragma unroll
     for (int j = 0; j < LORA_TT; ++j) {
-      const int sj = (j < nt) ? tok_slot[t0 + j] : 0;
+      const int row = (j < nt) ? lora_row(tok_row, t0 + j) : 0;
+      const int sj = (j < nt) ? tok_slot[row] : 0;
       if (sj <= 0) continue;
       const uint4* a0 = reinterpret_cast<const uint4*>(md.A + ((size_t)(sj - 1) * md.Rm + r0) * md.K);
-      const uint4* xrow = xq + (size_t)(t0 + j) * ldq;
+      const uint4* xrow = xq + (size_t)row * ldq;
       for (int kv = warp * 32 + lane; kv < nvec; kv += 256) {
         const F8 xf = cvt8(xrow[kv]);
 #pragma unroll
@@ -147,7 +152,7 @@ lora_shrink_kernel(const __nv_bfloat16* __restrict__ x, int ldx, const int32_t* 
   __syncthreads();
   if (threadIdx.x < LORA_RPC * LORA_TT) {
     const int q = threadIdx.x / LORA_TT, j = threadIdx.x % LORA_TT;
-    if (j < nt && tok_slot[t0 + j] > 0) {
+    if (j < nt && tok_slot[lora_row(tok_row, t0 + j)] > 0) {
       float s = 0.f;
 #pragma unroll
       for (int w = 0; w < 8; ++w) s += part[w][q][j];
@@ -178,8 +183,8 @@ __device__ __forceinline__ void st4f(__nv_bfloat16* p, const float (&f)[4]) {
   *reinterpret_cast<uint2*>(p) = r;
 }
 __global__ void __launch_bounds__(256)
-lora_expand_kernel(const float* __restrict__ v, const int32_t* __restrict__ tok_slot, LoraGroup g,
-                   __nv_bfloat16* __restrict__ y, int ldy, int T) {
+lora_expand_kernel(const float* __restrict__ v, const int32_t* __restrict__ tok_slot, const int32_t* __restrict__ tok_row,
+                   LoraGroup g, __nv_bfloat16* __restrict__ y, int ldy, int T) {
   __shared__ __align__(16) float vsT[LORA_MAX_RM][LORA_TT];  // [rank index][token of the tile]
   griddep_launch();
   griddep_wait();
@@ -190,7 +195,7 @@ lora_expand_kernel(const float* __restrict__ v, const int32_t* __restrict__ tok_
   bool any = false, uniform = true;
 #pragma unroll
   for (int j = 0; j < LORA_TT; ++j) {
-    const int sj = (t0 + j < T) ? tok_slot[t0 + j] : 0;
+    const int sj = (t0 + j < T) ? tok_slot[lora_row(tok_row, t0 + j)] : 0;
     if (j == 0) slot0 = sj;
     any |= sj > 0;
     uniform &= (t0 + j >= T) || sj == slot0;
@@ -208,12 +213,12 @@ lora_expand_kernel(const float* __restrict__ v, const int32_t* __restrict__ tok_
     for (int e = 0; e < LORA_EC; ++e) nxt[e] = *reinterpret_cast<const uint4*>(brow + (size_t)e * md.Rm);
 #pragma unroll
     for (int j = 0; j < LORA_TT; ++j)
-      yraw[j] = *reinterpret_cast<const uint2*>(y + (size_t)(t0 + (t0 + j < T ? j : 0)) * ldy + md.col0 + n0);
+      yraw[j] = *reinterpret_cast<const uint2*>(y + (size_t)lora_row(tok_row, t0 + (t0 + j < T ? j : 0)) * ldy + md.col0 + n0);
   }
   // the fp32 shrink sums enter the second product as bf16 (lora_expand_op.py casts the buffer to the weight dtype)
   for (int i = threadIdx.x; i < LORA_TT * md.Rm; i += 256) {
     const int j = i / md.Rm, r = i - j * md.Rm;
-    const bool live = t0 + j < T && tok_slot[t0 + j] > 0;
+    const bool live = t0 + j < T && tok_slot[lora_row(tok_row, t0 + j)] > 0;
     vsT[r][j] = live ? bf16_round(v[(size_t)(t0 + j) * g.v_ld + md.v_off + r]) : 0.f;
   }
   __syncthreads();
@@ -247,7 +252,7 @@ lora_expand_kernel(const float* __restrict__ v, const int32_t* __restrict__ tok_
 #pragma unroll
     for (int j = 0; j < LORA_TT; ++j) {
       if (t0 + j >= T) break;
-      __nv_bfloat16* yp = y + (size_t)(t0 + j) * ldy + md.col0 + n0;
+      __nv_bfloat16* yp = y + (size_t)lora_row(tok_row, t0 + j) * ldy + md.col0 + n0;
       float yv[LORA_EC] = {__uint_as_float(yraw[j].x << 16), __uint_as_float(yraw[j].x & 0xffff0000u),
                            __uint_as_float(yraw[j].y << 16), __uint_as_float(yraw[j].y & 0xffff0000u)};
 #pragma unroll
@@ -256,10 +261,11 @@ lora_expand_kernel(const float* __restrict__ v, const int32_t* __restrict__ tok_
     }
   } else {
     for (int j = 0; j < LORA_TT && t0 + j < T; ++j) {
-      const int sj = tok_slot[t0 + j];
+      const int row = lora_row(tok_row, t0 + j);
+      const int sj = tok_slot[row];
       if (sj <= 0) continue;
       const __nv_bfloat16* brow_j = md.B + ((size_t)(sj - 1) * md.N + n0) * md.Rm;
-      __nv_bfloat16* yp = y + (size_t)(t0 + j) * ldy + md.col0 + n0;
+      __nv_bfloat16* yp = y + (size_t)row * ldy + md.col0 + n0;
       float yv[LORA_EC];
       ld4f(yp, yv);
 #pragma unroll
@@ -318,23 +324,23 @@ static bool lora_group_ok(const LoraGroup& g) {
   return true;
 }
 
-cudaError_t lora_shrink_launch(const __nv_bfloat16* x, int ldx, const int32_t* tok_slot, const LoraGroup& g, float* v, int T,
-                               cudaStream_t stream) {
+cudaError_t lora_shrink_launch(const __nv_bfloat16* x, int ldx, const int32_t* tok_slot, const int32_t* tok_row,
+                               const LoraGroup& g, float* v, int T, cudaStream_t stream) {
   if (T <= 0) return cudaSuccess;
   if (!lora_group_ok(g) || ldx % 8 != 0) return cudaErrorInvalidValue;
   int groups = 0;
   for (int m = 0; m < g.n_mods; ++m) groups += g.mod[m].Rm / LORA_RPC;
-  return launch_k(lora_shrink_kernel, dim3((T + LORA_TT - 1) / LORA_TT, groups), dim3(256), 0, stream, x, ldx, tok_slot, g, v, T);
+  return launch_k(lora_shrink_kernel, dim3((T + LORA_TT - 1) / LORA_TT, groups), dim3(256), 0, stream, x, ldx, tok_slot, tok_row, g, v, T);
 }
 
-cudaError_t lora_expand_launch(const float* v, const int32_t* tok_slot, const LoraGroup& g, __nv_bfloat16* y, int ldy, int T,
-                               cudaStream_t stream) {
+cudaError_t lora_expand_launch(const float* v, const int32_t* tok_slot, const int32_t* tok_row, const LoraGroup& g,
+                               __nv_bfloat16* y, int ldy, int T, cudaStream_t stream) {
   if (T <= 0) return cudaSuccess;
   if (!lora_group_ok(g) || ldy % 8 != 0) return cudaErrorInvalidValue;
   int max_n = 0;
   for (int m = 0; m < g.n_mods; ++m) max_n = g.mod[m].N > max_n ? g.mod[m].N : max_n;
   return launch_k(lora_expand_kernel, dim3((max_n + LORA_ECOLS - 1) / LORA_ECOLS, (T + LORA_TT - 1) / LORA_TT, g.n_mods),
-                  dim3(256), 0, stream, v, tok_slot, g, y, ldy, T);
+                  dim3(256), 0, stream, v, tok_slot, tok_row, g, y, ldy, T);
 }
 
 cudaError_t silu_mul_interleaved_launch(const __nv_bfloat16* gate_up, __nv_bfloat16* act, int T, int ffn,

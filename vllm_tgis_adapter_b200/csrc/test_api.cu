@@ -908,8 +908,31 @@ int tgis_k_lora(const void* x_dev, int32_t ldx, const int32_t* tok_slot_dev, con
   g.n_mods = 1;
   g.v_ld = Rm;
   g.mod[0] = LoraModule{(const __nv_bfloat16*)a_dev, (const __nv_bfloat16*)b_dev, K, N, Rm, col0, 0};
-  KCK(lora_shrink_launch((const __nv_bfloat16*)x_dev, ldx, tok_slot_dev, g, v.p, T, 0));
-  KCK(lora_expand_launch(v.p, tok_slot_dev, g, (__nv_bfloat16*)y_dev, ldy, T, 0));
+  KCK(lora_shrink_launch((const __nv_bfloat16*)x_dev, ldx, tok_slot_dev, nullptr, g, v.p, T, 0));
+  KCK(lora_expand_launch(v.p, tok_slot_dev, nullptr, g, (__nv_bfloat16*)y_dev, ldy, T, 0));
+  KCK(cudaDeviceSynchronize());
+  return 0;
+}
+
+// a group of modules that read the same x, launched as engine.cu launches the qkv group: module m has its A, B and
+// dims[5 m ..] = {K, N, Rm, col0, v_off}; the shrink buffer holds v_ld floats per token; tok_row_dev (nullable): the
+// order the kernels walk the rows in, as the engine passes it
+int tgis_k_lora_group(const void* x_dev, int32_t ldx, const int32_t* tok_slot_dev, const int32_t* tok_row_dev, int32_t n_mods,
+                      const void* const* a_devs, const void* const* b_devs, const int32_t* dims, int32_t v_ld, void* y_dev,
+                      int32_t ldy, int32_t T) {
+  if (n_mods < 1 || n_mods > LORA_GROUP_MAX) return kfail("n_mods must be 1 to LORA_GROUP_MAX");
+  LoraGroup g{};
+  g.n_mods = n_mods;
+  g.v_ld = v_ld;
+  for (int m = 0; m < n_mods; ++m) {
+    const int32_t* d = dims + 5 * m;
+    if (d[4] < 0 || d[4] + d[2] > v_ld) return kfail("a module's shrink rows fall outside v_ld");
+    g.mod[m] = LoraModule{(const __nv_bfloat16*)a_devs[m], (const __nv_bfloat16*)b_devs[m], d[0], d[1], d[2], d[3], d[4]};
+  }
+  Tmp<float> v;
+  KCK(v.alloc((size_t)T * v_ld));
+  KCK(lora_shrink_launch((const __nv_bfloat16*)x_dev, ldx, tok_slot_dev, tok_row_dev, g, v.p, T, 0));
+  KCK(lora_expand_launch(v.p, tok_slot_dev, tok_row_dev, g, (__nv_bfloat16*)y_dev, ldy, T, 0));
   KCK(cudaDeviceSynchronize());
   return 0;
 }
@@ -929,12 +952,12 @@ int tgis_k_lora_bench(const void* x_dev, int32_t ldx, const int32_t* tok_slot_de
   KCK(cudaEventCreate(&e1));
   KCK(cudaEventCreate(&e2));
   if (iters < 1) iters = 1;
-  KCK(lora_shrink_launch((const __nv_bfloat16*)x_dev, ldx, tok_slot_dev, g, v.p, T, 0));
-  KCK(lora_expand_launch(v.p, tok_slot_dev, g, (__nv_bfloat16*)y_dev, ldy, T, 0));
+  KCK(lora_shrink_launch((const __nv_bfloat16*)x_dev, ldx, tok_slot_dev, nullptr, g, v.p, T, 0));
+  KCK(lora_expand_launch(v.p, tok_slot_dev, nullptr, g, (__nv_bfloat16*)y_dev, ldy, T, 0));
   KCK(cudaEventRecord(e0, 0));
-  for (int i = 0; i < iters; ++i) KCK(lora_shrink_launch((const __nv_bfloat16*)x_dev, ldx, tok_slot_dev, g, v.p, T, 0));
+  for (int i = 0; i < iters; ++i) KCK(lora_shrink_launch((const __nv_bfloat16*)x_dev, ldx, tok_slot_dev, nullptr, g, v.p, T, 0));
   KCK(cudaEventRecord(e1, 0));
-  for (int i = 0; i < iters; ++i) KCK(lora_expand_launch(v.p, tok_slot_dev, g, (__nv_bfloat16*)y_dev, ldy, T, 0));
+  for (int i = 0; i < iters; ++i) KCK(lora_expand_launch(v.p, tok_slot_dev, nullptr, g, (__nv_bfloat16*)y_dev, ldy, T, 0));
   KCK(cudaEventRecord(e2, 0));
   KCK(cudaDeviceSynchronize());
   float ms = 0.f;

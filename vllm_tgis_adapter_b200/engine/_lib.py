@@ -80,7 +80,7 @@ ENGINE_SYMBOLS = [
 KERNEL_SYMBOLS = [
     "tgis_k_last_error", "tgis_k_gemm_timeline", "tgis_k_step_timeline_enable", "tgis_k_step_timeline_read", "tgis_k_gemm", "tgis_k_rmsnorm", "tgis_k_rmsnorm_mult", "tgis_k_embed", "tgis_k_opt_layernorm", "tgis_k_opt_bias_act", "tgis_k_opt_embed", "tgis_k_silu_mul", "tgis_k_rope_kv", "tgis_k_gemm_rope", "tgis_k_attention", "tgis_k_attention_split", "tgis_k_attention_split_bench", "tgis_k_rope_attention",
     "tgis_k_attention_bench", "tgis_k_decode_items", "tgis_k_gemm_plan", "tgis_k_gemm_schedule", "tgis_k_gemm_chain", "tgis_k_gemm_blocks_per_sm",
-    "tgis_k_sampler", "tgis_k_sampler_ex", "tgis_k_sampler_masked", "tgis_k_sampler_scaled", "tgis_k_lora", "tgis_k_lora_bench", "tgis_k_silu_mul_interleaved", "tgis_k_sizeof_sample_row", "tgis_k_sizeof_sample_out", "tgis_k_kv_block",
+    "tgis_k_sampler", "tgis_k_sampler_ex", "tgis_k_sampler_masked", "tgis_k_sampler_scaled", "tgis_k_lora", "tgis_k_lora_group", "tgis_k_lora_bench", "tgis_k_silu_mul_interleaved", "tgis_k_sizeof_sample_row", "tgis_k_sizeof_sample_out", "tgis_k_kv_block",
     "tgis_k_rope_kv_hd", "tgis_k_attention_hd", "tgis_k_attention_split_hd", "tgis_k_attention_bench_hd",
     "tgis_k_rope_kv_qknorm", "tgis_k_tp_area_bytes", "tgis_k_tp_exchange", "tgis_k_logits_push", "tgis_k_logits_wait",
     "tgis_k_gather_relayout", "tgis_k_tp_exchange_check", "tgis_k_logits_wait_check",
@@ -174,6 +174,7 @@ def load_library() -> C.CDLL:
     lib.tgis_k_sampler.argtypes = [vp, i32, i32, vp, i32, vp, vp]
     lib.tgis_k_sampler_ex.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, i32, C.POINTER(f32)]
     lib.tgis_k_lora.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, i32, vp, i32, i32]
+    lib.tgis_k_lora_group.argtypes = [vp, i32, vp, vp, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(i32), i32, vp, i32, i32]
     lib.tgis_k_silu_mul_interleaved.argtypes = [vp, vp, i32, i32]
     lib.tgis_k_lora_bench.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, i32, C.POINTER(f32), C.POINTER(f32)]
     lib.tgis_k_sampler_masked.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, i32, C.POINTER(f32)]
