@@ -2,8 +2,8 @@
 7, which Qwen2.5 (0.5B: 14 / 2 heads of 64, 1.5B: 12 / 2, 7B: 28 / 4, 14B and 32B: 40 / 8), Qwen3-14B (40 / 8) and
 Mistral-Small-22B (48 / 8) have, at both head sizes, on their own before any engine relies on them.
 
-The cases, the poison and the bar are those of tests/test_sliding_window_gpu.py (imported, with window 0 for full
-attention), which are those of tests/test_attention_precision_gpu.py: every element within one bf16 ulp of a float64
+The cases, the poison and the bar are those of tests/test_sliding_window_gpu.py (tgis_gpu_utils.PagedCase, with window 0
+for full attention), which are those of tests/test_attention_precision_gpu.py: every element within one bf16 ulp of a float64
 reference or within 2^-16 of its row's largest |reference| times the chained-key factor, at least 99 % bit-exact, finite
 poison in every slot outside a sequence, and -- with a window -- NaN in every block wholly below it.  Two launches give
 the same bits.  Last, a qwen3-tiny engine with 5 q heads over 1 kv head (a Qwen3-14B-shaped group) follows
@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_sliding_window_gpu import Case, _assert_bar
+from tgis_gpu_utils import PagedCase, assert_attention_bar
 
 pytestmark = pytest.mark.gpu
 
@@ -50,9 +50,9 @@ def test_decode_at_groups_5_6_7_meets_float64_bar(g, D, n_q, n_kv):
     rng = np.random.RandomState(n_q * 100 + n_kv + D)
     while sum((n + 127) // 128 for n in lengths) * n_kv <= 3 * slots:
         lengths.append(int(rng.randint(1, 8193)))
-    case = Case(g, D, n_q, n_kv, [(n - 1, 1) for n in lengths], 0, seed=n_q * 10 + n_kv + D)
+    case = PagedCase(D, n_q, n_kv, [(n - 1, 1) for n in lengths], 0, seed=n_q * 10 + n_kv + D)
     out = case.run(0)
-    _assert_bar(g, out, *case.reference(), f"decode D={D} ({n_q}, {n_kv}), {len(lengths)} sequences")
+    assert_attention_bar(out, *case.reference(), f"decode D={D} ({n_q}, {n_kv}), {len(lengths)} sequences")
     assert torch.equal(out, case.run(0)), "two launches differ"
 
 
@@ -63,9 +63,9 @@ PREFILL_SPECS = [(0, 2048), (7680, 512), (4097, 2), (4097, 17), (3001, 1000), (3
 @pytest.mark.parametrize("D,n_q,n_kv", GROUP_CASES, ids=[_ids(c) for c in GROUP_CASES])
 def test_prefill_and_chunked_prefill_at_groups_5_6_7_meet_float64_bar(g, D, n_q, n_kv):
     """whole prompts, chunks over contexts up to 8191 off the 16 / 32 grid, and decode rows in the same call"""
-    case = Case(g, D, n_q, n_kv, PREFILL_SPECS, 0, seed=n_q * 1000 + n_kv + D)
+    case = PagedCase(D, n_q, n_kv, PREFILL_SPECS, 0, seed=n_q * 1000 + n_kv + D)
     out = case.run(0)
-    _assert_bar(g, out, *case.reference(), f"prefill + decode D={D} ({n_q}, {n_kv})")
+    assert_attention_bar(out, *case.reference(), f"prefill + decode D={D} ({n_q}, {n_kv})")
     assert torch.equal(out, case.run(0)), "two launches differ"
 
 
@@ -76,11 +76,11 @@ SPLIT_SPECS = [(1024, 128), (1024, 1), (8000, 100), (4097, 17), (2048, 16), (150
 def test_split_context_prefill_at_groups_5_6_7_meets_float64_bar(g, D, n_q, n_kv):
     """every prefill sequence on the split-context cluster kernel (mode 1: blockDim 32 G, the cluster merge over 2 G
     (head, row) pairs), then the engine's selection (mode 2)"""
-    case = Case(g, D, n_q, n_kv, SPLIT_SPECS, 0, seed=n_q * 7 + n_kv + D)
+    case = PagedCase(D, n_q, n_kv, SPLIT_SPECS, 0, seed=n_q * 7 + n_kv + D)
     ref, floor = case.reference()
     for mode in (1, 2):
         out = case.run(mode)
-        _assert_bar(g, out, ref, floor, f"split-context prefill D={D} mode {mode} ({n_q}, {n_kv})")
+        assert_attention_bar(out, ref, floor, f"split-context prefill D={D} mode {mode} ({n_q}, {n_kv})")
         assert torch.equal(out, case.run(mode)), "two launches differ"
 
 
@@ -93,13 +93,13 @@ def test_sliding_window_of_40_at_groups_5_6_7_meets_float64_bar(g, D, n_q, n_kv)
     split-context suffixes; every block wholly below a window is NaN"""
     W = 40
     dec = [(n - 1, 1) for n in (1, W - 1, W, W + 1, W + 32, W + 129, 2 * W + 5, 8192)]
-    case = Case(g, D, n_q, n_kv, dec + [(0, 2 * W + 37), (W + 5, 64), (1000, 1000), (4097, 33)], W,
+    case = PagedCase(D, n_q, n_kv, dec + [(0, 2 * W + 37), (W + 5, 64), (1000, 1000), (4097, 33)], W,
                 seed=W + n_q * 11 + n_kv + D)
     assert case.n_nan_blocks > 0
     ref, floor = case.reference()
     for mode in (0, 1):
         out = case.run(mode)
-        _assert_bar(g, out, ref, floor, f"W={W} D={D} mode {mode} ({n_q}, {n_kv})")
+        assert_attention_bar(out, ref, floor, f"W={W} D={D} mode {mode} ({n_q}, {n_kv})")
         assert torch.equal(out, case.run(mode)), "two launches differ"
 
 

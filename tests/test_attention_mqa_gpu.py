@@ -8,7 +8,7 @@ chained-key floor, at least 99 % bit-exact, poisoned cache slots outside the seq
 import pytest
 import torch
 
-from test_sliding_window_gpu import Case, _assert_bar, _scale
+from tgis_gpu_utils import PagedCase, assert_attention_bar, attention_scale
 
 pytestmark = pytest.mark.gpu
 
@@ -33,9 +33,9 @@ def _decode_specs():
 @pytest.mark.parametrize("W", [0, 40])
 @pytest.mark.parametrize("n_q,n_kv", HEADS)
 def test_large_group_decode_meets_float64_bar(g, n_q, n_kv, W):
-    case = Case(g, 128, n_q, n_kv, _decode_specs(), W, seed=n_q * 5 + n_kv + W)
+    case = PagedCase(128, n_q, n_kv, _decode_specs(), W, seed=n_q * 5 + n_kv + W)
     out = case.run()
-    _assert_bar(g, out, *case.reference(), f"decode ({n_q}, {n_kv}) W={W}")
+    assert_attention_bar(out, *case.reference(), f"decode ({n_q}, {n_kv}) W={W}")
     assert torch.equal(out, case.run()), "two launches differ"
 
 
@@ -47,9 +47,9 @@ def _prefill_specs():
 @pytest.mark.parametrize("W", [0, 40])
 @pytest.mark.parametrize("n_q,n_kv", HEADS)
 def test_large_group_prefill_and_chunked_prefill_meet_float64_bar(g, n_q, n_kv, W):
-    case = Case(g, 128, n_q, n_kv, _prefill_specs(), W, seed=n_q * 13 + n_kv + W)
+    case = PagedCase(128, n_q, n_kv, _prefill_specs(), W, seed=n_q * 13 + n_kv + W)
     out = case.run(0)
-    _assert_bar(g, out, *case.reference(), f"prefill + decode ({n_q}, {n_kv}) W={W}")
+    assert_attention_bar(out, *case.reference(), f"prefill + decode ({n_q}, {n_kv}) W={W}")
     assert torch.equal(out, case.run(0)), "two launches differ"
 
 
@@ -61,11 +61,11 @@ def _split_specs():
 @pytest.mark.parametrize("n_q,n_kv", HEADS)
 def test_large_group_split_context_prefill_meets_float64_bar(g, n_q, n_kv, W):
     """every prefill sequence on the split-context cluster kernel (mode 1), then the engine's selection (mode 2)"""
-    case = Case(g, 128, n_q, n_kv, _split_specs(), W, seed=n_q * 7 + n_kv + W)
+    case = PagedCase(128, n_q, n_kv, _split_specs(), W, seed=n_q * 7 + n_kv + W)
     ref, floor = case.reference()
     for mode in (1, 2):
         out = case.run(mode)
-        _assert_bar(g, out, ref, floor, f"split-context prefill mode {mode} ({n_q}, {n_kv}) W={W}")
+        assert_attention_bar(out, ref, floor, f"split-context prefill mode {mode} ({n_q}, {n_kv}) W={W}")
         assert torch.equal(out, case.run(mode)), "two launches differ"
 
 
@@ -74,10 +74,10 @@ def test_unbuilt_groups_are_reported_invalid_not_run(g, D, n_q, n_kv):
     """G = 65 (and groups above 8 at 64-dim heads) are refused by every launcher before anything runs"""
     for mode in (0, 1):
         for specs in ([(9, 1)], [(0, 20)]):
-            c = Case(g, D, n_q, n_kv, specs, 0, seed=3)
+            c = PagedCase(D, n_q, n_kv, specs, 0, seed=3)
             out = torch.zeros(c.q.shape, dtype=torch.bfloat16, device="cuda")
             rc = g.lib().tgis_k_attention_window(D, g.ptr(c.qkv), g.ptr(c.kc), g.ptr(c.vc), g.i32p(c.seqs.reshape(-1)),
                                                  1, g.i32p(c.bt.reshape(-1)), 1, c.bt_stride, g.ptr(out), n_q, n_kv,
-                                                 _scale(D), mode, 0)
+                                                 attention_scale(D), mode, 0)
             assert rc != 0 and "invalid" in g.kerr().lower(), (specs, mode, g.kerr())
             assert not bool(out.float().abs().sum()), "nothing may be written"

@@ -13,7 +13,7 @@ import torch
 
 from qwen2_oracle import CONFIGS, Qwen2Oracle, synthetic_weights
 from test_qwen3_gpu import _prompt, _sp, _ulp
-from test_sliding_window_gpu import k_cache_from_dense, v_cache_from_dense
+from tgis_gpu_utils import paged_k_cache as k_cache_from_dense, paged_v_cache as v_cache_from_dense
 
 pytestmark = pytest.mark.gpu
 

@@ -160,6 +160,190 @@ def dense_from_v_cache(vc: torch.Tensor) -> torch.Tensor:
     return x.permute(0, 2, 1, 3, 4).reshape(nb * KV_BLOCK, n_kv, HEAD_DIM)
 
 
+# ------------------------------------------------------------------------------------ paged attention cases, any D
+# Shared by the sliding-window and long-context tests: the cache is built on the device from a seeded generator (no
+# per-token Python loop: a case holds up to a few hundred thousand tokens), and the float64 reference runs on the device.
+POISON_K, POISON_V = 32.0, 512.0
+EXTREME_K, EXTREME_V = 16384.0, 32768.0
+Q_BIAS = 0.5
+MIN_EXACT = 0.99
+REF_SCORE_BYTES = 256 << 20   # the largest float64 score tensor the reference builds at once
+DECODE_SPLIT = 128            # tokens per decode split (kernels.h)
+
+
+def attention_scale(D: int) -> float:
+    import math
+
+    return float(np.float32(1.0 / math.sqrt(D)))
+
+
+def paged_k_cache(k: torch.Tensor, n_blocks: int) -> torch.Tensor:
+    """k [n_blocks * 32, n_kv, D] (token t in slot t) -> [blocks][n_kv][D / 8 chunks][32 tok][8]"""
+    n_kv, D = k.shape[1], k.shape[2]
+    return k.view(n_blocks, 32, n_kv, D // 8, 8).permute(0, 2, 3, 1, 4).contiguous()
+
+
+def paged_v_cache(v: torch.Tensor, n_blocks: int) -> torch.Tensor:
+    """-> [blocks][n_kv][32 tok][v_chunk(D / 8 chunks, tok)][8]: chunk ^ (tok & 7); at D = 96 chunks 8..11 are xor-ed
+    among themselves by (tok >> 1) & 3 (kernels.h v_chunk).  Both are involutions, so the gather index is the map."""
+    n_kv, D = v.shape[1], v.shape[2]
+    C_ = D // 8
+    x = v.view(n_blocks, 32, n_kv, C_, 8).permute(0, 2, 1, 3, 4).contiguous()
+    tok = torch.arange(32, device=v.device)[:, None]
+    chunk = torch.arange(C_, device=v.device)[None, :]
+    src = chunk ^ (tok & 7)
+    if D == 96:
+        src = torch.where(chunk < 8, src, 8 + ((chunk - 8) ^ ((tok >> 1) & 3)))
+    return torch.gather(x, 3, src[None, None, :, :, None].expand(n_blocks, n_kv, 32, C_, 8)).contiguous()
+
+
+def masked_reference_f64(q, k, v, first_pos, window, D):
+    """float64 softmax(q k^T / sqrt(D)) v of one sequence with the causal and window masks.  One kv head at a time, and
+    the query rows in chunks, so that no score tensor exceeds REF_SCORE_BYTES."""
+    q_len, n_q, _ = q.shape
+    kv_len, n_kv, _ = k.shape
+    G = n_q // n_kv
+    rows = max(1, REF_SCORE_BYTES // (8 * G * kv_len))
+    kpos = torch.arange(kv_len, device=q.device)[None, :]
+    out = torch.empty(q_len, n_q, D, dtype=torch.float64, device=q.device)
+    for h in range(n_kv):
+        kh, vh = k[:, h].double(), v[:, h].double()
+        for r0 in range(0, q_len, rows):
+            r1 = min(q_len, r0 + rows)
+            qpos = first_pos + torch.arange(r0, r1, device=q.device)[:, None]
+            hidden = kpos > qpos
+            if window:
+                hidden = hidden | (kpos <= qpos - window)
+            s = q[r0:r1, h * G:(h + 1) * G].double().transpose(0, 1) @ kh.t() * attention_scale(D)
+            p = torch.softmax(s.masked_fill_(hidden, float("-inf")), dim=-1)
+            out[r0:r1, h * G:(h + 1) * G] = (p @ vh).transpose(0, 1)
+            del s, p
+    return out
+
+
+def needle_positions(kv_len: int) -> list[int]:
+    """keys in decode splits 70 and 700 and in the last split (those the sequence has)"""
+    last = (kv_len - 1) // DECODE_SPLIT
+    pos = [sp * DECODE_SPLIT + off for sp, off in ((70, 37), (700, 91)) if sp < last]
+    return pos + [last * DECODE_SPLIT + min(5, kv_len - 1 - last * DECODE_SPLIT)]
+
+
+def paged_seq_kv(mode, kv_len, n_kv, D, gen):
+    """K / V of one sequence, drawn on the device.  The queries are randn + Q_BIAS in every dimension, so a key along
+    the all-ones direction scores about Q_BIAS * sqrt(D) per unit of its value (in units of the softmax's e-fold):
+      rand       K ~ 1.5 randn, V ~ randn
+      peak_last  K scaled by 4 and the last key lifted by 8
+      wide_v     V spread over 2^-12 .. 2^12
+      needles    rand plus keys in decode splits 70, 700 and the last one that score about 11 - 13 above the mean, each
+                 as heavy as a large part of the 8k - 128k bulk: the output depends on every chunk of 64 splits
+      rising     rand plus a ramp that lifts the scores by about 40 from the first key to the last: the running maximum
+                 moves from chunk to chunk, so the merge's exp2(m_split - m_final) rescaling carries the result
+      cliff      rand with the last split's keys lifted by about 200 (290 in the kernel's log2 domain; the spread over the
+                 query heads is 2 / sqrt(D) of that per standard deviation): a merge that took the row maximum without
+                 that split would overflow exp2f to inf in the typical head (NaN out)"""
+    k = torch.randn(kv_len, n_kv, D, generator=gen, device="cuda") * 1.5
+    v = torch.randn(kv_len, n_kv, D, generator=gen, device="cuda")
+    unit = 1.0 / (Q_BIAS * D ** 0.5)   # K value per unit of expected score along the all-ones direction
+    if mode == "peak_last":
+        k = k * 4.0
+        k[kv_len - 1] += 8.0
+    elif mode == "wide_v":
+        v = v * torch.exp2(torch.randint(-12, 13, v.shape, generator=gen, device="cuda").float())
+    elif mode == "needles":
+        for i, p in enumerate(needle_positions(kv_len)):
+            k[p] = (11.0 + i) * unit
+    elif mode == "rising":
+        k += (40.0 * unit / kv_len) * torch.arange(kv_len, device="cuda", dtype=torch.float32)[:, None, None]
+    elif mode == "cliff":
+        k[(kv_len - 1) // DECODE_SPLIT * DECODE_SPLIT:] += 200.0 * unit
+    else:
+        assert mode == "rand", mode
+    return k.bfloat16(), v.bfloat16()
+
+
+class PagedCase:
+    """specs = [(context before this step, q_len[, K / V mode])] over one paged cache of D-dim heads, blocks scattered
+    over a permuted pool; a spec without a mode takes modes[index % len(modes)].  Poisoned for `window`:
+      * every cache block wholly below the lowest position any row of the sequence sees is NaN (K and V): the kernels
+        must never load it, since a NaN value times p = 0 is still NaN;
+      * the positions of the block holding that lowest visible position that lie below it hold finite extremes (K 2^14,
+        V 2^15): loaded, and they must be masked;
+      * slots outside every sequence hold a finite poison (K 32, V 512)."""
+
+    def __init__(self, D, n_q, n_kv, specs, window, seed, modes=("rand", "peak_last", "wide_v")):
+        self.D, self.n_q, self.n_kv, self.window = D, n_q, n_kv, window
+        self.specs = [(s[0], s[1]) for s in specs]
+        self.modes = [s[2] if len(s) > 2 else modes[i % len(modes)] for i, s in enumerate(specs)]
+        gen = torch.Generator(device="cuda").manual_seed(seed)
+        T = sum(q for _, q in self.specs)
+        self.q = (torch.randn(T, n_q, D, generator=gen, device="cuda") + Q_BIAS).bfloat16()
+        self.qkv = torch.zeros(T, n_q + 2 * n_kv, D, dtype=torch.bfloat16, device="cuda")
+        self.qkv[:, :n_q] = self.q
+        nbs = [(c + q + 31) // 32 for c, q in self.specs]
+        self.bt_stride = max(nbs)
+        n_blocks = sum(nbs) + 8
+        order = torch.from_numpy(np.random.RandomState(seed).permutation(n_blocks)).cuda()
+        k_pool = torch.full((n_blocks * 32, n_kv, D), POISON_K, dtype=torch.bfloat16, device="cuda")
+        v_pool = torch.full((n_blocks * 32, n_kv, D), POISON_V, dtype=torch.bfloat16, device="cuda")
+        self.bt = np.zeros((len(self.specs), self.bt_stride), dtype=np.int32)
+        self.seqs = np.zeros((len(self.specs), 4), dtype=np.int32)
+        self.kv = []
+        self.n_nan_blocks = 0
+        cur, q_start = 0, 0
+        for s, ((ctx, ql), nb, mode) in enumerate(zip(self.specs, nbs, self.modes)):
+            blocks = order[cur: cur + nb]
+            cur += nb
+            self.bt[s, :nb] = blocks.cpu().numpy()
+            kv_len = ctx + ql
+            k, v = paged_seq_kv(mode, kv_len, n_kv, D, gen)
+            pos = torch.arange(kv_len, device="cuda")
+            slots = blocks[pos // 32] * 32 + pos % 32
+            k_pool[slots], v_pool[slots] = k, v
+            if window:
+                lo = max(0, ctx - window + 1)   # the lowest position the first query row sees
+                hid = pos < lo
+                nan = pos < (lo // 32) * 32
+                self.n_nan_blocks += lo // 32
+                k_pool[slots[hid]], v_pool[slots[hid]] = EXTREME_K, EXTREME_V
+                k_pool[slots[nan]], v_pool[slots[nan]] = float("nan"), float("nan")
+            self.kv.append((k, v))
+            self.seqs[s] = (q_start, ql, kv_len, s)
+            q_start += ql
+        self.kc = paged_k_cache(k_pool, n_blocks)
+        self.vc = paged_v_cache(v_pool, n_blocks)
+        del k_pool, v_pool
+
+    def run(self, mode=0, window=None):
+        """tgis_k_attention_window: mode 0 every prefill tile on the plain kernel, 1 on the split-context kernel, 2 the
+        engine's selection; decode rows (q_len 1) on the decode kernel and the split merge in every mode"""
+        out = torch.zeros(self.q.shape, dtype=torch.bfloat16, device="cuda")
+        rc = lib().tgis_k_attention_window(self.D, ptr(self.qkv), ptr(self.kc), ptr(self.vc),
+                                           i32p(self.seqs.reshape(-1)), len(self.specs), i32p(self.bt.reshape(-1)),
+                                           len(self.specs), self.bt_stride, ptr(out), self.n_q, self.n_kv,
+                                           attention_scale(self.D), mode, self.window if window is None else window)
+        assert rc == 0, kerr()
+        return out
+
+    def reference(self, floor=attention_floor_scale):
+        """float64 reference [T, n_q, D] and the per-row floor factor, floor(context, q_len) per sequence"""
+        ref = torch.empty(self.q.shape, dtype=torch.float64, device="cuda")
+        scale = torch.empty(self.q.shape[0], 1, 1, dtype=torch.float64)
+        for (ctx, ql), (k, v), (q0, *_) in zip(self.specs, self.kv, self.seqs):
+            ref[q0: q0 + ql] = masked_reference_f64(self.q[q0: q0 + ql], k, v, ctx, self.window, self.D)
+            scale[q0: q0 + ql] = floor(ctx, ql)
+        return ref, scale
+
+
+def assert_attention_bar(out, ref, floor, what):
+    """attention_bar with no element over it, no NaN and at least MIN_EXACT bit-exact; returns the worst-element text"""
+    assert not bool(torch.isnan(out).any()), f"{what}: NaN in the output"
+    n_bad, exact, worst = attention_bar(out, ref, floor)
+    print(f"{what}: {exact * 100:.2f} % bit-exact, {n_bad} over the bar ({worst})")
+    assert n_bad == 0, f"{what}: {n_bad} elements over the bar; {worst}"
+    assert exact >= MIN_EXACT, f"{what}: only {exact * 100:.2f} % bit-exact"
+    return worst
+
+
 def run_sampler(logits: torch.Tensor, rows: np.ndarray, bitmap: torch.Tensor | None = None, iters: int = 1,
                 return_us: bool = False, allow: torch.Tensor | None = None):
     """logits: fp32 (golden fixtures) or bf16 (the product path's dtype) [rows, V] on the device."""
