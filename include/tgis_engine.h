@@ -263,6 +263,8 @@ int tgis_engine_load_weight(tgis_engine* e, const char* name, const void* ptr, i
 /* cumulative tokens looked up / found in the cache (vllm:prefix_cache_queries / _hits: as in vLLM, the lookups of a
  * preempted request's recompute are not counted) and the keyed blocks right now */
 int tgis_engine_prefix_cache_stats(tgis_engine* e, int64_t* queried_tokens, int64_t* hit_tokens, int32_t* cached_blocks);
+/* Fails, naming what is missing, unless every tensor the model needs was loaded; lm_head.weight may be left out (it is
+ * then tied to the embedding), and so may tgis.rope_cos_sin unless rope_table_from_host is set. */
 int tgis_engine_start(tgis_engine* e);
 int tgis_engine_add_request(tgis_engine* e, const char* request_id, const int32_t* prompt_ids, int32_t n_prompt,
                             const tgis_sampling_params* params);

@@ -373,14 +373,15 @@ def test_granite_tiny_graphs_and_batch_invariance():
         assert len([r for r in recs if r.new_token is not None]) == 40
 
 
-def test_granite_scalars_only_before_start_and_64_dim_heads_refused():
+def test_granite_engine_starts_on_its_checkpoint_and_64_dim_heads_refused():
     import dataclasses
 
-    from granite_oracle import CONFIGS
+    from granite_oracle import CONFIGS, synthetic_weights
     from vllm_tgis_adapter_b200.engine.core import EngineError, NativeEngine
 
     cfg = CONFIGS["granite-tiny"]
     eng = NativeEngine(_mc(cfg), max_num_seqs=2, max_batched_tokens=64, kv_cache_bytes=16 << 20)
+    eng.load_weights(synthetic_weights(cfg, seed=1))   # start refuses a checkpoint with tensors missing
     eng.start()
     eng.close()
     with pytest.raises(EngineError, match="finite and non-negative"):

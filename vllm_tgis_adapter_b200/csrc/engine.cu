@@ -12,7 +12,6 @@
 #include <algorithm>
 #include <array>
 #include <list>
-#include <set>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -237,18 +236,28 @@ struct tgis_engine {
   // weights
   DevBuf<bf16> w_arena;
   bf16 *embed = nullptr, *lm_head = nullptr, *final_norm = nullptr, *cos_sin = nullptr;
-  bool lm_head_loaded = false, cos_sin_loaded = false;
-  bool rope_table_required = false;  // scaled RoPE: default_rope_table() is not this model's table
   // Qwen3 (tgis_config.qk_norm): layer l's q_norm [128] at qk_norm_w + 256 l, its k_norm 128 further, in an
-  // allocation of their own, so that the arena and the KV block count of every other model stay as they are;
-  // qk_norm_loaded: per layer, bit 0 = q_norm, bit 1 = k_norm
+  // allocation of their own, so that the arena and the KV block count of every other model stay as they are
   DevBuf<bf16> qk_norm_w;
-  std::vector<uint8_t> qk_norm_loaded;
   // Qwen2 (tgis_config.qkv_bias): layer l's q | k | v bias [qkv_dim] at qkv_bias_w + qkv_dim l, in wqkv's row order
-  // and an allocation of its own (the qkv GEMM then writes fp32 to y32); qkv_bias_loaded: per layer, bit 0 = q, 1 = k,
-  // 2 = v
+  // and an allocation of its own (the qkv GEMM then writes fp32 to y32)
   DevBuf<bf16> qkv_bias_w;
-  std::vector<uint8_t> qkv_bias_loaded;
+  // Every checkpoint tensor this engine accepts (weight_table(), at init): the copies that take the full, unsharded
+  // checkpoint tensor to its place, and whether start needs it.  A copy is one cudaMemcpy2D (a cudaMemcpy when both sides
+  // are contiguous), in elements: `height` rows of `width` from src_off, spitch apart in the source, dpitch apart at dst.
+  struct WeightCopy {
+    bf16* dst;
+    size_t src_off, spitch, dpitch, width, height;
+  };
+  struct WeightEntry {
+    std::string name;
+    int layer;  // -1: not a per-layer tensor
+    int64_t n;  // elements the tensor must have; 0: the positions table, which needs cols == hidden, rows >= pos_rows
+    bool required, loaded;
+    std::vector<WeightCopy> copies;
+  };
+  std::vector<WeightEntry> wtab;
+  std::unordered_map<std::string, size_t> wtab_at;  // name -> index in wtab
   // OPT (opt.cu): learned positions [max_model_len + 2, hidden], final LayerNorm bias; model head dim (64 or 128: every
   // head is zero-padded to the 128-dim attention tiles at load time); fp32 GEMM accumulators of the biased projections.
   // GPTBigCode runs the same layer stack (opt is set too): positions [max_model_len, hidden] without OPT's offset of 2,
@@ -266,7 +275,6 @@ struct tgis_engine {
   // GEMM's output rows stay 16-byte aligned for any vocabulary; the sampler is told ld = Vpad, vocab = V
   int Vpad = 0;
   DevBuf<float> y32;
-  std::set<std::string> opt_loaded;  // tensor names seen by load_weight_opt (completeness check at start)
   std::vector<LayerW> layers;
   CUtensorMap m_lm{};
   // kv cache
@@ -321,12 +329,10 @@ struct tgis_engine {
   // LoRA adapters (lora.cu): per layer and module  A [slots][Rm][K], B [slots][N][Rm] bf16, zero padded to the rank capacity;
   // gate_proj / up_proj form ONE module of capacity 2R over the interleaved gate_up projection
   int max_loras = 0, lora_R = 0;
-  struct LoraLayerW {
-    bf16 *A_q, *B_q, *A_k, *B_k, *A_v, *B_v, *A_o, *B_o, *A_gu, *B_gu, *A_d, *B_d;
-  };
   DevBuf<bf16> lora_arena;
-  size_t lora_slot_elems = 0;  // (unused by the kernels; bookkeeping for clear)
-  std::vector<LoraLayerW> lora_layers;
+  // per layer, lora.cu's groups of modules that read the same x, carved from lora_arena by init()
+  enum { LORA_QKV, LORA_O, LORA_GATE_UP, LORA_DOWN, LORA_GROUPS };
+  std::vector<std::array<LoraGroup, LORA_GROUPS>> lora_groups;
   DevBuf<float> lora_v;   // [T][3R] fp32 shrink sums
   DevBuf<bf16> gu_buf;    // [T][2F] raw (interleaved) gate_up output of steps that carry adapter tokens
   long long lora_steps = 0;
@@ -484,7 +490,6 @@ struct tgis_engine {
     res_mult = or_one(c.residual_multiplier);
     logit_scale = or_one(c.logit_scale);
     attn_window = c.sliding_window;
-    rope_table_required = c.rope_table_from_host != 0;
     prefix_caching = c.enable_prefix_caching != 0;
     pos_rows = bigcode ? c.max_model_len : opt ? c.max_model_len + 2 : 0;
     q_dim = nq * kv_head_dim;
@@ -575,20 +580,26 @@ struct tgis_engine {
                                      (size_t)2 * F * 2 * R + R * F + H * R);
       lora_arena.alloc(per_layer * L);
       lora_arena.zero();
-      lora_layers.resize(L);
       bf16* p = lora_arena.p;
-      auto take = [&](size_t n) {
-        bf16* r = p;
-        p += n;
-        return r;
+      // A [slots][Rm][K], then B [slots][N][Rm]
+      auto module = [&](size_t K, size_t N, size_t Rm, size_t col0, size_t v_off) {
+        const LoraModule m{p, p + Sl * Rm * K, (int)K, (int)N, (int)Rm, (int)col0, (int)v_off};
+        p += Sl * (Rm * K + N * Rm);
+        return m;
       };
-      for (auto& ll : lora_layers) {
-        ll.A_q = take(Sl * R * H);      ll.B_q = take(Sl * q_dim * R);
-        ll.A_k = take(Sl * R * H);      ll.B_k = take(Sl * kvd * R);
-        ll.A_v = take(Sl * R * H);      ll.B_v = take(Sl * kvd * R);
-        ll.A_o = take(Sl * R * q_dim);  ll.B_o = take(Sl * H * R);
-        ll.A_gu = take(Sl * 2 * R * H); ll.B_gu = take(Sl * (size_t)2 * F * 2 * R);
-        ll.A_d = take(Sl * R * F);      ll.B_d = take(Sl * H * R);
+      lora_groups.assign(L, {});
+      for (auto& gs : lora_groups) {
+        for (LoraGroup& g : gs) {
+          g.n_mods = 1;
+          g.v_ld = 3 * R;
+        }
+        gs[LORA_QKV].n_mods = 3;
+        gs[LORA_QKV].mod[0] = module(H, q_dim, R, 0, 0);
+        gs[LORA_QKV].mod[1] = module(H, kvd, R, q_dim, R);
+        gs[LORA_QKV].mod[2] = module(H, kvd, R, q_dim + kvd, 2 * R);
+        gs[LORA_O].mod[0] = module(q_dim, H, R, 0, 0);
+        gs[LORA_GATE_UP].mod[0] = module(H, 2 * F, 2 * R, 0, 0);  // gate_proj and up_proj
+        gs[LORA_DOWN].mod[0] = module(F, H, R, 0, 0);
       }
       lora_v.alloc(T_alloc * 3 * R);
       gu_buf.alloc(T_alloc * (size_t)2 * F);
@@ -695,15 +706,12 @@ struct tgis_engine {
     free_slots.resize(S_max);
     for (int i = 0; i < S_max; ++i) free_slots[i] = S_max - 1 - i;
     // after the KV cache: with kv_cache_bytes == 0 its size comes from the free memory, which these must not shrink
-    if (c.qk_norm) {
-      qk_norm_w.alloc((size_t)2 * L * HEAD_DIM);
-      qk_norm_loaded.assign(L, 0);
-    }
+    if (c.qk_norm) qk_norm_w.alloc((size_t)2 * L * HEAD_DIM);
     if (c.qkv_bias) {
       y32.alloc(T_alloc * qkv_dim);
       qkv_bias_w.alloc(L * qkv_dim);
-      qkv_bias_loaded.assign(L, 0);
     }
+    weight_table();
     if (prefix_caching) pcb.assign(num_blocks, PcBlock{});
     snapshot();
     CK(cudaStreamSynchronize(stream));
@@ -912,202 +920,145 @@ struct tgis_engine {
     CK(cudaMemcpy(cos_sin, tab.data(), tab.size() * sizeof(bf16), cudaMemcpyHostToDevice));
   }
 
-  // Copies the FULL (unsharded) tensor's shard for this rank into the arena: row blocks for column-parallel layers
-  // (q/k/v/gate/up, lm_head), column blocks for row-parallel layers (o, down), everything else replicated.
-  // OPT checkpoints (HF names, "model.decoder." or "decoder." prefix).  Single GPU: every tensor is kept whole.  q/k/v rows,
-  // out_proj columns and the q/k/v biases are spread head by head over 128-dim head slots (the upper 128 - head_dim dims of
-  // every slot stay zero: the arena was zeroed), so the attention kernels and the paged cache keep their one geometry.
-  int load_weight_opt(const std::string& full_name, const void* ptr, int64_t rows, int64_t cols) {
-    const tgis_config& c = cfg;
-    const int64_t H = c.hidden, F = c.ffn, V = c.vocab, hd = model_head_dim, nh = c.n_q_heads;
-    std::string name = full_name;
-    if (name.rfind("model.", 0) == 0) name = name.substr(6);
-    auto shape_err = [&]() {
-      return fail("shape mismatch for " + full_name + ": got " + std::to_string(rows) + "x" + std::to_string(cols));
-    };
-    auto copy = [&](bf16* dst, int64_t n) -> int {
-      if (rows * cols != n) return shape_err();
-      const cudaError_t e = cudaMemcpy(dst, ptr, (size_t)n * sizeof(bf16), cudaMemcpyDefault);
-      return e == cudaSuccess ? 0 : fail(std::string("cudaMemcpy(weight) failed: ") + cudaGetErrorString(e));
-    };
-    // n_rows source rows of `w` elements each -> destination rows `dpitch` elements apart
-    auto copy2d = [&](bf16* dst, int64_t dpitch, int64_t w, int64_t n_rows) -> int {
-      if (rows * cols != w * n_rows) return shape_err();
-      const cudaError_t e = cudaMemcpy2D(dst, (size_t)dpitch * sizeof(bf16), ptr, (size_t)w * sizeof(bf16),
-                                         (size_t)w * sizeof(bf16), (size_t)n_rows, cudaMemcpyDefault);
-      return e == cudaSuccess ? 0 : fail(std::string("cudaMemcpy2D(weight) failed: ") + cudaGetErrorString(e));
-    };
-    if (name == "lm_head.weight") { lm_head_loaded = true; return copy(lm_head, V * H); }
-    if (name.rfind("decoder.", 0) != 0) return fail("unknown weight " + full_name);
-    name = name.substr(8);
-    opt_loaded.insert(name);  // (a failed copy fails the load as a whole)
-    if (name == "embed_tokens.weight") return copy(embed, V * H);
-    if (name == "embed_positions.weight") {
-      // the checkpoint's table covers max_position_embeddings + 2 rows; the engine keeps what max_model_len can reach
-      if (cols != H || rows < pos_rows) return shape_err();
-      const cudaError_t e = cudaMemcpy(pos_embed, ptr, (size_t)pos_rows * H * sizeof(bf16), cudaMemcpyDefault);
-      return e == cudaSuccess ? 0 : fail(std::string("cudaMemcpy(weight) failed: ") + cudaGetErrorString(e));
-    }
-    if (name == "final_layer_norm.weight") return copy(final_norm, H);
-    if (name == "final_layer_norm.bias") return copy(final_norm_b, H);
-    if (name.rfind("layers.", 0) != 0) return fail("unknown weight " + full_name);
-    const size_t dot = name.find('.', 7);
-    if (dot == std::string::npos) return fail("bad weight name " + full_name);
-    const int li = atoi(name.substr(7, dot - 7).c_str());
-    if (li < 0 || li >= c.n_layers) return fail("layer index out of range in " + full_name);
-    LayerW& l = layers[li];
-    const std::string sub = name.substr(dot + 1);
-    const int64_t slot_w = (int64_t)HEAD_DIM * H;  // elements of one padded head's rows in wqkv
-    for (int j = 0; j < 3; ++j) {
-      static const char* const qkv_names[3] = {"q_proj", "k_proj", "v_proj"};
-      const std::string base = std::string("self_attn.") + qkv_names[j];
-      // head h's hd rows of [H] -> rows [h * 128, h * 128 + hd) of the projection's block
-      if (sub == base + ".weight") return copy2d(l.wqkv + (size_t)j * nh * slot_w, slot_w, hd * H, nh);
-      if (sub == base + ".bias") return copy2d(l.b_qkv + (size_t)j * nh * HEAD_DIM, HEAD_DIM, hd, nh);
-    }
-    // out_proj [H, nh * hd]: (row, head) pairs are the source rows of hd elements, 128 apart in wo [H, nh * 128]
-    if (sub == "self_attn.out_proj.weight") return copy2d(l.wo, HEAD_DIM, hd, H * nh);
-    if (sub == "self_attn.out_proj.bias") return copy(l.b_o, H);
-    if (sub == "self_attn_layer_norm.weight") return copy(l.ln1, H);
-    if (sub == "self_attn_layer_norm.bias") return copy(l.ln1_b, H);
-    if (sub == "fc1.weight") return copy(l.wgu, F * H);
-    if (sub == "fc1.bias") return copy(l.b_fc1, F);
-    if (sub == "fc2.weight") return copy(l.wd, H * F);
-    if (sub == "fc2.bias") return copy(l.b_fc2, H);
-    if (sub == "final_layer_norm.weight") return copy(l.ln2, H);
-    if (sub == "final_layer_norm.bias") return copy(l.ln2_b, H);
-    return fail("unknown layer weight " + full_name);
-  }
+  const char* layer_prefix() const { return bigcode ? "transformer.h." : opt ? "decoder.layers." : "model.layers."; }
 
-  // GPTBigCode checkpoints (HF names, "transformer." prefix).  Single GPU.  Every projection is an nn.Linear [out, in]
-  // of 128-dim heads.  c_attn's rows are q | k | v (wqkv's layout) with multi_query; multi-head checkpoints hold them
-  // head by head, [head][q | k | v] (transformers views the output as (heads, 3 * head_dim)), and are regrouped here.
-  // Every other tensor is one contiguous copy.
-  int load_weight_bigcode(const std::string& name, const void* ptr, int64_t rows, int64_t cols) {
+  // The tensors this engine accepts, under their checkpoint names.  lm_head.weight is optional (start ties it to the
+  // embedding), and so is tgis.rope_cos_sin unless the rotary embedding is scaled (default_rope_table() is unscaled).
+  // Llama family: this rank's shard -- row blocks of the column-parallel q/k/v/gate/up and lm_head, column blocks of the
+  // row-parallel o and down, everything else replicated.
+  // OPT (HF names after "decoder.", which load_weight also accepts under "model."; single GPU): q/k/v rows, out_proj
+  // columns and the q/k/v biases are spread head by head over 128-dim head slots (the upper 128 - head_dim dims of every
+  // slot stay zero: the arena was zeroed), so the attention kernels and the paged cache keep their one geometry.
+  // GPTBigCode (HF names, "transformer." prefix; single GPU): nn.Linear [out, in] of 128-dim heads.  c_attn's rows are
+  // q | k | v (wqkv's layout) with multi_query; multi-head checkpoints hold them head by head, [head][q | k | v]
+  // (transformers views the output as (heads, 3 * head_dim)), and are regrouped here.
+  void weight_table() {
     const tgis_config& c = cfg;
-    const int64_t H = c.hidden, F = c.ffn, V = c.vocab;
-    bf16* dst = nullptr;
-    int64_t n = 0;       // elements
-    int64_t c_attn = 0;  // c_attn's row width (H: weight, 1: bias), 0 for every other tensor
-    std::string key;
-    if (name == "lm_head.weight") {
-      dst = lm_head, n = V * H;
-    } else if (name.rfind("transformer.", 0) == 0) {
-      key = name.substr(12);
-      if (key == "wte.weight") dst = embed, n = V * H;
+    const size_t H = c.hidden, F = c.ffn, V = c.vocab, r = rank, qd = q_dim, kvd = (size_t)nkv * kv_head_dim, Fr = Fl;
+    auto add = [&](const std::string& name, int layer, size_t n, std::vector<WeightCopy> copies, bool required = true) {
+      wtab_at[name] = wtab.size();
+      wtab.push_back(WeightEntry{name, layer, (int64_t)n, required, false, std::move(copies)});
+    };
+    // n contiguous elements from element src_off of the source
+    auto whole = [](bf16* dst, size_t n, size_t src_off = 0) { return WeightCopy{dst, src_off, n, n, n, 1}; };
+    auto vec = [&](const std::string& name, int layer, bf16* dst, size_t n) { add(name, layer, n, {whole(dst, n)}); };
+    const std::string pre = layer_prefix();
+    if (bigcode) {
+      vec("transformer.wte.weight", -1, embed, V * H);
       // the checkpoint's table has n_positions rows: the engine keeps the max_model_len rows it can reach
-      else if (key == "wpe.weight") dst = pos_embed, n = (int64_t)pos_rows * H;
-      else if (key == "ln_f.weight") dst = final_norm, n = H;
-      else if (key == "ln_f.bias") dst = final_norm_b, n = H;
-      else if (key.rfind("h.", 0) == 0 && key.find('.', 2) != std::string::npos) {
-        const size_t dot = key.find('.', 2);
-        const int li = atoi(key.substr(2, dot - 2).c_str());
-        if (li < 0 || li >= c.n_layers) return fail("layer index out of range in " + name);
-        LayerW& l = layers[li];
-        const std::string sub = key.substr(dot + 1);
-        if (sub == "ln_1.weight") dst = l.ln1, n = H;
-        else if (sub == "ln_1.bias") dst = l.ln1_b, n = H;
-        else if (sub == "attn.c_attn.weight") dst = l.wqkv, n = (int64_t)qkv_dim * H, c_attn = H;
-        else if (sub == "attn.c_attn.bias") dst = l.b_qkv, n = qkv_dim, c_attn = 1;
-        else if (sub == "attn.c_proj.weight") dst = l.wo, n = H * q_dim;
-        else if (sub == "attn.c_proj.bias") dst = l.b_o, n = H;
-        else if (sub == "ln_2.weight") dst = l.ln2, n = H;
-        else if (sub == "ln_2.bias") dst = l.ln2_b, n = H;
-        else if (sub == "mlp.c_fc.weight") dst = l.wgu, n = F * H;
-        else if (sub == "mlp.c_fc.bias") dst = l.b_fc1, n = F;
-        else if (sub == "mlp.c_proj.weight") dst = l.wd, n = H * F;
-        else if (sub == "mlp.c_proj.bias") dst = l.b_fc2, n = H;
+      add("transformer.wpe.weight", -1, 0, {whole(pos_embed, pos_rows * H)});
+      vec("transformer.ln_f.weight", -1, final_norm, H);
+      vec("transformer.ln_f.bias", -1, final_norm_b, H);
+      add("lm_head.weight", -1, V * H, {whole(lm_head, V * H)}, false);
+      // c_attn's weight (w = H) or bias (w = 1); multi-head: per head 3 groups of 128 rows -> the q, k and v blocks
+      auto c_attn = [&](bf16* dst, size_t w) {
+        const size_t g = HEAD_DIM * w;
+        if (nkv == 1) return std::vector<WeightCopy>{whole(dst, qkv_dim * w)};
+        std::vector<WeightCopy> v;
+        for (size_t j = 0; j < 3; ++j) v.push_back({dst + j * nkv * g, j * g, 3 * g, g, g, (size_t)nkv});
+        return v;
+      };
+      for (int li = 0; li < c.n_layers; ++li) {
+        const LayerW& l = layers[li];
+        const std::string p = pre + std::to_string(li) + ".";
+        vec(p + "ln_1.weight", li, l.ln1, H);
+        vec(p + "ln_1.bias", li, l.ln1_b, H);
+        add(p + "attn.c_attn.weight", li, qkv_dim * H, c_attn(l.wqkv, H));
+        add(p + "attn.c_attn.bias", li, qkv_dim, c_attn(l.b_qkv, 1));
+        vec(p + "attn.c_proj.weight", li, l.wo, H * qd);
+        vec(p + "attn.c_proj.bias", li, l.b_o, H);
+        vec(p + "ln_2.weight", li, l.ln2, H);
+        vec(p + "ln_2.bias", li, l.ln2_b, H);
+        vec(p + "mlp.c_fc.weight", li, l.wgu, F * H);
+        vec(p + "mlp.c_fc.bias", li, l.b_fc1, F);
+        vec(p + "mlp.c_proj.weight", li, l.wd, H * F);
+        vec(p + "mlp.c_proj.bias", li, l.b_fc2, H);
+      }
+    } else if (opt) {
+      const size_t hd = model_head_dim, nh = c.n_q_heads, slot_w = HEAD_DIM * H;  // slot_w: one head slot's rows in wqkv
+      vec("decoder.embed_tokens.weight", -1, embed, V * H);
+      // the checkpoint's table covers max_position_embeddings + 2 rows; the engine keeps what max_model_len can reach
+      add("decoder.embed_positions.weight", -1, 0, {whole(pos_embed, pos_rows * H)});
+      vec("decoder.final_layer_norm.weight", -1, final_norm, H);
+      vec("decoder.final_layer_norm.bias", -1, final_norm_b, H);
+      add("lm_head.weight", -1, V * H, {whole(lm_head, V * H)}, false);
+      for (int li = 0; li < c.n_layers; ++li) {
+        const LayerW& l = layers[li];
+        const std::string p = pre + std::to_string(li) + ".";
+        for (size_t j = 0; j < 3; ++j) {
+          const std::string base = p + "self_attn." + "qkv"[j] + "_proj.";
+          // head h's hd rows of [H] -> rows [h * 128, h * 128 + hd) of the projection's block
+          add(base + "weight", li, nh * hd * H, {{l.wqkv + j * nh * slot_w, 0, hd * H, slot_w, hd * H, nh}});
+          add(base + "bias", li, nh * hd, {{l.b_qkv + j * nh * HEAD_DIM, 0, hd, HEAD_DIM, hd, nh}});
+        }
+        // out_proj [H, nh * hd]: (row, head) pairs are the source rows of hd elements, 128 apart in wo [H, nh * 128]
+        add(p + "self_attn.out_proj.weight", li, H * nh * hd, {{l.wo, 0, hd, HEAD_DIM, hd, H * nh}});
+        vec(p + "self_attn.out_proj.bias", li, l.b_o, H);
+        vec(p + "self_attn_layer_norm.weight", li, l.ln1, H);
+        vec(p + "self_attn_layer_norm.bias", li, l.ln1_b, H);
+        vec(p + "fc1.weight", li, l.wgu, F * H);
+        vec(p + "fc1.bias", li, l.b_fc1, F);
+        vec(p + "fc2.weight", li, l.wd, H * F);
+        vec(p + "fc2.bias", li, l.b_fc2, H);
+        vec(p + "final_layer_norm.weight", li, l.ln2, H);
+        vec(p + "final_layer_norm.bias", li, l.ln2_b, H);
+      }
+    } else {
+      const size_t q_rows = (size_t)c.n_q_heads * kv_head_dim, kv_rows = (size_t)c.n_kv_heads * kv_head_dim;
+      const size_t rope_n = (size_t)c.max_model_len * kv_head_dim;
+      vec("model.embed_tokens.weight", -1, embed, V * H);
+      add("lm_head.weight", -1, V * H, {whole(lm_head, Vl * H, r * Vl * H)}, false);
+      vec("model.norm.weight", -1, final_norm, H);
+      add("tgis.rope_cos_sin", -1, rope_n, {whole(cos_sin, rope_n)}, c.rope_table_from_host != 0);
+      for (int li = 0; li < c.n_layers; ++li) {
+        const LayerW& l = layers[li];
+        const std::string p = pre + std::to_string(li) + ".";
+        add(p + "self_attn.q_proj.weight", li, q_rows * H, {whole(l.wqkv, qd * H, r * qd * H)});
+        add(p + "self_attn.k_proj.weight", li, kv_rows * H, {whole(l.wqkv + qd * H, kvd * H, r * kvd * H)});
+        add(p + "self_attn.v_proj.weight", li, kv_rows * H, {whole(l.wqkv + (qd + kvd) * H, kvd * H, r * kvd * H)});
+        add(p + "self_attn.o_proj.weight", li, H * q_rows, {{l.wo, r * qd, q_rows, qd, qd, H}});
+        // gate / up rows are INTERLEAVED in wgu (row 2j = gate_j, row 2j+1 = up_j) so the GEMM epilogue can fuse SwiGLU
+        add(p + "mlp.gate_proj.weight", li, F * H, {{l.wgu, r * Fr * H, H, 2 * H, H, Fr}});
+        add(p + "mlp.up_proj.weight", li, F * H, {{l.wgu + H, r * Fr * H, H, 2 * H, H, Fr}});
+        add(p + "mlp.down_proj.weight", li, H * F, {{l.wd, r * Fr, F, Fr, Fr, H}});
+        vec(p + "input_layernorm.weight", li, l.ln1, H);
+        vec(p + "post_attention_layernorm.weight", li, l.ln2, H);
+        if (qk_norm_w.p) {
+          bf16* qn = qk_norm_w.p + (size_t)li * 2 * HEAD_DIM;
+          vec(p + "self_attn.q_norm.weight", li, qn, HEAD_DIM);
+          vec(p + "self_attn.k_norm.weight", li, qn + HEAD_DIM, HEAD_DIM);
+        }
+        if (qkv_bias_w.p) {
+          bf16* b = qkv_bias_w.p + (size_t)li * qkv_dim;
+          vec(p + "self_attn.q_proj.bias", li, b, qd);
+          vec(p + "self_attn.k_proj.bias", li, b + qd, kvd);
+          vec(p + "self_attn.v_proj.bias", li, b + qd + kvd, kvd);
+        }
       }
     }
-    if (!dst) return fail("unknown weight " + name);
-    const bool ok = dst == pos_embed ? cols == H && rows >= pos_rows : rows * cols == n;
-    if (!ok) return fail("shape mismatch for " + name + ": got " + std::to_string(rows) + "x" + std::to_string(cols));
-    cudaError_t e = cudaSuccess;
-    if (c_attn && nkv > 1) {
-      // multi-head c_attn: per head 3 groups of 128 rows (q, k, v) -> the q, k and v blocks of wqkv
-      const size_t w = (size_t)c_attn * HEAD_DIM * sizeof(bf16);  // bytes of one head's rows of one projection
-      for (int j = 0; j < 3 && e == cudaSuccess; ++j)
-        e = cudaMemcpy2D(reinterpret_cast<uint8_t*>(dst) + j * nkv * w, w, static_cast<const uint8_t*>(ptr) + j * w, 3 * w, w,
-                         nkv, cudaMemcpyDefault);
-    } else {
-      e = cudaMemcpy(dst, ptr, (size_t)n * sizeof(bf16), cudaMemcpyDefault);
-    }
-    if (e != cudaSuccess) return fail(std::string("cudaMemcpy(weight) failed: ") + cudaGetErrorString(e));
-    if (dst == lm_head) lm_head_loaded = true;
-    else opt_loaded.insert(key);
-    return 0;
   }
 
   int load_weight(const std::string& name, const void* ptr, int64_t rows, int64_t cols) {
-    if (bigcode) return load_weight_bigcode(name, ptr, rows, cols);
-    if (opt) return load_weight_opt(name, ptr, rows, cols);
-    const tgis_config& c = cfg;
-    const int64_t H = c.hidden, F = c.ffn, V = c.vocab;
-    const uint8_t* src = static_cast<const uint8_t*>(ptr);
-    bf16* dst = nullptr;
-    int64_t er = 0, ec = 0;             // expected full shape
-    int64_t r0 = 0, nr = 0, c0 = 0, nc = 0;  // shard = rows [r0, r0+nr) x cols [c0, c0+nc)
-    int interleave = 0;                      // destination row stride 2 (gate/up pairs)
-    auto rows_shard = [&](bf16* d, int64_t full_rows, int64_t full_cols, int64_t per_rank) {
-      dst = d; er = full_rows; ec = full_cols; r0 = rank * per_rank; nr = per_rank; c0 = 0; nc = full_cols;
-    };
-    auto cols_shard = [&](bf16* d, int64_t full_rows, int64_t full_cols, int64_t per_rank) {
-      dst = d; er = full_rows; ec = full_cols; r0 = 0; nr = full_rows; c0 = rank * per_rank; nc = per_rank;
-    };
-    auto full = [&](bf16* d, int64_t full_rows, int64_t full_cols) {
-      dst = d; er = full_rows; ec = full_cols; r0 = 0; nr = full_rows; c0 = 0; nc = full_cols;
-    };
-    if (name == "model.embed_tokens.weight") full(embed, V, H);
-    else if (name == "lm_head.weight") { rows_shard(lm_head, V, H, Vl); lm_head_loaded = true; }
-    else if (name == "model.norm.weight") full(final_norm, H, 1);
-    else if (name == "tgis.rope_cos_sin") { full(cos_sin, c.max_model_len, kv_head_dim); cos_sin_loaded = true; }
-    else if (name.rfind("model.layers.", 0) == 0) {
-      const size_t dot = name.find('.', 13);
-      if (dot == std::string::npos) return fail("bad weight name " + name);
-      const int li = atoi(name.substr(13, dot - 13).c_str());
-      if (li < 0 || li >= c.n_layers) return fail("layer index out of range in " + name);
-      LayerW& l = layers[li];
-      const std::string sub = name.substr(dot + 1);
-      const int64_t kvd = (int64_t)nkv * kv_head_dim;  // local
-      if (sub == "self_attn.q_proj.weight") rows_shard(l.wqkv, (int64_t)c.n_q_heads * kv_head_dim, H, q_dim);
-      else if (sub == "self_attn.k_proj.weight") rows_shard(l.wqkv + (size_t)q_dim * H, (int64_t)c.n_kv_heads * kv_head_dim, H, kvd);
-      else if (sub == "self_attn.v_proj.weight") rows_shard(l.wqkv + (size_t)(q_dim + kvd) * H, (int64_t)c.n_kv_heads * kv_head_dim, H, kvd);
-      else if (sub == "self_attn.o_proj.weight") cols_shard(l.wo, H, (int64_t)c.n_q_heads * kv_head_dim, q_dim);
-      // gate / up rows are INTERLEAVED in wgu (row 2j = gate_j, row 2j+1 = up_j) so the GEMM epilogue can fuse SwiGLU
-      else if (sub == "mlp.gate_proj.weight") { rows_shard(l.wgu, F, H, Fl); interleave = 1; }
-      else if (sub == "mlp.up_proj.weight") { rows_shard(l.wgu + H, F, H, Fl); interleave = 1; }
-      else if (sub == "mlp.down_proj.weight") cols_shard(l.wd, H, F, Fl);
-      else if (sub == "input_layernorm.weight") full(l.ln1, H, 1);
-      else if (sub == "post_attention_layernorm.weight") full(l.ln2, H, 1);
-      else if (qk_norm_w.p && (sub == "self_attn.q_norm.weight" || sub == "self_attn.k_norm.weight")) {
-        const int k = sub[10] == 'k';
-        full(qk_norm_w.p + (size_t)li * 2 * HEAD_DIM + k * HEAD_DIM, HEAD_DIM, 1);
-        if (rows * cols == HEAD_DIM) qk_norm_loaded[li] |= 1 << k;
-      }
-      else if (qkv_bias_w.p && (sub == "self_attn.q_proj.bias" || sub == "self_attn.k_proj.bias" ||
-                                sub == "self_attn.v_proj.bias")) {
-        const int k = sub[10] == 'q' ? 0 : sub[10] == 'k' ? 1 : 2;
-        const int64_t n = k == 0 ? q_dim : kvd;
-        full(qkv_bias_w.p + (size_t)li * qkv_dim + (k == 0 ? 0 : q_dim + (k - 1) * kvd), n, 1);
-        if (rows * cols == n) qkv_bias_loaded[li] |= 1 << k;
-      }
-      else return fail("unknown layer weight " + name);
-    } else {
-      return fail("unknown weight " + name);
+    const std::string key = opt && !bigcode && name.rfind("model.", 0) == 0 ? name.substr(6) : name;
+    const auto it = wtab_at.find(key);
+    if (it == wtab_at.end())
+      return fail((key.rfind(layer_prefix(), 0) == 0 ? "unknown layer weight " : "unknown weight ") + name);
+    WeightEntry& e = wtab[it->second];
+    if (e.n ? rows * cols != e.n : cols != cfg.hidden || rows < pos_rows)
+      return fail("shape mismatch for " + name + ": got " + std::to_string(rows) + "x" + std::to_string(cols) + " expected " +
+                  (e.n ? std::to_string(e.n) + " elements" : ">= " + std::to_string(pos_rows) + " rows of " +
+                                                                 std::to_string(cfg.hidden)));
+    e.loaded = false;
+    for (const WeightCopy& w : e.copies) {
+      const bf16* src = static_cast<const bf16*>(ptr) + w.src_off;
+      const cudaError_t err =
+          w.spitch == w.width && w.dpitch == w.width
+              ? cudaMemcpy(w.dst, src, w.width * w.height * sizeof(bf16), cudaMemcpyDefault)
+              : cudaMemcpy2D(w.dst, w.dpitch * sizeof(bf16), src, w.spitch * sizeof(bf16), w.width * sizeof(bf16), w.height,
+                             cudaMemcpyDefault);
+      if (err != cudaSuccess) return fail(std::string("cudaMemcpy(weight) failed: ") + cudaGetErrorString(err));
     }
-    if (rows * cols != er * ec) return fail("shape mismatch for " + name + ": got " + std::to_string(rows) + "x" +
-                                            std::to_string(cols) + " expected " + std::to_string(er) + "x" + std::to_string(ec));
-    cudaError_t e;
-    if (interleave) {
-      e = cudaMemcpy2D(dst, (size_t)2 * ec * sizeof(bf16), src + (size_t)r0 * ec * sizeof(bf16), (size_t)ec * sizeof(bf16),
-                       (size_t)ec * sizeof(bf16), (size_t)nr, cudaMemcpyDefault);
-    } else if (nc == ec) {
-      e = cudaMemcpy(dst, src + (size_t)r0 * ec * sizeof(bf16), (size_t)(nr * ec) * sizeof(bf16), cudaMemcpyDefault);
-    } else {
-      e = cudaMemcpy2D(dst, (size_t)nc * sizeof(bf16), src + (size_t)c0 * sizeof(bf16), (size_t)ec * sizeof(bf16),
-                       (size_t)nc * sizeof(bf16), (size_t)nr, cudaMemcpyDefault);
-    }
-    if (e != cudaSuccess) return fail(std::string("cudaMemcpy(weight) failed: ") + cudaGetErrorString(e));
+    e.loaded = true;
     return 0;
   }
 
@@ -1120,15 +1071,15 @@ struct tgis_engine {
   }
   template <class Fn>
   void lora_for_each(int32_t slot, Fn fn) {
-    const size_t R = lora_R, H = cfg.hidden, F = Fl, kvd = (size_t)nkv * kv_head_dim, s = (size_t)(slot - 1);
-    for (auto& ll : lora_layers) {
-      fn(ll.A_q + s * R * H, R * H);              fn(ll.B_q + s * q_dim * R, (size_t)q_dim * R);
-      fn(ll.A_k + s * R * H, R * H);              fn(ll.B_k + s * kvd * R, kvd * R);
-      fn(ll.A_v + s * R * H, R * H);              fn(ll.B_v + s * kvd * R, kvd * R);
-      fn(ll.A_o + s * R * q_dim, R * q_dim);      fn(ll.B_o + s * H * R, H * R);
-      fn(ll.A_gu + s * 2 * R * H, 2 * R * H);     fn(ll.B_gu + s * 2 * F * 2 * R, 2 * F * 2 * R);
-      fn(ll.A_d + s * R * F, R * F);              fn(ll.B_d + s * H * R, H * R);
-    }
+    const size_t s = slot - 1;
+    for (auto& gs : lora_groups)
+      for (const LoraGroup& g : gs)
+        for (int m = 0; m < g.n_mods; ++m) {
+          const LoraModule& md = g.mod[m];
+          const size_t a = (size_t)md.Rm * md.K, b = (size_t)md.N * md.Rm;
+          fn(const_cast<bf16*>(md.A) + s * a, a);
+          fn(const_cast<bf16*>(md.B) + s * b, b);
+        }
   }
   int clear_adapter(int32_t slot) {
     if (int rc = lora_slot_check(slot)) return rc;
@@ -1152,24 +1103,22 @@ struct tgis_engine {
     const std::string mod = rest.substr(0, dot2), which = rest.substr(dot2 + 1);
     if (which != "lora_A" && which != "lora_B") return fail("bad adapter weight name " + name);
     const bool isA = which == "lora_A";
-    const int64_t R = lora_R, H = cfg.hidden, F = Fl, kvd = (int64_t)nkv * kv_head_dim, s = slot - 1;
-    LoraLayerW& ll = lora_layers[li];
-    bf16* dst = nullptr;
-    int64_t fin = 0, fout = 0, cap = R;   // module geometry; cap: rank capacity of the stored tensor (row length of B)
-    int64_t b_row_stride = 0;             // B: destination elements between consecutive source rows
-    if (mod == "q_proj") { fin = H; fout = q_dim; dst = isA ? ll.A_q + s * R * H : ll.B_q + s * q_dim * R; }
-    else if (mod == "k_proj") { fin = H; fout = kvd; dst = isA ? ll.A_k + s * R * H : ll.B_k + s * kvd * R; }
-    else if (mod == "v_proj") { fin = H; fout = kvd; dst = isA ? ll.A_v + s * R * H : ll.B_v + s * kvd * R; }
-    else if (mod == "o_proj") { fin = q_dim; fout = H; dst = isA ? ll.A_o + s * R * q_dim : ll.B_o + s * H * R; }
-    else if (mod == "down_proj") { fin = F; fout = H; dst = isA ? ll.A_d + s * R * F : ll.B_d + s * H * R; }
-    else if (mod == "gate_proj" || mod == "up_proj") {
-      // one module of capacity 2R over the interleaved projection: A rows [0, R) gate / [R, 2R) up; B row 2j = gate_j
-      // (columns [0, R)), row 2j + 1 = up_j (columns [R, 2R))
-      const bool up = mod == "up_proj";
-      fin = H; fout = F; cap = 2 * R;
-      if (isA) dst = ll.A_gu + s * 2 * R * H + (up ? R * H : 0);
-      else { dst = ll.B_gu + s * 2 * F * 2 * R + (up ? 2 * R + R : 0); b_row_stride = 2 * cap; }
-    } else return fail("unsupported LoRA module " + mod);
+    static const struct {
+      const char* name;
+      int group, module;
+    } modules[] = {{"q_proj", LORA_QKV, 0},       {"k_proj", LORA_QKV, 1},     {"v_proj", LORA_QKV, 2},
+                   {"o_proj", LORA_O, 0},         {"gate_proj", LORA_GATE_UP, 0}, {"up_proj", LORA_GATE_UP, 0},
+                   {"down_proj", LORA_DOWN, 0}};
+    const auto* mi = std::find_if(std::begin(modules), std::end(modules), [&](const auto& m) { return mod == m.name; });
+    if (mi == std::end(modules)) return fail("unsupported LoRA module " + mod);
+    const LoraModule& md = lora_groups[li][mi->group].mod[mi->module];
+    // gate_proj / up_proj are the halves of one module of capacity 2R over the interleaved projection: A rows [0, R) gate
+    // / [R, 2R) up; B row 2j = gate_j (columns [0, R)), row 2j + 1 = up_j (columns [R, 2R))
+    const bool half = mi->group == LORA_GATE_UP, up = mod == "up_proj";
+    const int64_t R = lora_R, s = slot - 1, fin = md.K, fout = half ? md.N / 2 : md.N;
+    bf16* dst = const_cast<bf16*>(isA ? md.A + s * md.Rm * md.K + (up ? R * md.K : 0)
+                                      : md.B + s * md.N * md.Rm + (up ? md.Rm + R : 0));
+    const int64_t b_row_stride = half ? 2 * md.Rm : md.Rm;  // B: destination elements between consecutive source rows
     const int64_t r = isA ? rows : cols;
     if (r < 1 || r > R) return fail("adapter rank " + std::to_string(r) + " exceeds max_lora_rank " + std::to_string(R));
     if (isA ? cols != fin : rows != fout)
@@ -1178,7 +1127,6 @@ struct tgis_engine {
     if (isA) {
       CK(cudaMemcpy(dst, ptr, (size_t)(rows * cols) * sizeof(bf16), cudaMemcpyDefault));
     } else {
-      if (b_row_stride == 0) b_row_stride = cap;
       CK(cudaMemcpy2D(dst, (size_t)b_row_stride * sizeof(bf16), ptr, (size_t)cols * sizeof(bf16), (size_t)cols * sizeof(bf16),
                       (size_t)rows, cudaMemcpyDefault));
     }
@@ -1186,36 +1134,29 @@ struct tgis_engine {
     return 0;
   }
 
+  // A checkpoint with a tensor missing must not come up healthy on whatever the arena holds.
   void finalize_weights() {
-    if (bigcode) {
-      const size_t expected = 4 + (size_t)12 * cfg.n_layers;
-      if (opt_loaded.size() < expected)
-        throw CudaError("GPTBigCode checkpoint incomplete: " + std::to_string(opt_loaded.size()) + " of " +
-                        std::to_string(expected) + " tensors loaded (wte, wpe, ln_f.{weight,bias} and 12 per layer)");
-    } else if (opt) {
-      // an OPT checkpoint with a tensor missing must not come up healthy on zeros (the reference's engine fails the load)
-      const size_t expected = 4 + (size_t)16 * cfg.n_layers;
-      if (opt_loaded.size() < expected)
-        throw CudaError("OPT checkpoint incomplete: " + std::to_string(opt_loaded.size()) + " of " + std::to_string(expected) +
-                        " tensors loaded (embed_tokens, embed_positions, final_layer_norm.{weight,bias} and 16 per layer)");
-    }
-    if (rope_table_required && !cos_sin_loaded)
-      throw CudaError("this model's rotary embedding is scaled (rope_scaling): load its table as tgis.rope_cos_sin before "
-                      "starting; the built-in table is the unscaled one");
-    for (size_t li = 0; li < qk_norm_loaded.size(); ++li)
-      if (qk_norm_loaded[li] != 3)
-        throw CudaError("q/k norm (Qwen3) weights missing: layer " + std::to_string(li) + " has no " +
-                        (qk_norm_loaded[li] & 1 ? "" : "model.layers." + std::to_string(li) + ".self_attn.q_norm.weight ") +
-                        (qk_norm_loaded[li] & 2 ? "" : "model.layers." + std::to_string(li) + ".self_attn.k_norm.weight"));
-    for (size_t li = 0; li < qkv_bias_loaded.size(); ++li)
-      if (qkv_bias_loaded[li] != 7) {
-        std::string missing;
-        for (int k = 0; k < 3; ++k)
-          if (!(qkv_bias_loaded[li] & (1 << k)))
-            missing += " model.layers." + std::to_string(li) + ".self_attn." + "qkv"[k] + "_proj.bias";
-        throw CudaError("qkv bias (Qwen2) missing: layer " + std::to_string(li) + " has no" + missing);
+    constexpr int64_t listed = 8;  // missing tensors named in the message
+    int64_t n = 0, k = 0;
+    std::string missing;
+    for (const WeightEntry& e : wtab) {
+      if (!e.required) continue;
+      ++n;
+      if (e.loaded) {
+        ++k;
+        continue;
       }
-    if (!lm_head_loaded)  // tie_word_embeddings (tp == 1: with the zero padding rows)
+      if (e.name == "tgis.rope_cos_sin")
+        throw CudaError("this model's rotary embedding is scaled (rope_scaling): load its table as tgis.rope_cos_sin "
+                        "before starting; the built-in table is the unscaled one");
+      if (n - k <= listed)
+        missing += (e.layer >= 0 ? "; layer " + std::to_string(e.layer) + " has no " : std::string("; no ")) + e.name;
+    }
+    if (k < n)
+      throw CudaError(std::string(bigcode ? "GPTBigCode" : opt ? "OPT" : "Llama-family") + " checkpoint incomplete: " +
+                      std::to_string(k) + " of " + std::to_string(n) + " tensors loaded" + missing +
+                      (n - k > listed ? "; ..." : ""));
+    if (!wtab[wtab_at.at("lm_head.weight")].loaded)  // tie_word_embeddings (tp == 1: with the zero padding rows)
       CK(cudaMemcpy(lm_head, embed + (size_t)rank * Vl * cfg.hidden, (size_t)(tp == 1 ? Vpad : Vl) * cfg.hidden * sizeof(bf16),
                     cudaMemcpyDeviceToDevice));
   }
@@ -1322,7 +1263,6 @@ struct tgis_engine {
     const bool lora = (samp_complex & 4) != 0 && max_loras > 0;
     const int32_t* d_toklora = ds<int32_t>(off_toklora);
     const int32_t* d_lorarow = ds<int32_t>(off_lorarow);
-    const int LR = lora_R, kvd = nkv * kv_head_dim;
     auto lora_apply = [&](const LoraGroup& g, const bf16* x, int ldx, bf16* y, int ldy) {
       CK(lora_shrink_launch(x, ldx, d_toklora, d_lorarow, g, lora_v.p, T, stream));
       CK(lora_expand_launch(lora_v.p, d_toklora, d_lorarow, g, y, ldy, T, stream));
@@ -1359,16 +1299,7 @@ struct tgis_engine {
           CK(opt_bias_act_launch(y32.p, qkv_dim, qb, qkv.p, qkv_dim, T, qkv_dim, ACT_NONE, num_sms, stream));
           ++n_launches;
         }
-        if (lora) {
-          const LoraLayerW& ll = lora_layers[li];
-          LoraGroup g{};
-          g.n_mods = 3;
-          g.v_ld = 3 * LR;
-          g.mod[0] = LoraModule{ll.A_q, ll.B_q, H, q_dim, LR, 0, 0};
-          g.mod[1] = LoraModule{ll.A_k, ll.B_k, H, kvd, LR, q_dim, LR};
-          g.mod[2] = LoraModule{ll.A_v, ll.B_v, H, kvd, LR, q_dim + kvd, 2 * LR};
-          lora_apply(g, xn.p, H, qkv.p, qkv_dim);
-        }
+        if (lora) lora_apply(lora_groups[li][LORA_QKV], xn.p, H, qkv.p, qkv_dim);
       }
       bf16* kc = k_cache.p + (size_t)li * kv_layer_elems;
       bf16* vc = v_cache.p + (size_t)li * kv_layer_elems;
@@ -1392,13 +1323,7 @@ struct tgis_engine {
       }
       if (n_tiles > 0) prefill_attention(kc, vc, scale, n_tiles);
       gemm(xm_attn, l.m_o, attn_out.p, l.wo, ar_fused ? ar_buf(0) : tmp.p, T, H, q_dim);
-      if (lora) {
-        LoraGroup g{};
-        g.n_mods = 1;
-        g.v_ld = 3 * LR;
-        g.mod[0] = LoraModule{lora_layers[li].A_o, lora_layers[li].B_o, q_dim, H, LR, 0, 0};
-        lora_apply(g, attn_out.p, q_dim, tmp.p, H);
-      }
+      if (lora) lora_apply(lora_groups[li][LORA_O], attn_out.p, q_dim, tmp.p, H);
       if (ar_fused) {
         fused_ar_norm(0, l.ln2, T);
       } else {
@@ -1410,24 +1335,14 @@ struct tgis_engine {
       if (lora) {
         // raw interleaved gate_up -> + adapter deltas (gate and up as one module of capacity 2R) -> SwiGLU
         gemm(xm_xn, l.m_gu, xn.p, l.wgu, gu_buf.p, T, 2 * F, H, /*out_mode=*/0, /*ldy=*/2 * F);
-        LoraGroup g{};
-        g.n_mods = 1;
-        g.v_ld = 3 * LR;
-        g.mod[0] = LoraModule{lora_layers[li].A_gu, lora_layers[li].B_gu, H, 2 * F, 2 * LR, 0, 0};
-        lora_apply(g, xn.p, H, gu_buf.p, 2 * F);
+        lora_apply(lora_groups[li][LORA_GATE_UP], xn.p, H, gu_buf.p, 2 * F);
         CK(silu_mul_interleaved_launch(gu_buf.p, act.p, T, F, stream));
         ++n_launches;
       } else
       gemm(xm_xn, l.m_gu, xn.p, l.wgu, act.p, T, 2 * F, H, /*out_mode=*/2, /*ldy=*/F);
       bf16* down_out = ar_fused ? ar_buf(1) : tmp.p;
       gemm(xm_act, l.m_d, act.p, l.wd, down_out, T, H, F);
-      if (lora) {
-        LoraGroup g{};
-        g.n_mods = 1;
-        g.v_ld = 3 * LR;
-        g.mod[0] = LoraModule{lora_layers[li].A_d, lora_layers[li].B_d, F, H, LR, 0, 0};
-        lora_apply(g, act.p, F, down_out, H);
-      }
+      if (lora) lora_apply(lora_groups[li][LORA_DOWN], act.p, F, down_out, H);
       if (!ar_fused) all_reduce_tmp(T);
     }
     // The last down-proj exchange is run even when no row is sampled this step (R == 0): it is what guarantees that
