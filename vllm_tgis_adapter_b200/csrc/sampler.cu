@@ -591,6 +591,9 @@ tgis_sampler_kernel(const LT* __restrict__ logits, int ld, int V, const SampleRo
     }
     ms = am;
     token = ab.i;
+    if constexpr (MASKED) {
+      if (c.allow != nullptr && ab.v == -INFINITY) token = -1;  // every allowed token removed: see below
+    }
   } else {
     ms = cluster_maxsum(cl, ms, redf, xch);
     token = -1;
@@ -632,6 +635,23 @@ tgis_sampler_kernel(const LT* __restrict__ logits, int ld, int V, const SampleRo
       }
       best = cluster_argmax(cl, best, redf, redi, xch);
       token = best.i;
+      if constexpr (MASKED) {
+        if (c.allow != nullptr && best.v == -INFINITY) token = -1;
+      }
+    }
+    // Every allowed token removed (e.g. a mask that allows only EOS before min_tokens): an argmax over all -inf keeps
+    // the first index, which the mask may have cleared.  Such a row takes the sampling rows' fallback below instead --
+    // the largest raw (masked) logit, lowest index on ties -- so it returns an allowed token (vLLM returns token 0).
+    // Only in this instantiation: launches without guided rows keep their instructions.
+    if constexpr (MASKED) {
+      if (token < 0) {
+        ValIdx b2{-INFINITY, -1};
+        for (int i = lo + threadIdx.x; i < hi; i += SAMP_THREADS) {
+          const float v = load_x(c, i);
+          if (b2.i < 0 || v > b2.v) b2 = {v, i};
+        }
+        token = cluster_argmax(cl, b2, redf, redi, xch).i;
+      }
     }
   } else {
     // ---- processed logits / temperature -> scratch, running max
