@@ -37,11 +37,9 @@ def test_residual_multiplier_norm_is_bit_exact(g, T, H):
     assert g.lib().tgis_k_rmsnorm_mult(g.ptr(x), g.ptr(r), g.ptr(w), g.ptr(out), T, H, eps, m) == 0, g.kerr()
     # residual: bf16(r + bf16(x * m)), two roundings (bf16 torch ops)
     assert torch.equal(r, r0 + x * m)
-    # the norm that follows is the existing kernel's, on the pre-scaled input
-    r2, out2 = r0.clone(), torch.empty_like(out)
-    xs = (x * m).contiguous()
-    assert g.lib().tgis_k_rmsnorm(g.ptr(xs), g.ptr(r2), g.ptr(w), g.ptr(out2), T, H, eps) == 0, g.kerr()
-    assert torch.equal(r, r2) and torch.equal(out, out2)
+    # the norm that follows: rmsnorm_kernel's summation order and rounding points, bit for bit
+    want, z = g.rmsnorm_restated(x, w, eps, residual=r0, mult=m)
+    assert torch.equal(r, z) and torch.equal(out, want)
     # m = 1 is tgis_k_rmsnorm bit for bit
     r3, out3 = r0.clone(), torch.empty_like(out)
     r4, out4 = r0.clone(), torch.empty_like(out)

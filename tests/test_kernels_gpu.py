@@ -2,7 +2,8 @@
 
 Tolerances (written here, per the task contract):
   * integer / index results (greedy token ids, ranks, top-n ids, KV-cache placement, RoPE bits): bit-exact
-  * bf16 tensor results whose fp32 accumulation ORDER differs from the oracle's (GEMM, RMSNorm): <= 1 bf16 ulp per element
+  * bf16 tensor results whose fp32 accumulation ORDER differs from the oracle's (GEMM): <= 1 bf16 ulp per element
+  * RMSNorm and SiLU * mul: bit-exact (RMSNorm against tgis_gpu_utils.rmsnorm_restated, its summation order)
   * attention (both kernels feed P to the tensor cores as bf16 hi + lo): against a float64 softmax from the same bf16
     inputs, <= 1 bf16 ulp per element or <= 2^-16 of the row's largest output, and >= 99 % bit-exact
     (tgis_gpu_utils.attention_bar; tests/test_attention_precision_gpu.py runs the same bar at serving shapes)
@@ -108,30 +109,24 @@ def test_gemm_crosscheck_kernel_agrees(g):
 
 @pytest.mark.parametrize("T,H", [(1, 256), (5, 768), (32, 4096), (17, 8192)])
 def test_rmsnorm_and_fused_add(g, T, H):
-    from oracle.llama_oracle import CONFIGS, LlamaOracle
-
     torch.manual_seed(T + H)
-    x = torch.randn(T, H).bfloat16()
-    r = torch.randn(T, H).bfloat16()
-    w = (1 + 0.1 * torch.randn(H)).bfloat16()
+    x = torch.randn(T, H).bfloat16().cuda()
+    r = torch.randn(T, H).bfloat16().cuda()
+    w = (1 + 0.1 * torch.randn(H)).bfloat16().cuda()
     eps = 1e-5
-
-    def rms(z):
-        zf = z.float()
-        return w * (zf * torch.rsqrt(zf.pow(2).mean(-1, keepdim=True) + eps)).bfloat16()
-
     out = torch.empty(T, H, dtype=torch.bfloat16, device="cuda")
-    xc, wc = x.cuda(), w.cuda()
-    assert g.lib().tgis_k_rmsnorm(g.ptr(xc), None, g.ptr(wc), g.ptr(out), T, H, eps) == 0, g.kerr()
-    assert float(g.bf16_ulp_diff(out.cpu(), rms(x)).max()) <= 1.0
-    rc = r.cuda().clone()
-    assert g.lib().tgis_k_rmsnorm(g.ptr(xc), g.ptr(rc), g.ptr(wc), g.ptr(out), T, H, eps) == 0, g.kerr()
-    z = x + r  # bf16 add = fp32 add rounded to bf16 (vllm layernorm_kernels.cu: add in scalar_t)
-    assert torch.equal(rc.cpu(), z)
-    assert float(g.bf16_ulp_diff(out.cpu(), rms(z)).max()) <= 1.0
+    assert g.lib().tgis_k_rmsnorm(g.ptr(x), None, g.ptr(w), g.ptr(out), T, H, eps) == 0, g.kerr()
+    assert torch.equal(out, g.rmsnorm_restated(x, w, eps)[0])
+    rc = r.clone()
+    assert g.lib().tgis_k_rmsnorm(g.ptr(x), g.ptr(rc), g.ptr(w), g.ptr(out), T, H, eps) == 0, g.kerr()
+    want, z = g.rmsnorm_restated(x, w, eps, residual=r)
+    assert torch.equal(z, x + r)  # bf16 add = fp32 add rounded to bf16 (vllm layernorm_kernels.cu: add in scalar_t)
+    assert torch.equal(rc, z)
+    assert torch.equal(out, want)
 
 
 def test_silu_mul(g):
+    """bf16(bf16(silu(gate)) * up), the rounding points of bf16 torch ops (vllm activation_kernels.cu)"""
     torch.manual_seed(3)
     T, F = 9, 1536
     gu = (torch.randn(T, 2 * F) * 2).bfloat16()
@@ -139,9 +134,7 @@ def test_silu_mul(g):
     act = torch.empty(T, F, dtype=torch.bfloat16, device="cuda")
     guc = gu.cuda()
     assert g.lib().tgis_k_silu_mul(g.ptr(guc), g.ptr(act), T, F) == 0, g.kerr()
-    ulp = g.bf16_ulp_diff(act.cpu(), ref)
-    assert float(ulp.max()) <= 1.0
-    assert float((ulp == 0).float().mean()) > 0.995
+    assert torch.equal(act.cpu(), ref), int((act.cpu() != ref).sum())
 
 
 def test_rope_and_kv_scatter_bit_exact(g):

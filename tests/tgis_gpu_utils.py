@@ -64,6 +64,134 @@ def bf16_ulp_diff(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return (a32 - b32).abs() / ulp
 
 
+# ------------------------------------------------------------------------------ RMSNorm / LayerNorm restatements
+# The summation order of rmsnorm_kernel (csrc/elementwise.cu) and opt_layernorm_kernel (csrc/opt.cu) restated with fp32
+# torch ops on the device, so that the kernels can be compared with torch.equal.  On the device torch.rsqrt is the
+# kernels' rsqrtf, and the division by a 0-dim CUDA tensor is IEEE division like the kernels' (torch divides by a Python
+# number by multiplying with its reciprocal, which is not the same for widths that are not powers of two).
+NORM_THREADS = 256
+
+
+def rmsnorm_vectors(hidden: int) -> int:
+    """NORM_MAX_VEC of the rmsnorm_kernel instantiation rmsnorm_launch picks: 16-byte vectors per thread"""
+    return 1 if hidden <= NORM_THREADS * 8 else 2 if hidden <= NORM_THREADS * 16 else 4
+
+
+def layernorm_geometry(hidden: int) -> tuple[int, int]:
+    """(LN_THREADS, LN_MAX_VEC) of the opt_layernorm_kernel instantiation opt_layernorm_launch picks"""
+    if hidden <= 1024:
+        return 128, 1
+    return (256, 1) if hidden <= 2048 else (256, 2) if hidden <= 4096 else (256, 4)
+
+
+def norm_slices(v: torch.Tensor, threads: int, nvec: int) -> list[torch.Tensor]:
+    """v [T, H] -> the [T, threads] slices in the order every thread visits its elements: thread tid owns the 8-element
+    vectors i = tid + threads * j (j < nvec) and goes through them j by j, element by element.  Past H: zeros."""
+    T, H = v.shape
+    pad = torch.zeros(T, nvec * threads * 8, dtype=v.dtype, device=v.device)
+    pad[:, :H] = v
+    p = pad.view(T, nvec, threads, 8)
+    return [p[:, j, :, e] for j in range(nvec) for e in range(8)]
+
+
+def _xor_butterfly(v: torch.Tensor) -> torch.Tensor:
+    """[..., 32] lanes -> [...]: v += shfl_xor(v, o) for o = 16, 8, 4, 2, 1 (every lane ends with the same sum)"""
+    while v.shape[-1] > 1:
+        h = v.shape[-1] // 2
+        v = v[..., :h] + v[..., h:]
+    return v[..., 0]
+
+
+def norm_block_sum(partials: torch.Tensor) -> torch.Tensor:
+    """block_sum / bsum: [T, threads] per-thread fp32 partials -> [T].  Each warp's butterfly; the warp sums in lanes
+    0 .. threads / 32 - 1 and zeros in the other lanes; the same butterfly over those 32 lanes."""
+    T, threads = partials.shape
+    lanes = torch.zeros(T, 32, dtype=torch.float32, device=partials.device)
+    lanes[:, :threads // 32] = _xor_butterfly(partials.view(T, threads // 32, 32))
+    return _xor_butterfly(lanes)
+
+
+def f32(x: float, like: torch.Tensor) -> torch.Tensor:
+    """x as a 0-dim fp32 tensor on like's device (an operand, not a Python scalar: see above)"""
+    return torch.tensor(x, dtype=torch.float32, device=like.device)
+
+
+def rmsnorm_sum_of_squares(z: torch.Tensor) -> torch.Tensor:
+    """z [T, H] bf16 -> rmsnorm_kernel's fp32 sum of squares [T].  Each thread adds its squares to 0 one at a time; a
+    bf16 square is exact in fp32, so the kernel's fused multiply-add rounds like this multiply then add."""
+    zf = z.float()
+    sq = zf * zf
+    s = torch.zeros(z.shape[0], NORM_THREADS, dtype=torch.float32, device=z.device)
+    for part in norm_slices(sq, NORM_THREADS, rmsnorm_vectors(z.shape[1])):
+        s = s + part
+    return norm_block_sum(s)
+
+
+def rmsnorm_restated(x: torch.Tensor, w: torch.Tensor, eps: float, residual: torch.Tensor | None = None,
+                     mult: float = 1.0, divisor: int | None = None) -> tuple[torch.Tensor, torch.Tensor | None]:
+    """rmsnorm_kernel<ADD, NORM_MAX_VEC, MULT> in torch.  x [T, H] bf16, w [H] bf16.  With a residual (ADD):
+    z = bf16(bf16(x * m) + r) for m != 1, else bf16(x + r); without: z = x.  Then rs = rsqrt(sum of squares / H + eps)
+    and out = bf16(bf16(z * rs) * w).  Returns (out, z): z is what ADD writes back to the residual (None without).
+    divisor replaces H (the tests' mutants)."""
+    if residual is not None:
+        xf = x.float()
+        if mult != 1.0:
+            xf = (xf * f32(mult, x)).bfloat16().float()
+        z = (xf + residual.float()).bfloat16()
+    else:
+        z = x
+    n = f32(divisor or z.shape[1], z)
+    rs = torch.rsqrt(rmsnorm_sum_of_squares(z) / n + f32(eps, z))
+    out = ((z.float() * rs[:, None]).bfloat16().float() * w.float()).bfloat16()
+    return out, (z if residual is not None else None)
+
+
+def fma_f32(a: torch.Tensor, b: torch.Tensor, c: torch.Tensor) -> torch.Tensor:
+    """fp32 a * b + c rounded once, as an FFMA does.  The product of two fp32 values is exact in float64; the float64
+    sum's own rounding error is recovered (TwoSum) and decides the rounding where that sum lies exactly halfway between
+    two fp32 values (rounding it to fp32 as it stands would round twice)."""
+    p, cd = a.double() * b.double(), c.double()
+    s = p + cd
+    bv = s - p
+    err = (p - (s - bv)) + (cd - bv)
+    f = s.float()
+    inf = torch.full_like(f, float("inf"))
+    other = torch.nextafter(f, torch.where(s > f.double(), inf, -inf))      # the fp32 neighbour on s's side of f
+    tie = (s == (f.double() + other.double()) * 0.5) & (err != 0)
+    dinf = torch.full_like(s, float("inf"))
+    s = torch.where(tie, torch.nextafter(s, torch.where(err > 0, dinf, -dinf)), s)
+    return s.float()
+
+
+def layernorm_restated(resid: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float,
+                       acc: torch.Tensor | None = None, acc_bias: torch.Tensor | None = None,
+                       var_divisor: int | None = None) -> tuple[torch.Tensor, torch.Tensor | None]:
+    """opt_layernorm_kernel<ADD, LN_THREADS, LN_MAX_VEC> in torch.  resid [T, H] bf16, w / b [H] bf16.  With acc (ADD;
+    fp32 [T, H], acc_bias [H] bf16): z = bf16(r + bf16(acc + acc_bias)); without: z = resid.  Thread partials as
+    norm_slices, summed with norm_block_sum: mean = sum(z) / H; q += d * d with d = z - mean (an FFMA: fma_f32);
+    rstd = rsqrt(sum(q) / H + eps); out = bf16(fma(d * rstd, w, b)).  Returns (out, z if ADD else None).
+    var_divisor replaces H in the variance (the tests' mutants)."""
+    T, H = resid.shape
+    threads, nvec = layernorm_geometry(H)
+    if acc is not None:
+        z = (resid.float() + (acc + acc_bias.float()).bfloat16().float()).bfloat16()
+    else:
+        z = resid
+    zf = z.float()
+    n = f32(H, zf)
+    s = torch.zeros(T, threads, dtype=torch.float32, device=z.device)
+    for part in norm_slices(zf, threads, nvec):
+        s = s + part
+    mean = norm_block_sum(s) / n
+    d = zf - mean[:, None]
+    q = torch.zeros_like(s)
+    for part in norm_slices(d, threads, nvec):      # past H: d = 0, and fma(0, 0, q) = q
+        q = fma_f32(part, part, q)
+    rstd = torch.rsqrt(norm_block_sum(q) / f32(var_divisor or H, zf) + f32(eps, zf))
+    out = fma_f32(d * rstd[:, None], w.float().expand(T, H), b.float().expand(T, H)).bfloat16()
+    return out, (z if acc is not None else None)
+
+
 def attention_reference_f64(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, first_pos: int, scale: float
                             ) -> torch.Tensor:
     """float64 softmax(q k^T * scale) v of one sequence, causal by absolute position (query i sits at first_pos + i).

@@ -130,6 +130,13 @@ constexpr int NORM_MAX_VEC = 4;  // hidden <= 256 * 8 * 4 = 8192
 // map and the same reduction tree for every instantiation: results do not depend on it.
 // MULT (ADD only): Granite's residual multiplier; a separate instantiation, so that the Llama stack runs the code it ran
 // before the multiplier existed
+//
+// Numerics (tests/test_norm_exact_gpu.py holds them bit for bit; tgis_gpu_utils.rmsnorm_restated restates them):
+// z = x, or with ADD z = bf16(x + r) (MULT: bf16(bf16(x * m) + r)), written back to the residual.  Thread tid owns the
+// 16-byte vectors i = tid + 256 j (j < NORM_MAX_VEC, i < hidden / 8) and adds the fp32 squares of their 8 elements to
+// ss = 0, j by j, element by element; a bf16 square is exact in fp32, so the contraction into an FFMA changes nothing.
+// block_sum: each warp's xor-butterfly at distances 16, 8, 4, 2, 1, then the 8 warp sums in lanes 0..7 (zeros in
+// 8..31) through the same butterfly.  rs = rsqrtf(tot / hidden + eps) with IEEE division, out = bf16(bf16(z * rs) * w).
 template <bool ADD, int NORM_MAX_VEC, bool MULT = false>
 __global__ void __launch_bounds__(NORM_THREADS)
 rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ residual,

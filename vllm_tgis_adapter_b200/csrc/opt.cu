@@ -73,6 +73,12 @@ opt_embed_kernel(const int32_t* __restrict__ tok, const int32_t* __restrict__ po
 //   y = bf16(acc + acc_bias)   (the projection's output in the model dtype)
 //   h = bf16(residual + y)     (residual add in the model dtype), written back to `residual`
 // then out = bf16((h - mean) * rstd * w + b) with fp32 statistics over the bf16 values of h.
+// Numerics (tests/test_norm_exact_gpu.py holds them bit for bit; tgis_gpu_utils.layernorm_restated restates them):
+// thread tid owns the 16-byte vectors i = tid + LN_THREADS j (j < LN_MAX_VEC, i < hidden / 8) and visits them j by j,
+// element by element.  Pass 1 adds z to s = 0; bsum: each warp's xor-butterfly at distances 16, 8, 4, 2, 1, then the
+// LN_THREADS / 32 warp sums in the low lanes (zeros above) through the same butterfly; mean = sum / hidden (IEEE
+// division).  Pass 2 likewise with q = fma(d, d, q), d = z - mean (the compiler contracts it: one rounding per step);
+// rstd = rsqrtf(sum / hidden + eps); out = bf16(fma(d * rstd, w, b)), the product d * rstd rounded, the rest contracted.
 template <bool ADD, int LN_THREADS, int LN_MAX_VEC>
 __global__ void __launch_bounds__(LN_THREADS)
 opt_layernorm_kernel(const float* __restrict__ acc, const __nv_bfloat16* __restrict__ acc_bias,
